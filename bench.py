@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — path-QP solves/s on B200 (contract in the task statement).
+"""bench.py — path-QP solves/s on H100.
 
 One "step" = one pass of the hot path (assemble + OSQP-style ADMM to the reference's
 eps = 2e-3 + solution write-back, i.e. one `BaseSolver::solve` per instance) over one batch
@@ -11,13 +11,14 @@ of synthetic instances. Default workload: BASELINE.json configs[2] — batch 819
   e2e        : same metric through the host-buffer C ABI call (pinned host buffers, H2D + D2H
                inside the timed region)
   roofline   : algorithmic bytes (SURVEY.md §8d: 104 n + 56 per cold solve) / kernel time vs the
-               measured HBM peak (MEASURED_PEAKS.json)
+               measured HBM peak (MEASURED_PEAKS.json) or the H100 SXM data-sheet figure
   cpu_baseline: the oracle port (OSQP-algorithm restatement) on the host cores, bounded sample
   config.fp64 / config.secondary : the same metric with the FP64 instantiation of the kernel (the
                reference's OSQP is FP64), and the other BASELINE configs (configs[0] one path through
                the C++ drop-in incl. handle creation, configs[1] shared map, configs[4] receding horizon)
 
 `--impl reference` times that CPU path alone (kind "port": OSQP itself is not available).
+`--dump-outputs DIR` writes what the timed path returned in its last step as DIR/<name>.npy.
 """
 import argparse
 import ctypes as C
@@ -26,6 +27,7 @@ import math
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -186,40 +188,13 @@ def algorithmic_bytes(n, warm=False):
     return (296 * n + 72) if warm else (104 * n + 56)
 
 
-def measured_traffic(n, instances, cold_only):
-    """DRAM bytes per launch from the ncu --set full capture committed in the same round
-    (profiles/r2/traffic_*.json, written by profiles/traffic_from_ncu.py), or None."""
-    name = "traffic_cold_n%d%s.json" % (n, "_coldonly" if cold_only else "")
-    try:
-        with open(os.path.join(ROOT, "profiles", "r2", name)) as f:
-            return float(json.load(f)["dram_bytes_per_instance"]) * instances
-    except Exception:
-        return None
-
-
-def measured_issue(n, cold_only):
-    """What actually bounds the kernel, from the same capture: warp instructions per launch and the share of cycles
-    in which a scheduler issued (one warp per scheduler: the kernel is latency / issue bound, not HBM bound)."""
-    name = "traffic_cold_n%d%s.json" % (n, "_coldonly" if cold_only else "")
-    try:
-        with open(os.path.join(ROOT, "profiles", "r2", name)) as f:
-            r = json.load(f)
-        if r.get("issue_active_pct") is None:
-            return None
-        return {"warp_instructions_per_launch": r["warp_instructions"], "issue_active_pct": r["issue_active_pct"],
-                "registers_per_thread": r.get("registers_per_thread"), "batch": r["batch"],
-                "source": "ncu --set full capture of this round (profiles/r2/%s)" % name}
-    except Exception:
-        return None
-
-
 def hbm_peak():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     try:
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "measured"
     except Exception:
-        return 6650.0, "fallback"
+        return 3350.0, "H100 SXM data sheet"
 
 
 class ClockSampler(threading.Thread):
@@ -449,8 +424,8 @@ def barrier(world):
 def bind_to_gpu_numa_node(local_rank):
     """One process per GPU: run this rank's host threads on the CPUs of the GPU's NUMA node, so that the pinned
     host buffers it allocates (local allocation policy) sit behind the memory controllers next to its PCIe root.
-    Eight ranks move 8 x 205 MB of host memory per 5.7 ms step end to end; from one socket's memory that stops at
-    ~170 GB/s (profiles/r2/scale_r2_builder.txt). Returns the node, or None when the topology is not exposed."""
+    Every rank moves ~205 MB of host memory per step end to end, and several ranks drawing on one socket's memory
+    contend for it. Returns the node, or None when the topology is not exposed."""
     try:
         import torch
         pr = torch.cuda.get_device_properties(local_rank)
@@ -471,13 +446,28 @@ def bind_to_gpu_numa_node(local_rank):
         return None
 
 
-def sv_uses_tmem(n, batch):
-    """The library's storage policy (DESIGN.md §4): tensor memory for n_max >= 64."""
-    return n >= 64
+DUMP_LIMIT_BYTES = 64_000_000
+
+
+def dump_outputs(path, arrays):
+    """Write the arrays a caller of the timed path received as <path>/<name>.npy (float64), at most
+    DUMP_LIMIT_BYTES in all: beyond that, a fixed seeded sample of instances (first axis), listed in
+    sample_index.npy."""
+    os.makedirs(path, exist_ok=True)
+    arrays = {k: np.asarray(v, dtype=np.float64) for k, v in arrays.items()}
+    batch = len(next(iter(arrays.values())))
+    per_instance = sum(a.nbytes for a in arrays.values()) / batch
+    if per_instance * batch > DUMP_LIMIT_BYTES:
+        keep = int(DUMP_LIMIT_BYTES // (per_instance + 8))
+        idx = np.sort(np.random.default_rng(0).choice(batch, keep, replace=False))
+        arrays = {k: a[idx] for k, a in arrays.items()}
+        arrays["sample_index"] = idx.astype(np.float64)
+    for k, a in arrays.items():
+        np.save(os.path.join(path, k + ".npy"), a)
 
 
 def measure_cold(args, hb, option_bits, steps, warmup, e2e_steps, local_rank, world, dev, gather=True, clocks=False,
-                 inflight=1):
+                 inflight=1, keep_outputs=False):
     """Cold solves of this rank's batch `hb`: device-resident value, end-to-end value, kernel time.
     inflight = 2: consecutive steps alternate between two handles on two streams, so the next batch's CTAs take
     over SMs as the previous batch's persistent CTAs run out of work (iteration counts are heavy-tailed: 10 % of a
@@ -489,8 +479,9 @@ def measure_cold(args, hb, option_bits, steps, warmup, e2e_steps, local_rank, wo
     K = max(1, int(inflight))
     svs = [solver.PathQpSolver(params, n_max=n, batch_max=B, device=local_rank) for _ in range(K)]
     sv = svs[0]
-    # inputs smaller than L2 (the shared-map config): evict them between timed steps
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev) if hb.knots.nbytes < (160 << 20) else None
+    # inputs that fit in L2 (the shared-map config): evict them between timed steps
+    l2 = torch.cuda.get_device_properties(dev).L2_cache_size
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev) if hb.knots.nbytes < 1.25 * l2 else None
     d_knots, d_inst, d_n = (torch.from_numpy(v).to(dev) for v in (hb.knots, hb.inst, hb.n))
     outs = []
     for _ in range(K):
@@ -565,6 +556,8 @@ def measure_cold(args, hb, option_bits, steps, warmup, e2e_steps, local_rank, wo
     total_ms = reduce_max(my_ms, dev, world)
     last = (steps - 1) % K
     status, iters = outs[last][2].cpu().numpy(), outs[last][3].cpu().numpy()
+    outputs = {"sol": outs[last][0].cpu().numpy(), "cost": outs[last][1].cpu().numpy(), "status": status,
+               "iters": iters} if keep_outputs else None
     for k in range(K):  # every handle solved the same batch: identical results
         assert np.array_equal(outs[k][2].cpu().numpy(), status) or steps <= k
     if pipes[last]:  # the gathered table holds every rank's records; this rank's block must equal its own results
@@ -628,7 +621,7 @@ def measure_cold(args, hb, option_bits, steps, warmup, e2e_steps, local_rank, wo
     return {"value": world * B * steps / (total_ms * 1e-3), "ms_per_step": total_ms / steps, "kernel_ms": kernel_ms, "inflight": K,
             "kernel_ms_per_rank": kms, "e2e_value": world * B * e2e_steps / e2e_s, "e2e_steps": e2e_steps,
             "h2d": h2d, "d2h": d2h, "launches": int(launches), "clocks": clk, "status": status, "iters": iters,
-            "info": info, "params": params, "flushed": flush is not None, "steps": steps}
+            "info": info, "params": params, "flushed": flush is not None, "steps": steps, "outputs": outputs, "l2": l2}
 
 
 def run_receding(args, rank, local_rank, world, dev):
@@ -702,6 +695,9 @@ def run_receding(args, rank, local_rank, world, dev):
     value = world * B * args.steps / (total_ms * 1e-3)
     status = d_status.cpu().numpy()
     iters = d_iters.cpu().numpy()
+    if getattr(args, "dump_outputs", None) and rank == 0:
+        dump_outputs(args.dump_outputs, {"sol": d_sol.cpu().numpy(), "cost": d_cost.cpu().numpy(), "status": status,
+                                         "iters": iters})
     kms = gather_scalars(kernel_ms, dev, world)
 
     # e2e: the same tick through the host-pointer call (pinned host buffers, H2D + D2H timed);
@@ -751,7 +747,7 @@ def run_receding(args, rank, local_rank, world, dev):
         "gpu_launches": int(launches),
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
                      "frac": achieved / peak, "traffic": None, "peak_source": peak_src,
-                     "kernel": "pqp_admm_kernel_tmem (warm)", "kernel_ms": kernel_ms,
+                     "kernel": "pqp_admm_kernel_persistent (warm)", "kernel_ms": kernel_ms,
                      "algorithmic_bytes_per_launch": bytes_per_launch},
     }
 
@@ -772,10 +768,10 @@ def dropin_single_path(n=120, plans=200):
     hb = lines.to_host_batch(bnd[None], np.array([nv], dtype=np.int32))
     nn = int(hb.n[0])
     ref = np.stack([lines.states[0][1], lines.states[0][2], lines.states[0][3]])
-    path = os.path.join(ROOT, "gpurun_out", "bench_dropin_instance.txt")
-    os.makedirs(os.path.dirname(path), exist_ok=True)
-    test_dropin._write_instance(path, hb.knots[0], hb.inst[0], nn, ref, 0.0, constraint_end_heading=0)
-    out = subprocess.run([exe, path, str(plans)], capture_output=True, text=True, check=True).stdout.strip().split("\n")
+    with tempfile.TemporaryDirectory() as tmp:
+        path = os.path.join(tmp, "instance.txt")
+        test_dropin._write_instance(path, hb.knots[0], hb.inst[0], nn, ref, 0.0, constraint_end_heading=0)
+        out = subprocess.run([exe, path, str(plans)], capture_output=True, text=True, check=True).stdout.strip().split("\n")
     tok = out[0].split()
     if tok[0] != "plans":
         return {"error": out[0]}
@@ -877,7 +873,7 @@ def secondary(args, rank, local_rank, world, dev, hb_primary):
                     "(reproduces the FP64 oracle's iterates to 1e-8, tests/test_gpu_parity.py)"}
     # configs[4] at this N
     a4 = argparse.Namespace(**vars(args))
-    a4.batch, a4.n, a4.steps, a4.warmup, a4.e2e_steps = 512, 240, 20, 3, 5
+    a4.batch, a4.n, a4.steps, a4.warmup, a4.e2e_steps, a4.dump_outputs = 512, 240, 20, 3, 5, None
     l4 = run_receding(a4, rank, local_rank, world, dev)
     sec["configs[4]"] = {"workload": l4["config"]["workload"], "value": l4["value"], "unit": UNIT, "n_gpus": world,
                          "ms_per_step": l4["ms_per_step"], "e2e": l4["e2e"]["value"], "kernel_ms": l4["roofline"]["kernel_ms"],
@@ -926,13 +922,17 @@ def main():
                     help="batches in flight in the device-resident loop: 2 = consecutive steps alternate between two handles "
                          "on two streams (hides the launch tail of the persistent kernel); 1 = one launch at a time")
     ap.add_argument("--option-bits", type=int, default=128,
-                    help="pqp_params.reserved: 2 FP64 iterates, 4 no FP64 escalation, 8 state in tensor memory, "
-                         "16 state in shared memory, 32 increment-form ADMM step, 64 textbook form, 128 cold-only "
+                    help="pqp_params.reserved: 2 FP64 iterates, 4 no FP64 escalation, 8 persistent launch, "
+                         "16 one CTA per instance, 32 increment-form ADMM step, 64 textbook form, 128 cold-only "
                          "handle (default for the cold workloads: nothing is ever re-solved, so no warm state is written)")
     ap.add_argument("--workload", default="cold", choices=["cold", "receding", "sharedmap"],
                     help="cold: BASELINE configs[2]/[3] (default); receding: configs[4], warm re-solves with a "
                          "50-iteration cap on a window that advances one knot per step; sharedmap: configs[1], "
                          "1024 paths x 120 knots through the shared obstacle map")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the timed path returned in its last step (solution, cost, "
+                         "status, iterations) as DIR/<name>.npy, float64, at most 64 MB (a seeded sample of instances "
+                         "beyond that)")
     args = ap.parse_args()
     if args.workload == "receding" and args.batch == 8192:
         args.batch = 512  # configs[4]: 4096 instances over 8 GPUs
@@ -976,7 +976,9 @@ def main():
     extras.pop("_lines", None)
     extras.pop("_dmap", None)
     r = measure_cold(args, hb, args.option_bits, args.steps, args.warmup, args.e2e_steps or args.steps, local_rank,
-                     world, dev, gather=True, clocks=True, inflight=args.inflight)
+                     world, dev, gather=True, clocks=True, inflight=args.inflight, keep_outputs=bool(args.dump_outputs))
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, r["outputs"])
     fp64, sec = (None, None) if args.no_secondary else secondary(args, rank, local_rank, world, dev, hb)
 
     if rank == 0:
@@ -994,7 +996,7 @@ def main():
                 **extras,
                 "n_knots": n, "batch_per_gpu": B, "global_batch": world * B, "parallelism": "dp%d" % world,
                 "eps_abs": params.eps_abs, "eps_rel": params.eps_rel, "max_iter": params.max_iter,
-                "l2_policy": ("inputs larger than L2 (%.0f MB per step vs 126 MB)" % (hb.knots.nbytes / 1e6))
+                "l2_policy": ("inputs larger than L2 (%.0f MB per step vs %.0f MB)" % (hb.knots.nbytes / 1e6, r["l2"] / 1e6))
                 if not r["flushed"] else "L2 flushed between timed steps (256 MB fill inside the timed region)",
                 "collective": ("all_gather of {cost,status,iters} (16 B/instance): one pack kernel + NCCL on a side "
                                "stream, overlapping the next step's solve; the timed region ends after the last gather")
@@ -1014,9 +1016,10 @@ def main():
                 "admm_step": ("increment form (dx solve, carried row values)"
                               if (args.option_bits & 32) or (not (args.option_bits & (64 | 2)) and n >= 64)
                               else "textbook form"),
-                "state_storage": ("tensor memory (tcgen05.ld/st), persistent CTAs; %d KB of shared memory per warp for the groups "
-                                  "that do not fit the warp's columns" % (info["smem_per_warp"] // 1024))
-                                 if sv_uses_tmem(n, B) else "shared memory",
+                "state_storage": "shared memory, %d KB per warp; %s" % (
+                    info["smem_per_warp"] // 1024,
+                    "persistent one-warp CTAs on a work counter" if (args.option_bits & 8) or (n >= 128 and not (args.option_bits & (16 | 2)))
+                    else "one CTA per instance"),
             },
             "clocks": r["clocks"],
             "e2e": {"value": r["e2e_value"], "unit": UNIT, "h2d_bytes_per_step": r["h2d"], "d2h_bytes_per_step": r["d2h"],
@@ -1025,11 +1028,10 @@ def main():
                            "results; %d handle(s), one host thread per handle" % r["inflight"]},
             "gpu_launches": r["launches"],
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": achieved / peak, "traffic": measured_traffic(n, B, cold_only), "peak_source": peak_src,
-                         "kernel": "pqp_admm_kernel_tmem", "kernel_ms": r["kernel_ms"],
+                         "frac": achieved / peak, "traffic": None, "peak_source": peak_src,
+                         "kernel": "pqp_admm_kernel_persistent", "kernel_ms": r["kernel_ms"],
                          "algorithmic_bytes_per_launch": bytes_per_launch,
-                         "issue": measured_issue(n, cold_only),
-                         "note": "per-iteration state is on-chip (tensor memory / shared memory); the path is "
+                         "note": "per-iteration state is on-chip (shared memory); the path is "
                                  "latency/issue bound, not HBM bound (see DESIGN.md)"},
         }
         if fp64 is not None:

@@ -1,5 +1,5 @@
 /*
- * pqp.h — C ABI of the batched path-QP solver (B200 / sm_100a).
+ * pqp.h — C ABI of the batched path-QP solver (H100 / sm_90a).
  *
  * This is the drop-in boundary for the solve path of LiJiangnanBit/path_optimizer_2:
  *
@@ -115,9 +115,10 @@ typedef struct pqp_params {
     int32_t reserved;               /* option bits, default 0: 1 = (unused),
                                        2 = iterate in FP64 (whole kernel in double precision),
                                        4 = do not re-solve suspected-infeasible instances in FP64,
-                                       8 = FP32 state in tensor memory (persistent CTAs, tcgen05.ld/st): the
-                                           default for n_max >= 64,
-                                       16 = FP32 state in shared memory even where tensor memory is the default,
+                                       8 = persistent FP32 launch (one-warp CTAs that take instances from a
+                                           work counter; host calls stream their copies under one launch): the
+                                           default for n_max >= 128,
+                                       16 = one CTA per instance even where the persistent launch is the default,
                                        32 = ADMM step in increment form (dx solve, carried row values): the FP32
                                             kernel then follows an FP64 OSQP iteration count for count; the
                                             default for n_max >= 64 (bit 32 forces it below as well),
@@ -253,9 +254,8 @@ enum {
 int pqp_last_stage_ms(pqp_handle *h, float *ms);
 
 /* Device-side properties, for occupancy reporting: SM count, resident warps per SM of
- * the solve kernel, dynamic shared memory per warp in bytes (the whole per-QP state under the
- * shared-memory policy; only the groups that do not fit the warp's tensor-memory columns - 4 KB at
- * 64 <= n_max <= 127, 8 KB at 128..255, 80 KB at 256..511 - when the state lives in tensor memory). */
+ * the solve kernel, dynamic shared memory per warp in bytes (the whole per-QP state: 72 x 32 x C
+ * values for C stages per lane, plus the input-staging barrier). */
 int pqp_kernel_info(pqp_handle *h, int32_t *sm_count, int32_t *warps_per_sm,
                     int32_t *smem_per_warp);
 

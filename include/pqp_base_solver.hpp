@@ -20,7 +20,7 @@
 //
 // (see INTEGRATION.md). The host side only packs plain arrays; assembly of P/A/l/u, the OSQP
 // iteration and the warm state live on the GPU behind include/pqp.h. There is no CPU path:
-// without a B200 the constructor's handle creation fails and both calls return false.
+// without an H100 the constructor's handle creation fails and both calls return false.
 // Handles (device buffers, streams) come from a process-wide pool, so constructing a solver per
 // plan - as the reference's caller does at 30 Hz - costs no allocation after the first plan.
 #ifndef PQP_BASE_SOLVER_HPP_
@@ -53,7 +53,7 @@ inline double constrainAngle(double angle) {  // include/tools/tools.hpp:24-35
     return angle;
 }
 
-// Largest problem the CUDA library holds (512 stages on one warp pair of tensor-memory lanes). The
+// Largest problem the CUDA library holds (512 stages: 16 per lane of one warp). The
 // reference itself has no cap (base_solver.cpp:15-39): at its 0.15-0.3 m knot spacing 511 knots are
 // 77-153 m of path; beyond that the drop-in reports failure with an explicit error text.
 constexpr size_t kMaxKnots = 511;

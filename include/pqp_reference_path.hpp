@@ -11,8 +11,8 @@
 // truncation of reference_states_ at the first blocked state. Templates over the reference's own
 // State / VehicleStateBound types, so this header neither needs nor copies the reference's headers;
 // the two member functions of ReferencePathImpl become one-line forwards (INTEGRATION.md §4).
-// Nothing throws; errors come back as `false` with lastError(). There is no CPU path: without a
-// B200 the constructor's handle creation fails and both calls return false.
+// Nothing throws; errors come back as `false` with lastError(). There is no CPU path: without an
+// H100 the constructor's handle creation fails and both calls return false.
 #ifndef PQP_REFERENCE_PATH_HPP_
 #define PQP_REFERENCE_PATH_HPP_
 

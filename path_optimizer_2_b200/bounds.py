@@ -4,7 +4,7 @@
 (reference_path_impl.cpp:177-230): one handle owns the device copy of the map's distance layer;
 `compute()` takes the splines and reference states of a batch of paths and returns the
 front / rear / centre clearance bounds per state plus the index the reference would cut each
-path at. There is no CPU path: without the CUDA library or a B200, construction raises.
+path at. There is no CPU path: without the CUDA library or an H100, construction raises.
 """
 import ctypes as C
 

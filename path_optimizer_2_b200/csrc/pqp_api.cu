@@ -1,4 +1,4 @@
-// pqp_api.cu — C ABI (include/pqp.h) of the batched path-QP solver for B200 (sm_100a).
+// pqp_api.cu — C ABI (include/pqp.h) of the batched path-QP solver for H100 (sm_90a).
 //
 // Host side: handle with device buffers + per-instance warm state, H2D/D2H staging for the
 // host-pointer entry points, launches. Device side: the kernel entry (one warp = one CTA =
@@ -108,327 +108,27 @@ __global__ void __launch_bounds__(32) pqp_admm_kernel_gmem(const __grid_constant
     }
 }
 
-// ------------------------------------------------------------------ device: tensor-memory storage policy
-// The solver keeps a QP's per-stage state as [group][stage][lane] float4. Tensor memory is 128
-// lanes x 512 32-bit columns per SM and a warp reaches the 32 lanes of its own sub-partition
-// with tcgen05.ld/st (32x32b shapes: each thread gets N consecutive columns of "its" lane), so
-// the layout maps 1:1 with column = (k * kGroups + slot(g)) * 4 + component. A CTA of four
-// warps (four QPs) owns all 512 columns; at C = 8 sixteen of the eighteen groups fit and the two
-// least-frequently read ones (clearance weights / proximal weights) stay in shared memory.
-// Measured on B200 (profiles/r1/tmem_probe_result.txt): dependent tcgen05.ld latency <= LDS.128,
-// streaming bandwidth ~6x shared memory.
-__device__ __forceinline__ void tmem_alloc(uint32_t *dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols));
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ float tmem_ld1(uint32_t a) {
-    uint32_t r;
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(r) : "r"(a) : "memory");
-    tmem_wait_ld();
-    return __uint_as_float(r);
-}
-__device__ __forceinline__ void tmem_st1(uint32_t a, float v) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x1.b32 [%0], {%1};" ::"r"(a), "r"(__float_as_uint(v)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld4_nowait(uint32_t a, float (&o)[4]) {
-    uint32_t r0, r1, r2, r3;
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(a) : "memory");
-    o[0] = __uint_as_float(r0); o[1] = __uint_as_float(r1); o[2] = __uint_as_float(r2); o[3] = __uint_as_float(r3);
-}
-__device__ __forceinline__ void tmem_ldx8_nowait(uint32_t a, float *o) {
-    uint32_t r[8];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]) : "r"(a) : "memory");
-#pragma unroll
-    for (int i = 0; i < 8; ++i) o[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ldx16_nowait(uint32_t a, float *o) {
-    uint32_t r[16];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]) : "r"(a) : "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) o[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ldx32_nowait(uint32_t a, float *o) {
-    uint32_t r[32];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31]) : "r"(a) : "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) o[i] = __uint_as_float(r[i]);
-}
-// G consecutive float4 groups (G = 1, 2, 4, 8) starting at column address a, in ONE tcgen05.ld
-template <int G> __device__ __forceinline__ void tmem_ldg_nowait(uint32_t a, float *o) {
-    if (G == 8) tmem_ldx32_nowait(a, o);
-    else if (G == 4) tmem_ldx16_nowait(a, o);
-    else if (G == 2) tmem_ldx8_nowait(a, o);
-    else {
-        float t[4];
-        tmem_ld4_nowait(a, t);
-        o[0] = t[0]; o[1] = t[1]; o[2] = t[2]; o[3] = t[3];
-    }
-}
-__device__ __forceinline__ void tmem_st4(uint32_t a, const float4 &v) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(__float_as_uint(v.x)),
-                 "r"(__float_as_uint(v.y)), "r"(__float_as_uint(v.z)), "r"(__float_as_uint(v.w))
-                 : "memory");
-}
-
-// where the cyclic-reduction levels are unrolled (see cr_forward_level); overridable for A/B builds
-#ifndef PQP_UNROLL_CR_COND
-#define PQP_UNROLL_CR_COND true
-#endif
-template <int C, int COLS = 512>
-struct TmemStore {
-    typedef float4 Vec4;
-    static constexpr int kAll = pqp::NFIELD / 4;                       // 18 groups
-    static constexpr int kFit = COLS / (4 * C);                        // groups that fit in this warp's columns
-    static constexpr int kGroups = kFit < kAll ? kFit : kAll;          // groups kept in TMEM
-    static constexpr bool kUnrollCr = PQP_UNROLL_CR_COND;              // see cr_forward_level
-    static constexpr int kSpill = kAll - kGroups;                      // 2 at C = 8 (512 columns) and at C = 4 with 256 columns, 10 at C = 16, else 0
-    // Which groups leave tensor memory first when the warp's columns do not hold all 18.
-    // C <= 8 (two groups leave): the clearance / proximal weights GR5, GS6 (least frequently read), then the other
-    // read-only groups (4, 3, 2, 1, 0), then the factor from its end (17 .. 12), the read-write groups last.
-    // C = 16 (ten groups leave): the factor first (17 .. 12), then GR5, GS6, then 4, 3, .. (measured +2.6 % at
-    // n = 400). Sending the factor to shared memory at C = 8 as well - tensor memory is read at 64 B per cycle,
-    // shared memory at 128 B, and the sweeps' factor reads are half of all loads - measured -1.7 %
-    // (profiles/r2/README.md): four warps share the one shared-memory port.
-    static constexpr bool kFactorFirst = C >= 16;
-    uint32_t tb;  // TMEM address of this warp's lane block (lane base in bits 31:16)
-    uint32_t cur;  // stage cursor: tb + k * (columns per stage) of the stage a hot loop is at (see seek)
-    float *sm;    // spill area (shared memory) of this warp: [spill slot][k][lane] float4
-    int lane;
-    __device__ TmemStore(uint32_t t, float *s, int l) : tb(t), cur(t), sm(s), lane(l) {}
-    __host__ __device__ static constexpr int spill_rank(int g) {
-        return kFactorFirst
-                   ? (g >= pqp::GF0 ? 17 - g : g == pqp::GR5 ? 6 : g == pqp::GS6 ? 7 : g <= 4 ? 8 + (4 - g) : 13 + (11 - g))
-                   : (g == pqp::GR5 ? 0 : g == pqp::GS6 ? 1 : g <= 4 ? 6 - g : g >= pqp::GF0 ? 7 + (17 - g) : 13 + (11 - g));
-    }
-    __host__ __device__ static constexpr bool spilled(int g) { return spill_rank(g) < kSpill; }
-    // number of spilled groups with an index below g, in closed form (no loops: g reaches these helpers as a
-    // function argument and must fold to a constant after inlining - a loop here grew the kernel by 40 %)
-    __host__ __device__ static constexpr int imax(int a, int b) { return a > b ? a : b; }
-    __host__ __device__ static constexpr int imin(int a, int b) { return a < b ? a : b; }
-    __host__ __device__ static constexpr int spilled_below(int g) {
-        return kFactorFirst
-                   ? ((kSpill > 6 && g > pqp::GR5) ? 1 : 0) + ((kSpill > 7 && g > pqp::GS6) ? 1 : 0) +
-                         imax(0, imin(g, 5) - imax(0, 13 - kSpill)) +    // read-only groups 4, 3, .. leave from the top
-                         imax(0, imin(g, 12) - imax(7, 25 - kSpill)) +   // read-write groups 11 .. 7 (last to leave)
-                         imax(0, imin(g, 18) - imax(12, 18 - kSpill))    // factor groups 17 .. 12 (first to leave)
-                   : ((kSpill > 0 && g > pqp::GR5) ? 1 : 0) + ((kSpill > 1 && g > pqp::GS6) ? 1 : 0) +
-                         imax(0, imin(g, 5) - imax(0, 7 - kSpill)) +     // read-only groups 4, 3, .. leave from the top
-                         imax(0, imin(g, 12) - imax(7, 25 - kSpill)) +   // read-write groups 11 .. 7 (last to leave)
-                         imax(0, imin(g, 18) - imax(12, 25 - kSpill));   // factor groups 17 .. 12
-    }
-    __host__ __device__ static constexpr int slot(int g) { return g - spilled_below(g); }
-    __host__ __device__ static constexpr int spslot(int g) { return spilled_below(g); }
-    __device__ uint32_t col(int g, int k) const { return tb + (uint32_t)((k * kGroups + slot(g)) * 4); }
-    __device__ float4 *sp(int g, int k) const { return reinterpret_cast<float4 *>(sm) + ((spslot(g) * C + k) * 32 + lane); }
-    __device__ float ld(int f, int k) const {
-        const int g = f >> 2;
-        if (spilled(g)) return reinterpret_cast<const float *>(sp(g, k))[f & 3];
-        return tmem_ld1(col(g, k) + (f & 3));
-    }
-    __device__ void st(int f, int k, float v) {
-        const int g = f >> 2;
-        if (spilled(g)) { reinterpret_cast<float *>(sp(g, k))[f & 3] = v; return; }
-        tmem_st1(col(g, k) + (f & 3), v);
-        tmem_wait_st();
-    }
-    // Groups g0 .. g0+N-1 of one stage: groups kept in tensor memory sit in consecutive columns (slot(g) counts
-    // the unspilled groups below g), so a run of 2 / 4 / 8 of them is ONE tcgen05.ld.x8 / x16 / x32 instead of one
-    // .x4 per group. run_at(g, end): length of the longest such run starting at g.
-    __host__ __device__ static constexpr int run_at(int g, int end) {
-        int n = 0;
-        while (g + n < end && !spilled(g + n)) ++n;
-        return n >= 8 ? 8 : n >= 4 ? 4 : n >= 2 ? 2 : n;
-    }
-    template <int G0, int N, int I> struct Loader {
-        static constexpr int kRun = I < N ? (spilled(G0 + I) ? 0 : run_at(G0 + I, G0 + N)) : 0;
-        static constexpr int kStep = kRun > 0 ? kRun : 1;
-        // base: column address of the stage block; k: stage index for the spilled groups
-        __device__ static void go(const TmemStore &st, uint32_t base, int k, float *out) {
-            if (I >= N) return;
-            if (kRun == 0) {
-                const float4 v = *st.sp(G0 + I, k);
-                out[4 * I] = v.x; out[4 * I + 1] = v.y; out[4 * I + 2] = v.z; out[4 * I + 3] = v.w;
-            } else {
-                tmem_ldg_nowait<(kRun > 0 ? kRun : 1)>(base + (uint32_t)(slot(G0 + I) * 4), out + 4 * I);
-            }
-            Loader<G0, N, (I + kStep < N ? I + kStep : N)>::go(st, base, k, out);
-        }
-    };
-    __device__ float4 ld4(int g, int k) const {
-        if (spilled(g)) return *sp(g, k);
-        float o[4];
-        tmem_ld4_nowait(col(g, k), o);
-        tmem_wait_ld();
-        return make_float4(o[0], o[1], o[2], o[3]);
-    }
-    __device__ void st4(int g, int k, const float4 &v) {
-        if (spilled(g)) { *sp(g, k) = v; return; }
-        tmem_st4(col(g, k), v);
-    }
-    // split form: issue the loads of N consecutive groups, wait later (wait_ld) together with other batches
-    template <int N> __device__ void ld4n_nowait(int g0, int k, float (&out)[4 * N]) const {
-#pragma unroll
-        for (int g = 0; g < N; ++g) {
-            float o[4];
-            if (spilled(g0 + g)) {
-                const float4 v = *sp(g0 + g, k);
-                o[0] = v.x; o[1] = v.y; o[2] = v.z; o[3] = v.w;
-            } else {
-                tmem_ld4_nowait(col(g0 + g, k), o);
-            }
-            out[4 * g] = o[0]; out[4 * g + 1] = o[1]; out[4 * g + 2] = o[2]; out[4 * g + 3] = o[3];
-        }
-    }
-    __device__ void wait_ld() const { tmem_wait_ld(); }
-    // compile-time group range: runs of consecutive tensor-memory groups become one wide load (see Loader)
-    template <int G0, int N> __device__ void ld_run_nowait(int k, float (&out)[4 * N]) const {
-        Loader<G0, N, 0>::go(*this, tb + (uint32_t)(k * kGroups * 4), k, out);
-    }
-    template <int G0, int N> __device__ void ld_run_nowait_cur(int k, float (&out)[4 * N]) const {
-        Loader<G0, N, 0>::go(*this, cur, k, out);
-    }
-    template <int G0, int N> __device__ void ld_run_nowait_ahead(int k, float (&out)[4 * N]) const {
-        Loader<G0, N, 0>::go(*this, ahead(), k < C - 1 ? k + 1 : k, out);
-    }
-    // Stage cursor. tcgen05.ld/st take their address from a UNIFORM register; an address computed from a loop
-    // counter that ptxas keeps in a vector register costs one R2UR per access (5.7 % of the kernel's executed
-    // instructions before this, profiles/r2/README.md). seek(k) produces the stage's column base in a uniform
-    // register once per stage; the `_cur` accessors address "the cursor's stage" (the caller passes the same
-    // stage as k, used by the spilled groups).
-    static constexpr uint32_t kStride = (uint32_t)(kGroups * 4);
-    __device__ void seek(int k) {
-        // (redux.sync delivers its result in a uniform register; a loop-carried cursor would be moved to a vector
-        // register by ptxas and converted back at every access)
-        cur = C == 1 ? tb : __reduce_or_sync(0xffffffffu, tb + (uint32_t)k * kStride);
-    }
-    __device__ uint32_t ccol(int g) const { return cur + (uint32_t)(slot(g) * 4); }
-    __device__ void st4_cur(int g, int k, const float4 &v) {
-        if (spilled(g)) { *sp(g, k) = v; return; }
-        tmem_st4(ccol(g), v);
-    }
-    template <int N> __device__ void ld4n_nowait_cur(int g0, int k, float (&out)[4 * N]) const {
-#pragma unroll
-        for (int g = 0; g < N; ++g) {
-            float o[4];
-            if (spilled(g0 + g)) {
-                const float4 v = *sp(g0 + g, k);
-                o[0] = v.x; o[1] = v.y; o[2] = v.z; o[3] = v.w;
-            } else {
-                tmem_ld4_nowait(ccol(g0 + g), o);
-            }
-            out[4 * g] = o[0]; out[4 * g + 1] = o[1]; out[4 * g + 2] = o[2]; out[4 * g + 3] = o[3];
-        }
-    }
-    // the same for the stage AFTER the cursor's (prefetch; the cursor's own stage again when that is the last one)
-    __device__ uint32_t ahead() const {
-        const uint32_t last = tb + (uint32_t)((C - 1) * kGroups * 4);
-        return (cur == last) ? cur : cur + kStride;
-    }
-    template <int N> __device__ void ld4n_nowait_ahead(int g0, int k, float (&out)[4 * N]) const {
-        const uint32_t a = ahead();
-        const int ka = k < C - 1 ? k + 1 : k;
-#pragma unroll
-        for (int g = 0; g < N; ++g) {
-            float o[4];
-            if (spilled(g0 + g)) {
-                const float4 v = *sp(g0 + g, ka);
-                o[0] = v.x; o[1] = v.y; o[2] = v.z; o[3] = v.w;
-            } else {
-                tmem_ld4_nowait(a + (uint32_t)(slot(g0 + g) * 4), o);
-            }
-            out[4 * g] = o[0]; out[4 * g + 1] = o[1]; out[4 * g + 2] = o[2]; out[4 * g + 3] = o[3];
-        }
-    }
-    // group g two stages after the cursor's (clamped to the last stage)
-    __device__ void ld4_nowait_ahead_next(int g, int k, float (&out)[4]) const {
-        if (spilled(g)) {
-            const float4 v = *sp(g, k < C - 2 ? k + 2 : C - 1);
-            out[0] = v.x; out[1] = v.y; out[2] = v.z; out[3] = v.w;
-        } else {
-            const uint32_t last = tb + (uint32_t)((C - 1) * kGroups * 4);
-            const uint32_t a1 = ahead();
-            const uint32_t a2 = (a1 == last) ? a1 : a1 + kStride;
-            tmem_ld4_nowait(a2 + (uint32_t)(slot(g) * 4), out);
-        }
-    }
-    // group g of the stage AFTER the cursor's (of the cursor's own stage when that is the last one)
-    __device__ void ld4_nowait_next(int g, int k, float (&out)[4]) const {
-        if (spilled(g)) {
-            const float4 v = *sp(g, k < C - 1 ? k + 1 : k);
-            out[0] = v.x; out[1] = v.y; out[2] = v.z; out[3] = v.w;
-        } else {
-            const uint32_t last = tb + (uint32_t)((C - 1) * kGroups * 4);
-            const uint32_t a = (cur == last) ? cur : cur + kStride;
-            tmem_ld4_nowait(a + (uint32_t)(slot(g) * 4), out);
-        }
-    }
-    template <int N> __device__ void ld4n(int g0, int k, float (&out)[4 * N]) const {
-#pragma unroll
-        for (int g = 0; g < N; ++g) {
-            float o[4];
-            if (spilled(g0 + g)) {
-                const float4 v = *sp(g0 + g, k);
-                o[0] = v.x; o[1] = v.y; o[2] = v.z; o[3] = v.w;
-            } else {
-                tmem_ld4_nowait(col(g0 + g, k), o);
-            }
-            out[4 * g] = o[0]; out[4 * g + 1] = o[1]; out[4 * g + 2] = o[2]; out[4 * g + 3] = o[3];
-        }
-        tmem_wait_ld();
-    }
-    __device__ void fence() { tmem_wait_st(); }
-};
-
-
-// compile-time check of the closed-form spill map against its definition (rank order) for every store in use
-template <class Store> constexpr bool spill_map_consistent() {
-    int seen = 0;
-    for (int g = 0; g <= Store::kAll; ++g) {
-        if (Store::spilled_below(g) != seen) return false;
-        if (g < Store::kAll && Store::spilled(g)) ++seen;
-    }
-    if (seen != Store::kSpill) return false;
-    for (int a = 0; a < Store::kAll; ++a)  // the ranks are a permutation of 0 .. 17
-        for (int b = a + 1; b < Store::kAll; ++b)
-            if (Store::spill_rank(a) == Store::spill_rank(b)) return false;
-    return true;
-}
-static_assert(spill_map_consistent<TmemStore<1, 512>>() && spill_map_consistent<TmemStore<2, 512>>() &&
-                  spill_map_consistent<TmemStore<4, 256>>() && spill_map_consistent<TmemStore<8, 512>>() &&
-                  spill_map_consistent<TmemStore<16, 512>>(),
-              "TmemStore::spilled_below does not match spill_rank");
-
-// Tensor-memory persistent kernel (FP32): one CTA per SM with WT warps (4, or 8 when two warps
-// can share a TMEM sub-partition: 256 columns each); every warp solves one QP at a time and takes
-// the next unsolved instance from a global work counter (iteration counts vary 3x between
-// instances; a static assignment would idle).
-// A hybrid variant that added shared-memory-backed warps to the same CTA was measured slower
-// (instruction-fetch bound either as two instantiations or as one with run-time backend
-// selection): profiles/r1/README.md.
-template <int C, int WT, bool Incr>
-__global__ void __launch_bounds__(32 * WT, 1) pqp_admm_kernel_tmem(const __grid_constant__ pqp::KernelArgs ka) {
+// Persistent kernel (FP32): as many one-warp CTAs as fit on the SMs (shared memory bounds it: the
+// whole per-QP state of SmemStore, 37 KB at C = 4, 74 KB at C = 8, 147 KB at C = 16); every warp
+// solves one QP at a time and takes the next unsolved instance from a global work counter
+// (iteration counts vary 3x between instances; a static assignment would idle). Each instance's
+// knot block is staged into the warp's factor region by one TMA bulk copy, as in pqp_admm_kernel;
+// the mbarrier is initialised once and its phase advances by one per instance. Scratch slots
+// (Ruiz factors, delta_y) belong to the CTA, not to the instance.
+template <int C, bool Incr>
+__global__ void __launch_bounds__(32) pqp_admm_kernel_persistent(const __grid_constant__ pqp::KernelArgs ka) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    __shared__ uint32_t tbase_s;
-    constexpr int kShare = WT > 4 ? (WT + 3) / 4 : 1;  // warps per tensor-memory sub-partition
-    constexpr int kCols = 512 / kShare;
-    typedef TmemStore<C, kCols> Store;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    constexpr uint32_t need = (uint32_t)(Store::kGroups * 4 * C) * kShare;
-    constexpr uint32_t ncols = need <= 32 ? 32 : need <= 64 ? 64 : need <= 128 ? 128 : need <= 256 ? 256 : 512;
-    constexpr size_t kSpillFloats = (size_t)(Store::kSpill > 0 ? Store::kSpill : 0) * C * 32 * 4;
-    if (warp == 0) tmem_alloc(&tbase_s, ncols);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    // lanes of sub-partition (warp & 3); the second warp of a sub-partition takes the upper columns
-    const uint32_t tb_v = tbase_s + ((uint32_t)(32 * (warp & 3)) << 16) + (uint32_t)((warp >> 2) * Store::kGroups * 4 * C);
-    const uint32_t tb = __reduce_or_sync(0xffffffffu, tb_v);
-    float *spill = reinterpret_cast<float *>(smem_raw) + (size_t)warp * kSpillFloats;
+    float *smem = reinterpret_cast<float *>(smem_raw);
+    const int lane = threadIdx.x;
+    uint64_t *bar = reinterpret_cast<uint64_t *>(smem + pqp::NFIELD * C * 32);
+    double *stage = reinterpret_cast<double *>(smem + pqp::FDI * C * 32);
+    const uint32_t bytes = (uint32_t)(PQP_NFIELDS * ka.n_max * sizeof(double));
+    if (ka.use_tma && lane == 0) {
+        mbar_init(bar, 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncwarp();
+    uint32_t phase = 0;
     for (;;) {
         int qp = 0;
         if (lane == 0) qp = atomicAdd(ka.work_counter, 1);
@@ -459,10 +159,23 @@ __global__ void __launch_bounds__(32 * WT, 1) pqp_admm_kernel_tmem(const __grid_
             }
         }
         const double *src = ka.knots + (size_t)qp * PQP_NFIELDS * ka.n_max;
-        pqp::QpWarp<C, float, Store, Incr> w(ka, Store(tb, spill, lane), lane, qp);
-        w.run(src, ka.n_max, (size_t)(blockIdx.x * WT + warp));
-        if (ka.done) {
+        if (ka.use_tma) {
+            // the previous instance wrote the staging region through the generic proxy; order those writes
+            // before the bulk copy (async proxy) overwrites it
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
             __syncwarp();
+            if (lane == 0) {
+                mbar_expect_tx(bar, bytes);
+                tma_load_1d(stage, src, bytes, bar);
+            }
+            mbar_wait(bar, phase);
+            phase ^= 1u;
+            src = stage;
+        }
+        pqp::QpWarp<C, float, pqp::SmemStore<C, float>, Incr> w(ka, pqp::SmemStore<C, float>(smem, lane), lane, qp);
+        w.run(src, ka.n_max, (size_t)blockIdx.x);
+        __syncwarp();
+        if (ka.done) {
             if (lane == 0) {
                 __threadfence();  // this instance's outputs before the count
                 const int len = ka.chunk_lo[chunk + 1] - ka.chunk_lo[chunk];
@@ -473,9 +186,6 @@ __global__ void __launch_bounds__(32 * WT, 1) pqp_admm_kernel_tmem(const __grid_
             }
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tbase_s, ncols);
 }
 
 // BaseSolver::getOptimizedPath (base_solver.cpp:263-288) in FP64, one thread per knot.
@@ -590,7 +300,7 @@ struct pqp_handle {
     static const int kCounters = 64;
     int *d_counters = nullptr;
     unsigned counter_next = 0;
-    bool use_tmem = false;         // params.reserved bit 3: state in tensor memory (FP32 kernel)
+    bool persistent = false;       // params.reserved bit 3: persistent launch with a work counter (FP32 kernel)
     bool incr = false;             // ADMM step in increment form (FP32 kernels)
     bool fp64 = false;             // params.reserved bit 1: iterate in FP64
     bool escalate = true;          // params.reserved bit 2 clears it
@@ -685,62 +395,43 @@ cudaError_t prepare_chunk(int chunk, size_t smem, int *bps, bool incr = false) {
     }
 }
 
-// tensor-memory persistent variant: one CTA per SM (the dynamic shared-memory request is padded
-// so that a second CTA cannot be resident and spin on tcgen05.alloc)
-// Warps (= QPs) per CTA: 8 at C = 4 (two warps share a sub-partition, 256 columns each), 4 at
-// C <= 8, 2 at C = 16 (n <= 511: 8 groups in the warp's 512 columns + 10 groups = 80 KB of shared
-// memory per warp; a shared-memory-only layout would hold one QP per SM).
-template <int C> struct TmemCfg {
-    static constexpr int WT = (C == 4) ? 8 : (C == 16 ? 2 : 4);
-    typedef TmemStore<C, (WT > 4 ? 512 / (WT / 4) : 512)> Store;
-    static constexpr size_t kSpillBytes = (size_t)WT * Store::kSpill * C * 32 * 4 * sizeof(float);
-    // at least 120 KB so that a second CTA cannot become resident
-    static constexpr size_t kSmem = kSpillBytes > 120 * 1024 ? kSpillBytes : 120 * 1024;
-};
+// persistent variant: min(batch, resident) one-warp CTAs, resident = SMs x CTAs per SM at this shared-memory size
 template <int C, bool Incr>
-cudaError_t launch_tmem(const pqp::KernelArgs &ka, cudaStream_t s, int sm_count) {
-    constexpr int W = TmemCfg<C>::WT;
-    int ctas = (ka.batch + W - 1) / W;
-    if (ctas > sm_count) ctas = sm_count;
-    pqp_admm_kernel_tmem<C, W, Incr><<<ctas, 32 * W, TmemCfg<C>::kSmem, s>>>(ka);
+cudaError_t launch_persistent(const pqp::KernelArgs &ka, size_t smem, cudaStream_t s, int resident) {
+    const int ctas = ka.batch < resident ? ka.batch : resident;
+    pqp_admm_kernel_persistent<C, Incr><<<ctas, 32, smem, s>>>(ka);
     return cudaGetLastError();
 }
 template <int C>
-cudaError_t launch_tmem_form(const pqp::KernelArgs &ka, cudaStream_t s, int sm_count, bool incr) {
-    return incr ? launch_tmem<C, true>(ka, s, sm_count) : launch_tmem<C, false>(ka, s, sm_count);
+cudaError_t launch_persistent_form(const pqp::KernelArgs &ka, size_t smem, cudaStream_t s, int resident, bool incr) {
+    return incr ? launch_persistent<C, true>(ka, smem, s, resident) : launch_persistent<C, false>(ka, smem, s, resident);
 }
-cudaError_t launch_tmem_chunk(int chunk, const pqp::KernelArgs &ka, cudaStream_t s, int sm_count, bool incr) {
+cudaError_t launch_persistent_chunk(int chunk, const pqp::KernelArgs &ka, size_t smem, cudaStream_t s, int resident, bool incr) {
     switch (chunk) {
-        case 1: return launch_tmem_form<1>(ka, s, sm_count, incr);
-        case 2: return launch_tmem_form<2>(ka, s, sm_count, incr);
-        case 4: return launch_tmem_form<4>(ka, s, sm_count, incr);
-        case 8: return launch_tmem_form<8>(ka, s, sm_count, incr);
-        default: return launch_tmem_form<16>(ka, s, sm_count, incr);
+        case 1: return launch_persistent_form<1>(ka, smem, s, resident, incr);
+        case 2: return launch_persistent_form<2>(ka, smem, s, resident, incr);
+        case 4: return launch_persistent_form<4>(ka, smem, s, resident, incr);
+        case 8: return launch_persistent_form<8>(ka, smem, s, resident, incr);
+        default: return launch_persistent_form<16>(ka, smem, s, resident, incr);
     }
+}
+template <int C, bool Incr>
+cudaError_t prepare_persistent(size_t smem, int *blocks_per_sm) {
+    cudaError_t e = cudaFuncSetAttribute(pqp_admm_kernel_persistent<C, Incr>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    return cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks_per_sm, pqp_admm_kernel_persistent<C, Incr>, 32, smem);
 }
 template <int C>
-cudaError_t prepare_tmem() {
-    cudaError_t e = cudaFuncSetAttribute(pqp_admm_kernel_tmem<C, TmemCfg<C>::WT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TmemCfg<C>::kSmem);
-    if (e != cudaSuccess) return e;
-    return cudaFuncSetAttribute(pqp_admm_kernel_tmem<C, TmemCfg<C>::WT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TmemCfg<C>::kSmem);
+cudaError_t prepare_persistent_form(size_t smem, int *bps, bool incr) {
+    return incr ? prepare_persistent<C, true>(smem, bps) : prepare_persistent<C, false>(smem, bps);
 }
-cudaError_t prepare_tmem_chunk(int chunk) {
+cudaError_t prepare_persistent_chunk(int chunk, size_t smem, int *bps, bool incr) {
     switch (chunk) {
-        case 1: return prepare_tmem<1>();
-        case 2: return prepare_tmem<2>();
-        case 4: return prepare_tmem<4>();
-        case 8: return prepare_tmem<8>();
-        default: return prepare_tmem<16>();
-    }
-}
-int tmem_warps(int chunk) { return chunk == 4 ? 8 : (chunk == 16 ? 2 : 4); }
-size_t tmem_spill_bytes(int chunk) {  // per warp
-    switch (chunk) {
-        case 1: return TmemCfg<1>::kSpillBytes / TmemCfg<1>::WT;
-        case 2: return TmemCfg<2>::kSpillBytes / TmemCfg<2>::WT;
-        case 4: return TmemCfg<4>::kSpillBytes / TmemCfg<4>::WT;
-        case 8: return TmemCfg<8>::kSpillBytes / TmemCfg<8>::WT;
-        default: return TmemCfg<16>::kSpillBytes / TmemCfg<16>::WT;
+        case 1: return prepare_persistent_form<1>(smem, bps, incr);
+        case 2: return prepare_persistent_form<2>(smem, bps, incr);
+        case 4: return prepare_persistent_form<4>(smem, bps, incr);
+        case 8: return prepare_persistent_form<8>(smem, bps, incr);
+        default: return prepare_persistent_form<16>(smem, bps, incr);
     }
 }
 
@@ -815,12 +506,12 @@ int run_device(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *out, 
         } else {
             PQP_CUDA(h, launch_chunk<double>(h->chunk, ka, h->smem_bytes64, s));
         }
-    } else if (h->use_tmem) {
+    } else if (h->persistent) {
         // one work counter per concurrently running launch (pipeline chunk); counters rotate
         int *ctr = h->d_counters + (h->counter_next++ % pqp_handle::kCounters);
         PQP_CUDA(h, cudaMemsetAsync(ctr, 0, sizeof(int), s));
         ka.work_counter = ctr;
-        PQP_CUDA(h, launch_tmem_chunk(h->chunk, ka, s, h->sm_count, h->incr));
+        PQP_CUDA(h, launch_persistent_chunk(h->chunk, ka, h->smem_bytes, s, h->sm_count * h->warps_per_sm, h->incr));
     } else {
         PQP_CUDA(h, launch_chunk<float>(h->chunk, ka, h->smem_bytes, s, h->incr));
     }
@@ -923,7 +614,7 @@ int escalate_fp64(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *ou
 
 
 
-// Host-buffer solve on the persistent tensor-memory kernel as ONE launch over the whole batch:
+// Host-buffer solve on the persistent kernel as ONE launch over the whole batch:
 // the kernel starts immediately and each warp waits (ready[chunk]) until the H2D copy of the
 // chunk its next instance belongs to has landed; finished chunks are announced through mapped
 // host memory (host_done[chunk]) so their D2H copies overlap the rest of the solve. Compared
@@ -933,7 +624,7 @@ int run_host_streamed(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out
     const size_t nvm = 6 * (size_t)nmax - 1, mm = 6 * (size_t)nmax + 2;
     // up to kStreams chunks of >= 256 instances: small batches (configs[1]: 1024) still overlap
     // their copies with the solve, large ones (8192) move 1024 instances per chunk
-    const int min_chunk = 256;  // profiles/chunk_sweep.sh
+    const int min_chunk = 256;
     int nchunks = (B + min_chunk - 1) / min_chunk;
     if (nchunks > pqp_handle::kStreams) nchunks = pqp_handle::kStreams;
     const int per = (B + nchunks - 1) / nchunks;
@@ -1043,7 +734,7 @@ int run_host(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *out, in
         if (mode == 1 && (!h->solved || B != h->last_batch)) return fail(h, PQP_E_STATE, "resolve needs a previous solve of the same batch");
         h->host_inputs_resident = true;
         h->d_p_valid = in->p != nullptr;
-        if (h->use_tmem && B >= 512) {
+        if (h->persistent && B >= 512) {
             const size_t nvm0 = 6 * (size_t)nmax - 1, mm0 = 6 * (size_t)nmax + 2;
             if (out->x_full && !h->d_xf) PQP_CUDA(h, dmalloc(&h->d_xf, (size_t)h->batch_max * nvm0));
             if (out->y_full && !h->d_yf) PQP_CUDA(h, dmalloc(&h->d_yf, (size_t)h->batch_max * mm0));
@@ -1189,8 +880,8 @@ int pqp_create(const pqp_params *params, int32_t n_max, int32_t batch_max, int32
     if (device < 0 || device >= ndev) return fail(nullptr, PQP_E_NO_DEVICE, "device index out of range");
     cudaDeviceProp prop;
     if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) return cuda_fail(nullptr, e, "cudaGetDeviceProperties");
-    if (prop.major != 10)
-        return fail(nullptr, PQP_E_NO_DEVICE, "this library is built for sm_100a (B200) only; found sm_" +
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(nullptr, PQP_E_NO_DEVICE, "this library is built for sm_90a (H100) only; found sm_" +
                                                   std::to_string(prop.major) + std::to_string(prop.minor));
     pqp_handle *h = new (std::nothrow) pqp_handle;
     if (!h) return fail(nullptr, PQP_E_INVALID, "out of host memory");
@@ -1214,29 +905,33 @@ int pqp_create(const pqp_params *params, int32_t n_max, int32_t batch_max, int32
     h->fp64 = (params->reserved & 2) != 0;
     h->escalate = (params->reserved & 4) == 0;
     h->cold_only = (params->reserved & 128) != 0;
-    // storage policy of the FP32 kernel (measured, profiles/r2/policy_ab.log): tensor memory for n_max >= 64
-    // (chunks of 4, 8, 16 stages per lane: 8 / 4 / 2 QPs per SM; at n = 240 shared memory would hold 3 per SM, at
-    // n = 120 it holds 6 but runs 3.48 ms against 3.21 ms per 8192 instances, at 1024 instances 0.92 vs 0.76 ms),
-    // shared memory below (n = 60: 1.59 vs 1.82 ms). Bits 8 / 16 force one or the other.
-    const bool auto_tmem = h->chunk >= 4;
-    h->use_tmem = !h->fp64 && ((params->reserved & 8) != 0 || (auto_tmem && (params->reserved & 16) == 0));
+    // launch of the FP32 kernel (measured on H100, 8192 instances, DESIGN.md §5): persistent (work counter, one
+    // streamed launch per host call) for n_max >= 128, where three QPs fill an SM's shared memory (n = 240: 0.5-1 %
+    // ahead); one CTA per instance below (n = 120: 2.7 % ahead, n = 60: equal). Both keep the state in shared
+    // memory. Bits 8 / 16 force one or the other.
+    const bool auto_persistent = h->chunk >= 8;
+    h->persistent = !h->fp64 && ((params->reserved & 8) != 0 || (auto_persistent && (params->reserved & 16) == 0));
     // form of the ADMM step (FP32 kernels): the increment form (dx solve, row values A x carried and
-    // advanced by alpha A dx) follows the FP64 oracle's rho schedule - same iteration count in ~99-100 %
-    // of instances, ~6 % fewer iterations - for ~6 % more work per iteration. Measured against the
-    // textbook form: n = 240 equal (892 k solves/s), n = 120 +5 %, the 1024 x 120 shared-map batch
-    // +15 % (one wave: its slowest instances need fewer iterations), n = 60 -3.5 %. Default: increment
-    // form for n_max >= 64, textbook form below; bits 32 / 64 force one or the other.
+    // advanced by alpha A dx) follows the FP64 oracle's rho schedule - the same iteration count in almost
+    // every instance, fewer iterations on average - for a few per cent more work per iteration. Default:
+    // increment form for n_max >= 64, textbook form below; bits 32 / 64 force one or the other.
     h->incr = !h->fp64 && ((params->reserved & 32) != 0 || ((params->reserved & 64) == 0 && h->chunk >= 4));
-    if (h->use_tmem) PQP_CREATE_CUDA(prepare_tmem_chunk(h->chunk));
     h->smem_bytes64 = pqp::smem_floats(h->chunk) * sizeof(double) + 16;
     int bps = 0;
     if (h->fp64) {
         PQP_CREATE_CUDA(prepare_chunk<double>(h->chunk, h->smem_bytes64, &bps));
         h->prepared64 = true;
+    } else if (h->persistent) {
+        PQP_CREATE_CUDA(prepare_persistent_chunk(h->chunk, h->smem_bytes, &bps, h->incr));
     } else {
         PQP_CREATE_CUDA(prepare_chunk<float>(h->chunk, h->smem_bytes, &bps, h->incr));
     }
-    h->warps_per_sm = h->use_tmem ? tmem_warps(h->chunk) : bps;
+    if (bps < 1) {
+        g_create_error = "the solve kernel does not fit on an SM";
+        pqp_destroy(h);
+        return PQP_E_CUDA;
+    }
+    h->warps_per_sm = bps;
     for (int i = 0; i < pqp_handle::kStreams; ++i) {
         PQP_CREATE_CUDA(cudaStreamCreateWithFlags(&h->streams[i], cudaStreamNonBlocking));
         PQP_CREATE_CUDA(cudaEventCreateWithFlags(&h->evs[i], cudaEventDisableTiming));
@@ -1258,13 +953,13 @@ int pqp_create(const pqp_params *params, int32_t n_max, int32_t batch_max, int32
     // Warm state (scaled x, z, y and rho: the OSQP workspace that persists between solve and
     // updateProblemFormulationAndSolve) is per instance; a cold-only handle keeps none. The Ruiz
     // factors and delta_y are scratch of one solve: per instance under the one-CTA-per-instance
-    // launch, per resident warp under the persistent launch (592 blocks that live in L2).
+    // launch, per resident warp under the persistent launch.
     if (!h->cold_only) {
         PQP_CREATE_CUDA(cudaMalloc(&h->d_warm, B * pqp::warm_floats(c) * esz));
         PQP_CREATE_CUDA(cudaMemset(h->d_warm, 0, B * pqp::warm_floats(c) * esz));
         PQP_CREATE_CUDA(cudaMalloc(&h->d_rho, B * esz));
     }
-    const size_t slots = h->use_tmem ? (size_t)h->sm_count * tmem_warps(h->chunk) : B;
+    const size_t slots = h->persistent ? (size_t)h->sm_count * h->warps_per_sm : B;
     PQP_CREATE_CUDA(cudaMalloc(&h->d_scal, slots * pqp::scal_floats(c) * esz));
     PQP_CREATE_CUDA(cudaMalloc(&h->d_dy, slots * pqp::dy_floats(c) * esz));
     for (int i = 0; i < 4; ++i) PQP_CREATE_CUDA(cudaEventCreate(&h->ev_st[i]));
@@ -1445,9 +1140,7 @@ int pqp_kernel_info(pqp_handle *h, int32_t *sm_count, int32_t *warps_per_sm, int
     if (!h) return PQP_E_INVALID;
     if (sm_count) *sm_count = h->sm_count;
     if (warps_per_sm) *warps_per_sm = h->warps_per_sm;
-    // tensor-memory policy: only the groups that do not fit the warp's columns live in shared memory
-    if (smem_per_warp)
-        *smem_per_warp = h->use_tmem ? (int32_t)tmem_spill_bytes(h->chunk) : (int32_t)h->smem_bytes;
+    if (smem_per_warp) *smem_per_warp = (int32_t)h->smem_bytes;
     return PQP_OK;
 }
 

@@ -5,7 +5,7 @@
 //   OSQP setup (Ruiz scaling, rho vec) base_solver.cpp:87   (osqp_setup through osqp-eigen)
 //   OSQP ADMM loop, termination, rho   base_solver.cpp:88,110
 //   warm update of A and bounds        base_solver.cpp:102-107
-// How (B200 design, see DESIGN.md):
+// How (see DESIGN.md):
 //   * one warp per QP instance, lane L owns the C consecutive stages [L*C, L*C+C) of the
 //     stage chain (stage 0 is a virtual stage whose outgoing rows are the x0 rows, stage
 //     g>=1 is knot g-1, the last knot's outgoing rows are the two end-state rows);
@@ -283,16 +283,15 @@ PQP_DEV void soft_bounds(double lb, double ub, double margin, double &olb, doubl
 // ------------------------------------------------------------------ storage policies
 // Where a QP's per-stage state lives. Logical field f = 4*group + component; the policy maps
 // (field, local stage k, this lane) to storage. Only the owning lane ever touches an element:
-// neighbour values travel by warp shuffle, never by cross-lane loads, so the same solver code
-// runs on shared memory (SmemStore) and on tensor memory (TmemStore in pqp_api.cu).
+// neighbour values travel by warp shuffle, never by cross-lane loads, so the solver code is
+// written against the policy's interface (loads in batches, a stage cursor) rather than raw indexing.
 template <int C, typename real>
 struct SmemStore {
     typedef typename Vec4T<real>::type Vec4;
     real *sm;
     int lane;
-    // cyclic-reduction levels unrolled? Under this policy several warps share a scheduler and the hot loop should
-    // stay small: measured +5 % / +7.5 % at C = 2 / 1 (n = 60 / 30), -5.5 % at C = 4 (n = 120), -4 % in FP64
-    // (profiles/r2/cr_unroll_smem_ab.log)
+    // cyclic-reduction levels unrolled? Several warps share a scheduler and the hot loop should stay small: unrolled
+    // only at C <= 2 in FP32, where the levels are a large share of the work
     static constexpr bool kUnrollCr = C <= 2 && sizeof(real) == 4;
     PQP_DEV SmemStore(real *s, int l) : sm(s), lane(l) {}
     PQP_DEV real ld(int f, int k) const { return sm[(((f >> 2) * C + k) * 32 + lane) * 4 + (f & 3)]; }
@@ -311,7 +310,7 @@ struct SmemStore {
     template <int N> PQP_DEV void ld4n_nowait(int g0, int k, real (&out)[4 * N]) const { ld4n<N>(g0, k, out); }
     PQP_DEV void wait_ld() const {}
     PQP_DEV void fence() {}  // stores of this lane are visible to its later loads
-    // stage cursor (see TmemStore): plain stage indexing under this policy
+    // stage cursor: plain stage indexing under this policy
     PQP_DEV void seek(int) {}
     template <int G0, int N> PQP_DEV void ld_run_nowait(int k, real (&out)[4 * N]) const { ld4n<N>(G0, k, out); }
     template <int G0, int N> PQP_DEV void ld_run_nowait_cur(int k, real (&out)[4 * N]) const { ld4n<N>(G0, k, out); }
@@ -324,12 +323,11 @@ struct SmemStore {
 };
 
 // =========================================================================================
-// Which loops are unrolled is a measured choice (profiles/r1, profiles/r2 README):
-//  * per-stage loops with large bodies (stage update, residuals, set-up) stay rolled (#pragma unroll 1): the first
-//    version of this kernel unrolled them, which produced a 45 KB hot loop that thrashed the instruction cache (40 %
-//    no_inst stalls, profiles/r1/ncu_v1_unrolled_summary.txt); the rolled stage-update loop fits the 6 KB L0;
-//  * the substitution sweeps are fully unrolled: rolled, half of their instructions were register copies of the
-//    prefetched factor and address conversions (profiles/r2/README.md);
+// Which loops are unrolled:
+//  * per-stage loops with large bodies (stage update, residuals, set-up) stay rolled (#pragma unroll 1): unrolled,
+//    they make a hot loop of tens of KB that thrashes the instruction cache;
+//  * the substitution sweeps are fully unrolled: rolled, much of their instruction stream is register copies of the
+//    prefetched factor and address arithmetic;
 //  * the cyclic-reduction levels are unrolled per storage policy (Store::kUnrollCr).
 #define PQP_ROLL _Pragma("unroll 1")
 #define PQP_SWEEP_UNROLL _Pragma("unroll")
@@ -338,8 +336,8 @@ struct SmemStore {
 // K dx = -(r_dual + A'R r_prim), x~ = x + dx, with l carried as l + l_lo) instead of the textbook
 // form (solve K x~ = S x + A'(R z - y)): algebraically the same iteration, but its rounding error
 // scales with |dx| instead of |x|, so the FP32 kernel follows the FP64 oracle's rho schedule
-// (same iteration count in 98-99 % of instances instead of 85 %, ~6 % fewer iterations) at ~8 % more
-// instructions per iteration (profiles/r1/README.md).
+// (tests/test_gpu_parity.py: same iteration count in >= 95 % of instances) at a few per cent more
+// instructions per iteration.
 
 template <int C, typename real, typename Store = SmemStore<C, real>, bool Incr = false>
 struct QpWarp {
@@ -472,8 +470,7 @@ struct QpWarp {
     // weights R / classes / S in shared memory.
     // One Ruiz pass: reads D, E from the three groups GF0 + 3 CUR .. (d0 d1 d2 d3 | d4 d5 e0 e1 | e2 e3 e4 e5), writes
     // the other half. Whole groups, one load batch per stage (the stage's a-coefficients, its D / E, the next stage's D)
-    // and three group stores: the first version read and wrote the 24 values one 32-bit tensor-memory access at a
-    // time, each with its own wait (~2400 dependent round trips per solve, profiles/r2/README.md).
+    // and three group stores, instead of 24 single-value accesses each with its own round trip.
     template <int CUR>
     PQP_DEV void ruiz_pass(real c, real &psum) {
         constexpr int G0 = GF0 + 3 * CUR, G1 = GF0 + 3 * (1 - CUR);
@@ -537,8 +534,8 @@ struct QpWarp {
 #pragma unroll
             for (int j = 0; j < 6; ++j) {
                 // 1/sqrt as one MUFU.RSQ in FP32 (2 ulp): the Ruiz factors are only required to be
-                // positive - any D, E give an equivalent problem - and 960 sqrt + divide pairs per
-                // solve were 7 % of the kernel's stall samples; the FP64 instantiation stays exact
+                // positive - any D, E give an equivalent problem - and a sqrt + divide pair per entry
+                // is costly in the set-up; the FP64 instantiation stays exact
                 dn[j] = dk[j] * xfast_rsqrt(limit_scaling(cn[j]));
                 en[j] = ek[j] * xfast_rsqrt(limit_scaling(rn[j]));
                 psum += dn[j] * dn[j] * pw[j];
@@ -719,8 +716,8 @@ struct QpWarp {
     }
 
     // -------------------------------------------------------------- factorisation
-    // What the factorisation reads of one stage, fetched as whole groups in ONE load batch (it used to read these
-    // ~18 values - several of them twice - one 32-bit tensor-memory access and one wait at a time).
+    // What the factorisation reads of one stage, fetched as whole groups in ONE load batch (~18 values, several of
+    // them needed twice).
     struct FacIn {
         real a00, a01, a10, a11, a12, ds, ob[3], Ro[3], Rk, Rc[2], Sw[6];
     };
@@ -1071,8 +1068,7 @@ struct QpWarp {
             bs[r] = bk[r] - fr;
         }
         // cyclic reduction over the 32 separators: 5 forward levels, 3x3 solve, 5 backward levels; unrolled with
-        // constant shuffle distances and lane masks under the tensor-memory policy (Store::kUnrollCr; at C = 4 with
-        // two warps per scheduler: +8..21 % on 1024-instance batches, profiles/r2/cr_unroll_c4_ab.log)
+        // constant shuffle distances and lane masks where the storage policy asks for it (Store::kUnrollCr)
         if (Store::kUnrollCr) {
 #pragma unroll
             for (int t = 0; t < 5; ++t) cr_forward_level(t, bs);
@@ -1459,8 +1455,8 @@ struct QpWarp {
     }
 
     // ADMM update of all stages (ascending; the left neighbour's outgoing rows are carried in
-    // registers). A variant fused with the next forward sweep was measured slower (in-order issue
-    // serialises the sweep step behind each stage's update; profiles/r1/README.md).
+    // registers). It is not fused with the next forward sweep: in-order issue would serialise the sweep
+    // step behind each stage's update.
     // in: GBV = x~; out: iterates advanced, GBV = rhs of the next solve.
     template <bool kCheck>
     PQP_DEV void admm_update(bool first, bool warm) {
@@ -1636,8 +1632,7 @@ struct QpWarp {
     }
 
     // kMaybeFirst = false: the caller knows this is not the first iteration of a solve, and the stage loop carries
-    // no branch around the z0 code (that taken branch and the refetch behind it were 3.5 % of the kernel's stall
-    // samples, profiles/r2/README.md)
+    // no branch around the z0 code (a taken branch and an instruction refetch in the hottest loop)
     template <bool kCheck, bool kMaybeFirst>
     PQP_DEV void admm_update_incr(bool first_arg, bool warm) {
         const bool first = kMaybeFirst && first_arg;
@@ -1740,7 +1735,7 @@ struct QpWarp {
                 if (Incr) {
                     // c d_j straight from the Ruiz D (the increment form keeps no S on chip; recomputing
                     // S = sigma / (c d^2) only to take kd / sqrt(S) = c d cost a division and a rsqrt per entry:
-                    // 0.9 % of the instructions but 4.7 % of the stall samples, profiles/r2/README.md)
+                    // few instructions but long stalls)
 #pragma unroll
                     for (int j = 0; j < 6; ++j) {
                         const bool exists = (j == 3) ? sp.mid : (j == 5 ? sp.act1 : sp.real);
@@ -1980,7 +1975,7 @@ struct QpWarp {
         bool need_factor = true, initial = true;
         // Heavy, rarely executed pieces (factorisation, rhs rebuild, residuals, termination) have
         // exactly one call site each: instruction-cache footprint matters once the resident
-        // warps of an SM drift out of phase (profiles/r1/README.md).
+        // warps of an SM drift out of phase.
         PQP_ROLL
         for (;;) {
             if (need_factor) {

@@ -6,7 +6,7 @@ paths: `solve()` is `BaseSolver::solve` (base_solver.cpp:56-95), `resolve()` is
 the device buffers and the per-instance warm state the way the reference's solver object
 owns its OSQP workspace (base_solver.hpp:62).
 
-There is no CPU path: if the CUDA library is missing or no B200 is visible, construction
+There is no CPU path: if the CUDA library is missing or no H100 is visible, construction
 raises.
 """
 import ctypes as C
@@ -20,7 +20,7 @@ from . import abi
 _PKG = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("PQP_LIB_PATH", os.path.join(_PKG, "libpqp_b200.so"))  # override: A/B builds
 _CSRC = os.path.join(_PKG, "csrc")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-diag-suppress", "607,177",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-diag-suppress", "607,177",
               "--shared", "-Xcompiler", "-fPIC"]
 _lib = None
 
@@ -32,7 +32,7 @@ class PqpError(RuntimeError):
 
 
 def build_library(force=False, verbose=False):
-    """nvcc-compile the CUDA library in-tree for sm_100a (no GPU needed to compile)."""
+    """nvcc-compile the CUDA library in-tree for sm_90a (no GPU needed to compile)."""
     root = os.path.dirname(_PKG)
     cu = [os.path.join(_CSRC, f) for f in ("pqp_api.cu", "pqp_bounds.cu", "pqp_multi.cu", "pqp_smoother.cu")]
     deps = cu + [os.path.join(_CSRC, f) for f in ("pqp_kernel.cuh", "pqp_host_common.h", "pqp_bounds_core.cuh", "pqp_device_guard.h",

@@ -17,27 +17,26 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BIN = os.path.join(ROOT, "tests", "cpp", "dropin_test")
 
 
-BIN_REAL = BIN + "_real"
-REF = "/root/reference"
+BIN_REAL = os.path.join(ROOT, "oracle", "_ref", "dropin_test_real")
+REF = os.environ.get("PQP_REFERENCE_ROOT")  # a checkout of the original path_optimizer_2 (default: oracle/Makefile's)
 
 
 def _build(real=False):
-    """real=True: bind the drop-in to the reference's OWN boundary types (data_struct.hpp,
-    vehicle_state_frenet.{hpp,cpp} compile standalone, SURVEY.md §8c). Only possible where
-    /root/reference exists (the CPU box); the binary is git-ignored but travels to the GPU box."""
+    """real=True: the drop-in bound to the original project's OWN boundary types (data_struct.hpp,
+    vehicle_state_frenet.{hpp,cpp} compile standalone, SURVEY.md §8c), built by oracle/Makefile into
+    oracle/_ref/ where a checkout of it is readable; None where it was never built."""
     solver.build_library()
-    out = BIN_REAL if real else BIN
+    if real:
+        subprocess.check_call(["make", "-C", os.path.join(ROOT, "oracle"), "-s", "ref"] +
+                              (["REFERENCE=" + os.path.abspath(REF)] if REF else []))
+        return BIN_REAL if os.path.exists(BIN_REAL) else None
     src = os.path.join(ROOT, "tests", "cpp", "dropin_test.cpp")
     deps = [src, os.path.join(ROOT, "include", "pqp_base_solver.hpp"), os.path.join(ROOT, "tests", "cpp", "ref_stub.hpp"),
             solver.LIB_PATH]
-    if real and not os.path.isdir(REF):
-        return out if os.path.exists(out) else None
-    if not os.path.exists(out) or any(os.path.getmtime(d) > os.path.getmtime(out) for d in deps):
-        extra = ["-DPQP_TEST_REAL_TYPES", "-I", os.path.join(REF, "include"), "-w",
-                 os.path.join(REF, "src", "data_struct", "vehicle_state_frenet.cpp")] if real else ["-Wall"]
-        subprocess.check_call(["g++", "-std=c++11", "-O1", "-o", out, src] + extra + [
-            solver.LIB_PATH, "-Wl,-rpath," + os.path.dirname(solver.LIB_PATH)])
-    return out
+    if not os.path.exists(BIN) or any(os.path.getmtime(d) > os.path.getmtime(BIN) for d in deps):
+        subprocess.check_call(["g++", "-std=c++11", "-O1", "-o", BIN, src, "-Wall", solver.LIB_PATH,
+                               "-Wl,-rpath," + os.path.dirname(solver.LIB_PATH)])
+    return BIN
 
 
 def _write_instance(path, knots, inst, n, ref, target_heading, constraint_end_heading=1):
@@ -55,7 +54,7 @@ def _write_instance(path, knots, inst, n, ref, target_heading, constraint_end_he
 def test_dropin_compiles_and_fails_loudly_without_gpu(tmp_path, real):
     exe = _build(real)
     if exe is None:
-        pytest.skip("the reference tree is not present on this box")
+        pytest.skip("oracle/_ref/dropin_test_real was not built (no checkout of the original project at build time)")
     try:
         import torch
         if torch.cuda.is_available():
@@ -75,7 +74,7 @@ def test_dropin_matches_python_binding(tmp_path, real):
     from oracle import oracle
     exe = _build(real)
     if exe is None:
-        pytest.skip("dropin_test_real was not built on the CPU box")
+        pytest.skip("oracle/_ref/dropin_test_real was not built (no checkout of the original project at build time)")
     params = abi.default_params()
     for idx in range(3):
         knots, inst, n, ref = synthetic.make_instance(3, idx, 120)

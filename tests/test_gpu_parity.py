@@ -301,11 +301,11 @@ def test_increment_form_tracks_the_oracle_iteration_counts(solver_mod, n):
 
 
 @pytest.mark.parametrize("n", [20, 120, 240, 400])
-def test_tensor_memory_policy_matches_shared_memory_policy(solver_mod, n):
-    """params.reserved bit 3 / bit 4: the same solver code with its per-stage state in tensor
-    memory (tcgen05.ld/st, persistent CTAs) or in shared memory. Same arithmetic -> same answers.
-    (Default: tensor memory for n_max >= 128, shared memory below.)"""
-    hb = synthetic.make_batch(3, 9, n)   # 9: exercises a partially filled last CTA (4 QPs per CTA)
+def test_persistent_launch_matches_per_instance_launch(solver_mod, n):
+    """params.reserved bit 3 / bit 4: the same solver code launched persistently (one-warp CTAs that take
+    instances from a work counter) or as one CTA per instance. Same arithmetic -> same answers.
+    (Default: persistent for n_max >= 128, one CTA per instance below.)"""
+    hb = synthetic.make_batch(3, 9, n)
     for form in (64, 32):  # textbook / increment form of the ADMM step, the same on both sides
         res = {}
         for bits in (16, 8):
@@ -321,7 +321,7 @@ def test_tensor_memory_policy_matches_shared_memory_policy(solver_mod, n):
     params = abi.default_params(reserved=8)
     for b in range(hb.batch):
         s = parity.oracle_reference(params, hb, b)
-        parity.check_instance(params, hb, res[8][0], b, oracle_solver=s, label="tmem n=%d" % n)
+        parity.check_instance(params, hb, res[8][0], b, oracle_solver=s, label="persistent n=%d" % n)
 
 
 def test_cold_only_handle_and_device_side_size_check(solver_mod):
@@ -376,7 +376,7 @@ def test_two_handles_driven_by_two_host_threads(solver_mod):
     answers of a lone call, bit for bit, whatever the interleaving of their launches and copies."""
     import threading
     params = abi.default_params(reserved=128)
-    hb = synthetic.make_batch(3, 1500, 240)   # > 592 resident warps: the two persistent launches really share the SMs
+    hb = synthetic.make_batch(3, 1500, 240)   # > 396 resident warps: the two persistent launches really share the SMs
     ref_sv = solver_mod.PathQpSolver(params, n_max=hb.n_max, batch_max=hb.batch)
     ref = ref_sv.solve(hb)
     ref_sv.close()
