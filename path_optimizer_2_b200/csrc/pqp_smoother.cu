@@ -128,6 +128,9 @@ int launch(pqp_smoother_handle *h, KArgs &a, cudaStream_t s) {
     a.scratch = h->d_scratch;
     a.scratch_stride = h->scratch_stride;
     const int grid = a.batch < h->grid_max ? a.batch : h->grid_max;
+    // the dynamic shared-memory limit is an attribute of the kernel, not of the handle: a handle created later with a
+    // smaller p_max lowers it, so each launch sets this handle's own
+    PQS_CUDA(h, cudaFuncSetAttribute(smoother_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem));
     PQS_CUDA(h, cudaEventRecord(h->ev0, s));
     smoother_kernel<<<grid, 32, h->smem, s>>>(a);
     PQS_CUDA(h, cudaGetLastError());

@@ -169,6 +169,34 @@ class LineBatch:
         return np.ascontiguousarray(self.states[:, 1:4])
 
 
+def make_plan_inputs(batch, n=120, first=0, dmap=None, seed=11, noise=0.03):
+    """Inputs of a whole plan (include/pqp_plan.h) from the lines of `make_lines`: the line sampled about every 1 m
+    with `noise` m of noise stands in for bSpline()'s samples; the start lies up to 1 m beside the line at s = 0.5
+    with its heading and curvature, the target on the line 1 m before its end. -> (raw_x, raw_y lists, start [B][4],
+    target [B][3])."""
+    lines = make_lines(batch, n, first=first, dmap=dmap)
+    rng = np.random.default_rng(seed + first)
+    raw_x, raw_y = [], []
+    start, target = np.zeros((batch, 4)), np.zeros((batch, 3))
+    for b in range(batch):
+        rows = lines.spline_rows(b)
+        end = float(rows[0, -1])
+        s = np.arange(0.0, end, 1.0)
+        x, dx, ddx = _eval(rows, s, 0)
+        y, dy, ddy = _eval(rows, s, 1)
+        raw_x.append(x + rng.normal(0, noise, len(s)))
+        raw_y.append(y + rng.normal(0, noise, len(s)))
+        x0, dx0, ddx0 = (float(v) for v in _eval(rows, 0.5, 0))
+        y0, dy0, ddy0 = (float(v) for v in _eval(rows, 0.5, 1))
+        h = math.atan2(dy0, dx0)
+        off = rng.uniform(-1.0, 1.0)
+        start[b] = x0 - off * math.sin(h), y0 + off * math.cos(h), h, (dx0 * ddy0 - dy0 * ddx0) / math.pow(dx0 * dx0 + dy0 * dy0, 1.5)
+        xe, dxe, _ = (float(v) for v in _eval(rows, end - 1.0, 0))
+        ye, dye, _ = (float(v) for v in _eval(rows, end - 1.0, 1))
+        target[b] = xe, ye, math.atan2(dye, dxe)
+    return raw_x, raw_y, start, target
+
+
 def make_lines(batch, n=120, first=0, cfg_id=2, dmap=None):
     """Lines [first, first + batch) of the shared-map config; line i depends only on (cfg_id, i)."""
     dmap = dmap or DistanceMap()

@@ -36,19 +36,25 @@ def build_library(force=False, verbose=False):
     root = os.path.dirname(_PKG)
     cu = [os.path.join(_CSRC, f) for f in ("pqp_api.cu", "pqp_bounds.cu", "pqp_multi.cu", "pqp_smoother.cu")]
     deps = cu + [os.path.join(_CSRC, f) for f in ("pqp_kernel.cuh", "pqp_host_common.h", "pqp_bounds_core.cuh", "pqp_device_guard.h",
-                                                  "pqp_dp.cu", "pqp_dp_core.cuh", "pqp_bounds_internal.h", "pqp_smoother_core.cuh")]
-    deps += [os.path.join(root, "include", f) for f in ("pqp.h", "pqp_bounds.h", "pqp_multi.h", "pqp_dp.h", "pqp_smoother.h")]
+                                                  "pqp_dp.cu", "pqp_dp_core.cuh", "pqp_bounds_internal.h", "pqp_smoother_core.cuh",
+                                                  "pqp_plan.cu", "pqp_plan_core.cuh")]
+    deps += [os.path.join(root, "include", f) for f in ("pqp.h", "pqp_bounds.h", "pqp_multi.h", "pqp_dp.h", "pqp_smoother.h",
+                                                        "pqp_plan.h")]
     stale = not os.path.exists(LIB_PATH) or any(
         os.path.getmtime(s) > os.path.getmtime(LIB_PATH) for s in deps)
     if force or stale:
-        # the lattice DP (pqp_dp.cu) is a chain of threshold / strict-minimum decisions in FP64: it is compiled
-        # without multiply-add contraction so that every operation rounds as in the host restatement
-        obj = os.path.join(_PKG, "pqp_dp.o")
+        # the lattice DP (pqp_dp.cu) is a chain of threshold / strict-minimum decisions in FP64, and the plan glue
+        # (pqp_plan.cu) is threshold decisions plus spline fits that must equal the host restatement bit for bit: both
+        # are compiled without multiply-add contraction so that every operation rounds as in the host restatement
         common = [f for f in NVCC_FLAGS if f != "--shared"] + (["-Xptxas", "-v"] if verbose else []) + [
             "-I", os.path.join(root, "include")]
-        subprocess.check_call(["nvcc"] + common + ["--fmad=false", "-c", os.path.join(_CSRC, "pqp_dp.cu"), "-o", obj])
+        objs = []
+        for src in ("pqp_dp.cu", "pqp_plan.cu"):
+            obj = os.path.join(_PKG, src[:-3] + ".o")
+            subprocess.check_call(["nvcc"] + common + ["--fmad=false", "-c", os.path.join(_CSRC, src), "-o", obj])
+            objs.append(obj)
         cmd = ["nvcc"] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + [
-            "-I", os.path.join(root, "include"), "-o", LIB_PATH] + cu + [obj, "-ldl"]
+            "-I", os.path.join(root, "include"), "-o", LIB_PATH] + cu + objs + ["-ldl"]
         subprocess.check_call(cmd)
     return LIB_PATH
 
