@@ -5,7 +5,8 @@ every 1 m with 3 cm of noise as the bSpline() samples, the start up to 1 m besid
 1 m before its end. Prints one JSON line: plans/s at B = 1024 (device call, CUDA events around the timed loop), ms per
 plan at B = 1 (host call), the per-stage device times of the last call, kernel launches per plan, the status histogram,
 the CPU Python oracle chain's plans/s on a sample (the Python restatement, not the reference), and the GPU's name and
-power limit read in the same run. Writes nothing to the source tree.
+power limit read in the same run. --smoothing-method selects the reference smoother (TENSION2, the default, or
+TENSION). Writes nothing to the source tree.
 """
 import argparse
 import json
@@ -37,16 +38,19 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--oracle-sample", type=int, default=8)
+    ap.add_argument("--smoothing-method", choices=("TENSION2", "TENSION"), default="TENSION2",
+                    help="the reference's --smoothing_method: TensionSmoother2 (default) or TensionSmoother")
     args = ap.parse_args()
     import torch
 
-    from oracle import plan_oracle
+    from oracle import cartesian_oracle, plan_oracle
     from path_optimizer_2_b200 import plan, sharedmap
     dmap = sharedmap.DistanceMap()
     B = args.batch
     raw_x, raw_y, start, target = sharedmap.make_plan_inputs(B, dmap=dmap)
     R, P, L, N = 64, 64, 64, 255
-    pl = plan.Planner(dmap.dist, dmap.res, r_max=R, p_max=P, layers_max=L, n_max=N, batch_max=B)
+    params = plan.default_params(args.smoothing_method)
+    pl = plan.Planner(dmap.dist, dmap.res, r_max=R, p_max=P, layers_max=L, n_max=N, batch_max=B, params=params)
     dev = torch.device("cuda:0")
     r = np.array([len(v) for v in raw_x], dtype=np.int32)
     rx, ry = np.zeros((B, R)), np.zeros((B, R))
@@ -70,7 +74,7 @@ def main():
     status = out["status"].cpu().numpy()
     hist = {plan.STATUS_NAMES[c]: int(np.sum(status == c)) for c in sorted(set(status.tolist()))}
 
-    one = plan.Planner(dmap.dist, dmap.res, r_max=R, p_max=P, layers_max=L, n_max=N, batch_max=1)
+    one = plan.Planner(dmap.dist, dmap.res, r_max=R, p_max=P, layers_max=L, n_max=N, batch_max=1, params=params)
     for _ in range(args.warmup):
         one.plan(raw_x[:1], raw_y[:1], start[:1], target[:1])
     t0 = time.perf_counter()
@@ -82,10 +86,11 @@ def main():
     one.close()
 
     k = min(args.oracle_sample, B)
+    oracle_plan = cartesian_oracle.plan if args.smoothing_method == "TENSION" else plan_oracle.plan
     t0 = time.perf_counter()
     for b in range(k):
-        plan_oracle.plan(dmap.dist, dmap.res, raw_x[b], raw_y[b], start[b], target[b], params=pl.params.solver,
-                         p_max=P, layers_max=L, n_max=N)
+        oracle_plan(dmap.dist, dmap.res, raw_x[b], raw_y[b], start[b], target[b], params=pl.params.solver,
+                    p_max=P, layers_max=L, n_max=N)
     oracle_s = time.perf_counter() - t0
     pl.close()
     print(json.dumps({
@@ -95,7 +100,7 @@ def main():
         "ms_per_plan_b1_host_call": ms_one, "stage_ms_last_batch": stages, "stage_ms_b1": stages_one,
         "kernel_launches_per_plan_call": launches, "status_histogram": hist,
         "python_oracle_chain_plans_per_s": k / oracle_s, "python_oracle_sample": k,
-        "gpu": gpu_info(), "steps": args.steps, "warmup": args.warmup}))
+        "gpu": gpu_info(), "steps": args.steps, "warmup": args.warmup, "smoothing_method": args.smoothing_method}))
 
 
 if __name__ == "__main__":

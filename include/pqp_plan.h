@@ -3,9 +3,10 @@
  *
  * reference interface replaced:
  *   PathOptimizer::solve                         src/path_optimizer.cpp:34-71
- *     ReferencePathSmoother::solve (TENSION2)    src/reference_path_smoother/reference_path_smoother.cpp:31-45
+ *     ReferencePathSmoother::solve               src/reference_path_smoother/reference_path_smoother.cpp:17-45
  *       segmentRawReference + s_list_             :47-85, :519-523
  *       TensionSmoother2::osqpSmooth + spline     tension_smoother_2.cpp:20-72, tension_smoother.cpp:36-41
+ *       or TensionSmoother::osqpSmooth (TENSION)  tension_smoother.cpp:20-177, clearance Map.cpp:16-22
  *       graphSearchDp, postSmooth                 reference_path_smoother.cpp:142-295, :526-580
  *     processReferencePath                        src/path_optimizer.cpp:73-122, src/tools/tools.cpp:57-126
  *     optimizePath (solve, re-solve, path)        src/path_optimizer.cpp:124-161, src/solver/base_solver.cpp
@@ -37,7 +38,7 @@ enum {
     PQP_PLAN_OK = 0,
     PQP_PLAN_SPLINE_DEGENERATE = 1, /* fewer than 3 samples, or abscissae (arc lengths) not increasing */
     PQP_PLAN_TOO_MANY_POINTS = 2,   /* resampled list longer than p_max, or more DP layers than layers_max */
-    PQP_PLAN_TENSION_FAILED = 3,    /* tension QP not solved (tension_smoother.cpp:32-35) */
+    PQP_PLAN_TENSION_FAILED = 3,    /* tension QP (either method) not solved (tension_smoother.cpp:32-35) */
     PQP_PLAN_DP_VEHICLE_FAR = 4,    /* graphSearchDp: |vehicle offset| > lateral range */
     PQP_PLAN_POST_TOO_SHORT = 5,    /* postSmooth: fewer than 4 DP layers kept */
     PQP_PLAN_POST_FAILED = 6,       /* post-smooth QP not solved */
@@ -70,8 +71,17 @@ typedef struct pqp_plan_params {
     int32_t dynamic_segmentation;     /* 1 */
     int32_t rough_constraints_far_away; /* 0: p[b] = n[b]; 1: p[b] = states with s < precise_planning_length */
     int32_t constraint_end_heading;   /* 1 */
-    int32_t reserved;
+    int32_t smoothing_method;         /* PQP_PLAN_SMOOTH_*: the reference's --smoothing_method (0 = TENSION2);
+                                         any other value makes pqp_plan_create fail with PQP_E_INVALID */
 } pqp_plan_params;
+
+/* pqp_plan_params.smoothing_method (planning_flags.cpp:27-32, reference_path_smoother.cpp:17-29) */
+enum {
+    PQP_PLAN_SMOOTH_TENSION2 = 0, /* TensionSmoother2: Frenet-style QP over x, y, heading, curvature (default) */
+    PQP_PLAN_SMOOTH_TENSION = 1   /* TensionSmoother: Cartesian QP over x, y and a lateral shift bounded by the map's
+                                     obstacle distance at each resampled point (one more kernel per call; p_max <= 877
+                                     on an H100, checked by pqp_plan_create) */
+};
 
 /* Inputs. Host pointers for pqp_plan, device pointers for pqp_plan_device. */
 typedef struct pqp_plan_in {
@@ -114,6 +124,8 @@ typedef struct pqp_plan_trace {
     int32_t *status1, *iters1;
     double *x_full1, *y_full1, *z_full1; /* as pqp_batch_out, first solve */
     double *x_full2, *y_full2, *z_full2; /* second solve */
+    double *tension_clearance; /* [b][P] obstacle distance at the seg_x / seg_y points (TENSION only; untouched
+                                  under TENSION2) */
 } pqp_plan_trace;
 
 typedef struct pqp_plan_out {

@@ -13,8 +13,10 @@
 #include <string>
 
 #include "../../include/pqp_plan.h"
+#include "pqp_bounds_internal.h"
 #include "pqp_device_guard.h"
 #include "pqp_plan_core.cuh"
+#include "pqp_smoother_internal.h"
 
 namespace {
 
@@ -94,6 +96,18 @@ __global__ void segment_kernel(Dims d, const double *__restrict__ raw_rows, cons
     sa_[o] = a;
     sk_[o] = k;
     ss_[o] = s;
+}
+
+// TENSION only: Map::getObstacleDistance at each resampled point (tension_smoother.cpp:166-168), the clearance of the
+// Cartesian tension QP; one thread per (path, point), paths without points (seg_p = 0) skipped
+__global__ void clearance_kernel(Dims d, const pqb::MapView map, const int32_t *__restrict__ seg_p,
+                                 const double *__restrict__ sx_, const double *__restrict__ sy_, double *clearance) {
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (long long)d.B * d.P) return;
+    const int b = (int)(t / d.P), j = (int)(t % d.P);
+    if (j >= seg_p[b]) return;
+    const size_t o = (size_t)b * d.P + j;
+    clearance[o] = pqb::map_distance(map, sx_[o], sy_[o]);
 }
 
 __device__ void write_placeholder(double *rows, int stride, int32_t *k, double *length) {
@@ -327,6 +341,7 @@ struct pqp_plan_handle {
     double *dp_ls = nullptr, *dp_lo = nullptr, *dp_up = nullptr, *dp_vl = nullptr, *dp_ts = nullptr;
     int32_t *post_p = nullptr, *post_status = nullptr, *post_iters = nullptr, *rk = nullptr;
     double *post_off = nullptr, *r_rows = nullptr, *r_len = nullptr, *max_s = nullptr;
+    double *t_clear = nullptr;  // [B][P] clearance of the Cartesian tension QP (TENSION only)
     double *states = nullptr, *curv = nullptr, *bnd = nullptr, *knots = nullptr, *knots2 = nullptr, *inst = nullptr,
            *ref_xyh = nullptr, *xyh = nullptr;
     int32_t *n_states = nullptr, *total = nullptr, *n_valid = nullptr, *n1 = nullptr, *n2 = nullptr, *p = nullptr;
@@ -430,6 +445,7 @@ int copy_trace(pqp_plan_handle *h, const pqp_plan_trace *t, int B, cudaStream_t 
     PQL_T(t->x_full2, h->full[3], b * nv * d);
     PQL_T(t->y_full2, h->full[4], b * m * d);
     PQL_T(t->z_full2, h->full[5], b * m * d);
+    if (h->t_clear) PQL_T(t->tension_clearance, h->t_clear, b * P * d);
 #undef PQL_T
     return PQP_OK;
 }
@@ -449,7 +465,14 @@ int run(pqp_plan_handle *h, const pqp_plan_in *in, const pqp_plan_out *out, cuda
     segment_kernel<<<blocks_for((long long)B * h->P), kThreads, 0, s>>>(d, h->raw_rows, h->raw_k, h->seg_p, h->seg[0],
                                                                          h->seg[1], h->seg[2], h->seg[3], h->seg[4]);
     PQL_LAUNCH(h);
-    {
+    if (h->prm.smoothing_method == PQP_PLAN_SMOOTH_TENSION) {
+        clearance_kernel<<<blocks_for((long long)B * h->P), kThreads, 0, s>>>(d, *pqb::handle_map(h->bounds), h->seg_p,
+                                                                               h->seg[0], h->seg[1], h->t_clear);
+        PQL_LAUNCH(h);
+        pqp_cartesian_tension_in ci = {B, h->P, h->seg_p, h->seg[0], h->seg[1], h->seg[2], h->t_clear};
+        pqp_tension_out to = {h->t_x, h->t_y, h->t_s, h->t_status, h->t_iters, nullptr};
+        PQL_SUB(h, pqp_cartesian_tension_smooth_device(h->tension, &ci, &to, s), pqp_smoother_last_error, h->tension);
+    } else {
         pqp_tension_in ti = {B, h->P, h->seg_p, h->seg[0], h->seg[1], h->seg[2], h->seg[3], h->seg[4]};
         pqp_tension_out to = {h->t_x, h->t_y, h->t_s, h->t_status, h->t_iters, nullptr};
         PQL_SUB(h, pqp_tension_smooth_device(h->tension, &ti, &to, s), pqp_smoother_last_error, h->tension);
@@ -581,7 +604,7 @@ void pqp_plan_default_params(pqp_plan_params *p) {
     p->dynamic_segmentation = 1;
     p->rough_constraints_far_away = 0;
     p->constraint_end_heading = 1;
-    p->reserved = 0;
+    p->smoothing_method = PQP_PLAN_SMOOTH_TENSION2;
 }
 
 const char *pqp_plan_last_error(const pqp_plan_handle *h) { return h ? h->err.c_str() : g_plan_create_error.c_str(); }
@@ -603,6 +626,11 @@ int pqp_plan_create(const pqp_bounds_map *map, const pqp_plan_params *params, in
         delete h;
         return pfail(nullptr, PQP_E_INVALID, "pqp_plan_create: output_spacing must be positive");
     }
+    if (h->prm.smoothing_method != PQP_PLAN_SMOOTH_TENSION2 && h->prm.smoothing_method != PQP_PLAN_SMOOTH_TENSION) {
+        delete h;
+        return pfail(nullptr, PQP_E_INVALID,
+                     "pqp_plan_create: smoothing_method must be PQP_PLAN_SMOOTH_TENSION2 (0) or PQP_PLAN_SMOOTH_TENSION (1)");
+    }
     h->device = device;
     h->R = r_max;
     h->P = p_max;
@@ -620,6 +648,12 @@ int pqp_plan_create(const pqp_bounds_map *map, const pqp_plan_params *params, in
         rc = pqp_smoother_create(&h->prm.smoother, p_max, batch_max, device, &h->tension);
         if (rc == PQP_OK) rc = pqp_smoother_create(&h->prm.smoother, layers_max, batch_max, device, &h->post);
         if (rc != PQP_OK) g_plan_create_error = std::string("pqp_plan_create: ") + pqp_smoother_last_error(nullptr);
+    }
+    if (rc == PQP_OK && h->prm.smoothing_method == PQP_PLAN_SMOOTH_TENSION) {
+        if (const char *why = pqs::cartesian_unavailable(h->tension)) {
+            rc = PQP_E_INVALID;
+            g_plan_create_error = std::string("pqp_plan_create: smoothing_method TENSION: ") + why;
+        }
     }
     if (rc == PQP_OK) {
         rc = pqp_create(&h->prm.solver, n_max, batch_max, device, &h->solver);
@@ -699,6 +733,7 @@ int pqp_plan_create(const pqp_bounds_map *map, const pqp_plan_params *params, in
     if (e == cudaSuccess) e = dalloc(&h->status2, B);
     if (e == cudaSuccess) e = dalloc(&h->iters2, B);
     for (int i = 0; i < 6 && e == cudaSuccess; ++i) e = dalloc(&h->full[i], B * (i % 3 == 0 ? 6 * N - 1 : 6 * N + 2));
+    if (e == cudaSuccess && h->prm.smoothing_method == PQP_PLAN_SMOOTH_TENSION) e = dalloc(&h->t_clear, B * P);
     // spline rows are zero beyond each path's k, so every row read past the end of a fit is defined
     if (e == cudaSuccess) e = cudaMemset(h->raw_rows, 0, B * S * R * sizeof(double));
     if (e == cudaSuccess) e = cudaMemset(h->t_rows, 0, B * S * P * sizeof(double));
@@ -729,7 +764,7 @@ void pqp_plan_destroy(pqp_plan_handle *h) {
                         h->states, h->curv, h->bnd, h->knots, h->knots2, h->inst, h->ref_xyh, h->xyh, h->n_states,
                         h->total, h->n_valid, h->n1, h->n2, h->p, h->sol1, h->sol2, h->cost1, h->cost2, h->status1,
                         h->iters1, h->status2, h->iters2, h->full[0], h->full[1], h->full[2], h->full[3], h->full[4],
-                        h->full[5]};
+                        h->full[5], h->t_clear};
         for (void *p : bufs) cudaFree(p);
         for (cudaEvent_t ev : h->ev)
             if (ev) cudaEventDestroy(ev);

@@ -1,4 +1,4 @@
-// pqp_smoother.cu — include/pqp_smoother.h: the two smoother QPs of the reference's front end on the GPU.
+// pqp_smoother.cu — include/pqp_smoother.h: the three smoother QPs of the reference's front end on the GPU.
 // One warp (= one CTA) per QP runs pqp_smoother_core.cuh (OSQP on a stage-banded QP, FP64). The serial part of an
 // iteration is the banded forward / backward substitution, so its band factor and right-hand side live in shared
 // memory; everything else (problem data, iterates) is per-CTA scratch in global memory that stays in L1/L2. A grid
@@ -11,6 +11,7 @@
 #include "../../include/pqp_smoother.h"
 #include "pqp_device_guard.h"
 #include "pqp_smoother_core.cuh"
+#include "pqp_smoother_internal.h"
 
 namespace {
 
@@ -78,12 +79,55 @@ __global__ void __launch_bounds__(32) smoother_kernel(const KArgs a) {
     }
 }
 
+struct CArgs {
+    int batch, p_max;
+    pqs::Settings st;
+    pqs::CartesianWeights cw;
+    const int32_t *p;
+    const double *x, *y, *angle, *clearance;
+    double *ox, *oy, *os, *x_full;
+    int32_t *status, *iters;
+    unsigned char *scratch;
+    size_t scratch_stride;
+};
+
+// TensionSmoother::osqpSmooth: the same solver at half-bandwidth 9, so its own kernel (band in shared memory:
+// (3 p_max + 9) * 11 doubles). The minimum of one block per SM lets ptxas keep the wider band loops in registers
+// (191, no spills, CUDA 12.9) instead of capping at 168 with spills; shared memory bounds the residency anyway.
+__global__ void __launch_bounds__(32, 1) cartesian_kernel(const CArgs a) {
+    extern __shared__ __align__(16) double band[];
+    pqs::Work W;
+    pqs::cartesian_carve(W, a.scratch + (size_t)blockIdx.x * a.scratch_stride, a.p_max, band);
+    const WarpLane c;
+    for (int b = blockIdx.x; b < a.batch; b += gridDim.x) {
+        const int p = a.p[b];
+        const size_t o = (size_t)b * a.p_max;
+        if (p < 3 || p > a.p_max) {
+            if (threadIdx.x == 0) { a.status[b] = pqs::kNumerical; a.iters[b] = 0; }
+            continue;
+        }
+        const pqs::Result R = pqs::cartesian_tension_smooth(c, W, a.st, a.cw, p, a.x + o, a.y + o, a.angle + o, a.clearance + o,
+                                                            a.ox + o, a.oy + o, a.os + o,
+                                                            a.x_full ? a.x_full + (size_t)b * 3 * a.p_max : nullptr);
+        if (threadIdx.x == 0) {
+            a.status[b] = R.status;
+            a.iters[b] = R.iters;
+        }
+        __syncwarp();
+    }
+}
+
 }  // namespace
 
 struct pqp_smoother_handle {
     pqp_smoother_params prm{};
     int device = 0, p_max = 0, batch_max = 0, grid_max = 0;
-    size_t scratch_stride = 0, smem = 0;
+    size_t scratch_stride = 0, smem = 0, scratch_total = 0;
+    // Cartesian tension QP: its own working-set size, band and resident-CTA count; cart_err is set when p_max is
+    // beyond its shared-memory limit (the other calls are unaffected)
+    int cart_grid_max = 0;
+    size_t cart_stride = 0, cart_smem = 0;
+    std::string cart_err;
     unsigned char *d_scratch = nullptr;
     cudaStream_t stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
@@ -138,12 +182,41 @@ int launch(pqp_smoother_handle *h, KArgs &a, cudaStream_t s) {
     return PQP_OK;
 }
 
+int launch_cartesian(pqp_smoother_handle *h, CArgs &a, cudaStream_t s) {
+    a.p_max = h->p_max;
+    a.st = settings_of(h->prm);
+    a.cw = {h->prm.cartesian_curvature_weight, h->prm.cartesian_curvature_rate_weight, h->prm.cartesian_deviation_weight};
+    a.scratch = h->d_scratch;
+    a.scratch_stride = h->cart_stride;
+    const int grid = a.batch < h->cart_grid_max ? a.batch : h->cart_grid_max;
+    PQS_CUDA(h, cudaFuncSetAttribute(cartesian_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->cart_smem));
+    PQS_CUDA(h, cudaEventRecord(h->ev0, s));
+    cartesian_kernel<<<grid, 32, h->cart_smem, s>>>(a);
+    PQS_CUDA(h, cudaGetLastError());
+    PQS_CUDA(h, cudaEventRecord(h->ev1, s));
+    return PQP_OK;
+}
+
+int check_cartesian(pqp_smoother_handle *h, const pqp_cartesian_tension_in *in, const pqp_tension_out *out) {
+    if (!h) return PQP_E_INVALID;
+    if (!h->cart_err.empty()) return sfail(h, PQP_E_INVALID, h->cart_err.c_str());
+    if (!in || !out || !in->p || !in->x || !in->y || !in->angle || !in->clearance || !out->x || !out->y || !out->s ||
+        !out->status || !out->iters)
+        return sfail(h, PQP_E_INVALID, "null buffer");
+    if (in->batch < 1 || in->batch > h->batch_max || in->p_max != h->p_max) return sfail(h, PQP_E_INVALID, "batch / p_max do not fit the handle");
+    return PQP_OK;
+}
+
 template <typename T>
 cudaError_t dalloc(T **p, size_t n) {
     return cudaMalloc(reinterpret_cast<void **>(p), (n ? n : 1) * sizeof(T));
 }
 
 }  // namespace
+
+const char *pqs::cartesian_unavailable(const pqp_smoother_handle *h) {
+    return (h && !h->cart_err.empty()) ? h->cart_err.c_str() : nullptr;
+}
 
 extern "C" {
 
@@ -169,6 +242,9 @@ void pqp_smoother_default_params(pqp_smoother_params *p) {
     p->adaptive_rho = 1;
     p->adaptive_rho_interval = 25;
     p->reserved = 0;
+    p->cartesian_curvature_weight = 1.0;
+    p->cartesian_curvature_rate_weight = 50.0;
+    p->cartesian_deviation_weight = 0.0;
 }
 
 const char *pqp_smoother_last_error(const pqp_smoother_handle *h) { return h ? h->err.c_str() : g_smoother_create_error.c_str(); }
@@ -208,8 +284,31 @@ int pqp_smoother_create(const pqp_smoother_params *params, int32_t p_max, int32_
     if (per_sm > 16) per_sm = 16;
     h->grid_max = prop.multiProcessorCount * per_sm;
     if (h->grid_max > batch_max) h->grid_max = batch_max;
+    // the Cartesian QP's band is wider: beyond its limit only the Cartesian calls are refused
+    h->cart_stride = pqs::cartesian_scratch_bytes(p_max);
+    h->cart_smem = pqs::cartesian_band_doubles(p_max) * sizeof(double);
+    if (e == cudaSuccess && h->cart_smem > (size_t)prop.sharedMemPerBlockOptin) {
+        h->cart_err = "pqp_cartesian_tension_smooth: p_max = " + std::to_string(p_max) +
+                      " too large for the Cartesian QP's shared-memory band ((3 p_max + 9) * 11 doubles = " +
+                      std::to_string(h->cart_smem) + " bytes, the device allows " +
+                      std::to_string((size_t)prop.sharedMemPerBlockOptin) + " per block)";
+    } else if (e == cudaSuccess) {
+        e = cudaFuncSetAttribute(cartesian_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->cart_smem);
+        int cart_per_sm = 1;
+        if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cart_per_sm, cartesian_kernel, 32, h->cart_smem);
+        if (cart_per_sm < 1) cart_per_sm = 1;
+        if (cart_per_sm > 16) cart_per_sm = 16;
+        h->cart_grid_max = prop.multiProcessorCount * cart_per_sm;
+        if (h->cart_grid_max > batch_max) h->cart_grid_max = batch_max;
+    }
+    // one scratch block serves both working-set shapes: the Cartesian grid is capped by how many of its (larger)
+    // working sets fit, and the block holds at least one
+    h->scratch_total = (size_t)h->grid_max * h->scratch_stride;
+    if (h->cart_err.empty() && h->scratch_total < h->cart_stride) h->scratch_total = h->cart_stride;
+    if (h->cart_err.empty() && (size_t)h->cart_grid_max > h->scratch_total / h->cart_stride)
+        h->cart_grid_max = (int)(h->scratch_total / h->cart_stride);
     const size_t B = batch_max, Ls = B * p_max;
-    if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void **>(&h->d_scratch), (size_t)h->grid_max * h->scratch_stride);
+    if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void **>(&h->d_scratch), h->scratch_total);
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking);
     if (e == cudaSuccess) e = cudaEventCreate(&h->ev0);
     if (e == cudaSuccess) e = cudaEventCreate(&h->ev1);
@@ -278,6 +377,49 @@ int pqp_post_smooth_device(pqp_smoother_handle *h, const pqp_post_in *in, const 
     a.status = out->status;
     a.iters = out->iters;
     return launch(h, a, static_cast<cudaStream_t>(stream));
+}
+
+int pqp_cartesian_tension_smooth_device(pqp_smoother_handle *h, const pqp_cartesian_tension_in *in,
+                                        const pqp_tension_out *out, void *stream) {
+    const int rc = check_cartesian(h, in, out);
+    if (rc != PQP_OK) return rc;
+    pqp::DeviceGuard guard_(h->device);
+    CArgs a{};
+    a.batch = in->batch;
+    a.p = in->p;
+    a.x = in->x; a.y = in->y; a.angle = in->angle; a.clearance = in->clearance;
+    a.ox = out->x; a.oy = out->y; a.os = out->s;
+    a.x_full = out->x_full;
+    a.status = out->status;
+    a.iters = out->iters;
+    return launch_cartesian(h, a, static_cast<cudaStream_t>(stream));
+}
+
+int pqp_cartesian_tension_smooth(pqp_smoother_handle *h, const pqp_cartesian_tension_in *in, const pqp_tension_out *out) {
+    int rc = check_cartesian(h, in, out);
+    if (rc != PQP_OK) return rc;
+    for (int b = 0; b < in->batch; ++b)
+        if (in->p[b] < 3 || in->p[b] > in->p_max) return sfail(h, PQP_E_INVALID, "p[b] must be in [3, p_max]");
+    pqp::DeviceGuard guard_(h->device);
+    cudaStream_t s = h->stream;
+    const size_t B = in->batch, Ls = B * h->p_max;
+    const double *src[4] = {in->x, in->y, in->angle, in->clearance};
+    for (int i = 0; i < 4; ++i) PQS_CUDA(h, cudaMemcpyAsync(h->d_in[i], src[i], Ls * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQS_CUDA(h, cudaMemcpyAsync(h->d_p, in->p, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    for (int i = 0; i < 3; ++i) PQS_CUDA(h, cudaMemsetAsync(h->d_out[i], 0, Ls * sizeof(double), s));
+    if (out->x_full) PQS_CUDA(h, cudaMemsetAsync(h->d_xfull, 0, Ls * 3 * sizeof(double), s));
+    pqp_cartesian_tension_in din = {in->batch, in->p_max, h->d_p, h->d_in[0], h->d_in[1], h->d_in[2], h->d_in[3]};
+    pqp_tension_out dout = {h->d_out[0], h->d_out[1], h->d_out[2], h->d_status, h->d_iters, out->x_full ? h->d_xfull : nullptr};
+    rc = pqp_cartesian_tension_smooth_device(h, &din, &dout, s);
+    if (rc != PQP_OK) return rc;
+    double *dst[3] = {out->x, out->y, out->s};
+    for (int i = 0; i < 3; ++i) PQS_CUDA(h, cudaMemcpyAsync(dst[i], h->d_out[i], Ls * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PQS_CUDA(h, cudaMemcpyAsync(out->status, h->d_status, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    PQS_CUDA(h, cudaMemcpyAsync(out->iters, h->d_iters, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    if (out->x_full) PQS_CUDA(h, cudaMemcpyAsync(out->x_full, h->d_xfull, Ls * 3 * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PQS_CUDA(h, cudaStreamSynchronize(s));
+    PQS_CUDA(h, cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1));
+    return PQP_OK;
 }
 
 int pqp_tension_smooth(pqp_smoother_handle *h, const pqp_tension_in *in, const pqp_tension_out *out) {

@@ -1,13 +1,16 @@
-// pqp_smoother_core.cuh — the two QPs of the reference's front end (SURVEY.md §8 row f-3) through one
+// pqp_smoother_core.cuh — the three QPs of the reference's front end (SURVEY.md §8 row f-3) through one
 // OSQP-style ADMM routine for small stage-banded QPs, FP64, one warp per QP:
 //   TensionSmoother2::osqpSmooth   /root/reference/src/reference_path_smoother/tension_smoother_2.cpp:20-158
+//   TensionSmoother::osqpSmooth    src/reference_path_smoother/tension_smoother.cpp:49-177 (Cartesian tension)
 //   ReferencePathSmoother::postSmooth (its QP)  src/reference_path_smoother/reference_path_smoother.cpp:526-636
-// Both hand OSQP (defaults, eps 1e-3: only verbosity and warm start are set, :33-34 / :533-534) a QP whose
-// variables can be ordered stage by stage so that P + sigma I + A' diag(rho) A is banded (half-bandwidth 4) and
-// every row / column of A has at most 4 entries. The routine below is OSQP 0.6.x on such a QP - Ruiz equilibration
-// with cost scaling, rho vector, relaxed ADMM step with the x-update done on the reduced banded system (banded
-// LDL', refactored on rho updates), unscaled termination test, primal / dual infeasibility certificates, adaptive
-// rho - i.e. the algorithm of oracle/osqp_generic.py, which is the oracle of this row.
+// All hand OSQP (defaults, eps 1e-3: only verbosity and warm start are set, :33-34 / :62-63 / :533-534) a QP whose
+// variables can be ordered stage by stage so that P + sigma I + A' diag(rho) A is banded (half-bandwidth 4 for
+// TENSION2 and post, 9 for the Cartesian QP) and every row / column of A has at most 4 entries. The routine below is
+// OSQP 0.6.x on such a QP - Ruiz equilibration with cost scaling, rho vector, relaxed ADMM step with the x-update
+// done on the reduced banded system (banded LDL', refactored on rho updates), unscaled termination test, primal /
+// dual infeasibility certificates, adaptive rho - i.e. the algorithm of oracle/osqp_generic.py, which is the oracle
+// of this row. The half-bandwidths of the reduced matrix (HB) and of P (HBP) are template parameters of the band
+// routines.
 //
 // One templated routine over a warp context: the CUDA kernel (pqp_smoother.cu) and the CPU test driver
 // (tests/emu/smoother_driver.cpp, 1 "lane") compile this same source.
@@ -24,9 +27,10 @@
 
 namespace pqs {
 
-constexpr int kHB = 4;    // half-bandwidth of the reduced matrix (both QPs: entries of a row lie within 4 columns)
-constexpr int kHBP = 4;   // half-bandwidth of P
-constexpr int kEll = 4;   // entries per row / column of A
+constexpr int kHB = 4;    // half-bandwidth of the reduced matrix (TENSION2, post: entries of a row lie within 4 columns)
+constexpr int kHBP = 4;   // half-bandwidth of P (TENSION2, post)
+constexpr int kHBC = 9;   // Cartesian tension QP: half-bandwidth of P and of the reduced matrix (x_i .. x_{i+3})
+constexpr int kEll = 4;   // entries per row / column of A (all three QPs)
 
 struct Settings {  // OSQP settings (defaults = OSQP 0.6.x defaults; the reference overrides none of them here)
     double rho, sigma, alpha, eps_abs, eps_rel, eps_prim_inf, eps_dual_inf, adaptive_rho_tolerance;
@@ -35,6 +39,7 @@ struct Settings {  // OSQP settings (defaults = OSQP 0.6.x defaults; the referen
 
 struct TensionWeights { double deviation, curvature, curvature_rate; };  // planning_flags.cpp:57-61: 0.005, 1, 10
 struct PostWeights { double x, dx, ddx; };                               // reference_path_smoother.cpp:590-592: 1, 100, 1000
+struct CartesianWeights { double curvature, curvature_rate, deviation; }; // planning_flags.cpp:51-55: 1, 50, 0
 
 // status codes as in include/pqp.h
 enum { kSolved = 0, kMaxIter = 1, kPrimInf = 2, kDualInf = 3, kSolvedInacc = 4, kPrimInfInacc = 5, kDualInfInacc = 6, kNumerical = 7 };
@@ -42,8 +47,8 @@ enum { kSolved = 0, kMaxIter = 1, kPrimInf = 2, kDualInf = 3, kSolvedInacc = 4, 
 // Working set of one QP (pointers into the CTA's scratch; `Lb`, `w` may be shared memory)
 struct Work {
     int N, M;            // variables, rows
-    int Np;              // N padded for the band arrays (N + kHB)
-    double *Pb;          // [Np][kHBP+1]  P(j, j+d), upper band, scaled in place
+    int Np;              // N padded for the band arrays (N + HB)
+    double *Pb;          // [Np][HBP+1]  P(j, j+d), upper band, scaled in place
     double *q;           // [N]
     double *Av;          // [M][kEll] values, row-ELL
     int16_t *Ac;         // [M][kEll] columns (-1 = empty)
@@ -57,7 +62,7 @@ struct Work {
     double *x, *z, *y;   // iterates (scaled)
     double *xp;          // [N] previous x (delta_x for the dual certificate)
     double *dy;          // [M] delta_y
-    double *Lb;          // [Np][kHB+1] band of the reduced matrix -> its LDL' (d in [.][0], L(j+i, j) in [.][i])
+    double *Lb;          // [Np][HB+1] band of the reduced matrix -> its LDL' (d in [.][0], L(j+i, j) in [.][i])
     double *w;           // [Np] rhs / solution of the reduced solve
     double *t1, *t2;     // [max(N, M)] temporaries
     double c, rho;
@@ -189,6 +194,69 @@ PQS_HD void assemble_post(const Ctx &c, Work &W, int p, const double *layer_s, c
     c.sync();
 }
 
+// TensionSmoother (tension_smoother.cpp:102-177), variables interleaved per point: x_i, y_i, d_i at 3 i .. 3 i + 2
+// (d_i: lateral shift of point i); rows per point: 3 i (x_i - cos(theta_i) d_i = x_list_i), 3 i + 1 (the same in y),
+// 3 i + 2 (d_i in its clearance range), theta_i = angle_i + pi / 2. P couples x_i with x_{i+3}: half-bandwidth 9.
+// Each entry of P is the sum of the dense blocks that cover it, added in the reference's order (block i ascending,
+// the curvature block before the curvature-rate block); P(d_i, d_i) is set, not added.
+constexpr double kCartesianDefaultClearance = 2.0;  // tension_smoother.cpp:163
+PQS_HD double dds_coef(int k) { return k == 1 ? -2.0 : 1.0; }                                         // [1 -2 1]
+PQS_HD double ddds_coef(int k) { return k == 0 ? -1.0 : (k == 1 ? 3.0 : (k == 2 ? -3.0 : 1.0)); }    // [-1 3 -3 1]
+template <class Ctx>
+PQS_HD void assemble_cartesian(const Ctx &c, Work &W, int p, const double *xl, const double *yl, const double *al,
+                               const double *cl, const CartesianWeights &cw) {
+    constexpr int S = kHBC + 1;  // row stride of the P band
+    const int N = 3 * p, M = 3 * p;
+    W.N = N;
+    W.M = M;
+    for (int j = c.lane(); j < W.Np * S; j += c.lanes()) W.Pb[j] = 0.0;
+    for (int r = c.lane(); r < M * kEll; r += c.lanes()) {
+        W.Av[r] = 0.0;
+        W.Ac[r] = -1;
+    }
+    c.sync();
+    for (int j = c.lane(); j < p; j += c.lanes()) {
+        // P(x_j, x_{j+e}) = P(y_j, y_{j+e}), 3 e columns apart
+        for (int e = 0; e <= 3 && j + e < p; ++e) {
+            double s = 0.0;
+            for (int i = (j + e - 3 > 0 ? j + e - 3 : 0); i <= j; ++i) {
+                if (i <= p - 3 && j + e <= i + 2) s += dds_coef(j - i) * dds_coef(j + e - i) * cw.curvature;
+                if (i <= p - 4) s += ddds_coef(j - i) * ddds_coef(j + e - i) * cw.curvature_rate;   // the i != size - 3 rule
+            }
+            W.Pb[(size_t)(3 * j) * S + 3 * e] = s;
+            W.Pb[(size_t)(3 * j + 1) * S + 3 * e] = s;
+        }
+        W.Pb[(size_t)(3 * j + 2) * S] = cw.deviation;
+        W.q[3 * j] = W.q[3 * j + 1] = W.q[3 * j + 2] = 0.0;
+        const double theta = al[j] + M_PI_2;
+        int r = 3 * j;
+        W.Ac[r * kEll + 0] = (int16_t)(3 * j);      W.Av[r * kEll + 0] = 1;
+        W.Ac[r * kEll + 1] = (int16_t)(3 * j + 2);  W.Av[r * kEll + 1] = -cos(theta);
+        W.l[r] = W.u[r] = xl[j];
+        r = 3 * j + 1;
+        W.Ac[r * kEll + 0] = (int16_t)(3 * j + 1);  W.Av[r * kEll + 0] = 1;
+        W.Ac[r * kEll + 1] = (int16_t)(3 * j + 2);  W.Av[r * kEll + 1] = -sin(theta);
+        W.l[r] = W.u[r] = yl[j];
+        r = 3 * j + 2;
+        W.Ac[r * kEll] = (int16_t)(3 * j + 2);      W.Av[r * kEll] = 1;
+        double lo, hi;
+        if (j == 0) {
+            lo = hi = 0.0;
+        } else if (j == p - 1) {
+            lo = -0.5;
+            hi = 0.5;
+        } else {
+            // std::min(clearance, 2): the clearance unless 2 is smaller (Map::getObstacleDistance, 0 off the map)
+            const double cr = kCartesianDefaultClearance < cl[j] ? kCartesianDefaultClearance : cl[j];
+            lo = -cr;
+            hi = cr;
+        }
+        W.l[r] = lo;
+        W.u[r] = hi;
+    }
+    c.sync();
+}
+
 // column lists of A from the row lists; rows are visited in ascending order, so every column's list is sorted by
 // row and sums over a column always run in the same order (deterministic rounding)
 template <class Ctx>
@@ -235,12 +303,12 @@ template <class Ctx> PQS_HD void mat_tvec_A(const Ctx &c, const Work &W, const d
         out[j] = s;
     }
 }
-template <class Ctx> PQS_HD void mat_vec_P(const Ctx &c, const Work &W, const double *x, double *out) {   // out = P x (symmetric band)
+template <int HBP, class Ctx> PQS_HD void mat_vec_P(const Ctx &c, const Work &W, const double *x, double *out) {   // out = P x (symmetric band)
     for (int j = c.lane(); j < W.N; j += c.lanes()) {
-        double s = W.Pb[(size_t)j * (kHBP + 1)] * x[j];
-        for (int d = 1; d <= kHBP; ++d) {
-            if (j + d < W.N) s += W.Pb[(size_t)j * (kHBP + 1) + d] * x[j + d];
-            if (j - d >= 0) s += W.Pb[(size_t)(j - d) * (kHBP + 1) + d] * x[j - d];
+        double s = W.Pb[(size_t)j * (HBP + 1)] * x[j];
+        for (int d = 1; d <= HBP; ++d) {
+            if (j + d < W.N) s += W.Pb[(size_t)j * (HBP + 1) + d] * x[j + d];
+            if (j - d >= 0) s += W.Pb[(size_t)(j - d) * (HBP + 1) + d] * x[j - d];
         }
         out[j] = s;
     }
@@ -257,7 +325,7 @@ template <class Ctx> PQS_HD double inf_norm_scaled(const Ctx &c, const double *s
 }
 
 // OSQP scale_data (App. B.2) on band-P / ELL-A
-template <class Ctx>
+template <int HBP, class Ctx>
 PQS_HD void scale_data(const Ctx &c, Work &W, int passes) {
     const int N = W.N, M = W.M;
     for (int j = c.lane(); j < N; j += c.lanes()) W.D[j] = 1.0;
@@ -267,10 +335,10 @@ PQS_HD void scale_data(const Ctx &c, Work &W, int passes) {
     for (int pass = 0; pass < passes; ++pass) {
         // column norms of [P; A] -> t1 (Dt), row norms of A -> t2 (Et)
         for (int j = c.lane(); j < N; j += c.lanes()) {
-            double m = dabs(W.Pb[(size_t)j * (kHBP + 1)]);
-            for (int d = 1; d <= kHBP; ++d) {
-                if (j + d < N) m = dmax2(m, dabs(W.Pb[(size_t)j * (kHBP + 1) + d]));
-                if (j - d >= 0) m = dmax2(m, dabs(W.Pb[(size_t)(j - d) * (kHBP + 1) + d]));
+            double m = dabs(W.Pb[(size_t)j * (HBP + 1)]);
+            for (int d = 1; d <= HBP; ++d) {
+                if (j + d < N) m = dmax2(m, dabs(W.Pb[(size_t)j * (HBP + 1) + d]));
+                if (j - d >= 0) m = dmax2(m, dabs(W.Pb[(size_t)(j - d) * (HBP + 1) + d]));
             }
             for (int e = 0; e < kEll; ++e) {
                 const int r = W.Cr[j * kEll + e];
@@ -286,8 +354,8 @@ PQS_HD void scale_data(const Ctx &c, Work &W, int passes) {
         }
         c.sync();
         for (int j = c.lane(); j < N; j += c.lanes()) {
-            for (int d = 0; d <= kHBP; ++d)
-                if (j + d < N) W.Pb[(size_t)j * (kHBP + 1) + d] *= W.t1[j] * W.t1[j + d];
+            for (int d = 0; d <= HBP; ++d)
+                if (j + d < N) W.Pb[(size_t)j * (HBP + 1) + d] *= W.t1[j] * W.t1[j + d];
             W.q[j] *= W.t1[j];
             W.D[j] *= W.t1[j];
         }
@@ -302,10 +370,10 @@ PQS_HD void scale_data(const Ctx &c, Work &W, int passes) {
         // cost scaling: 1 / max(mean column norm of P, |q|_inf), both limited
         double psum = 0.0, qmax = 0.0;
         for (int j = c.lane(); j < N; j += c.lanes()) {
-            double m = dabs(W.Pb[(size_t)j * (kHBP + 1)]);
-            for (int d = 1; d <= kHBP; ++d) {
-                if (j + d < N) m = dmax2(m, dabs(W.Pb[(size_t)j * (kHBP + 1) + d]));
-                if (j - d >= 0) m = dmax2(m, dabs(W.Pb[(size_t)(j - d) * (kHBP + 1) + d]));
+            double m = dabs(W.Pb[(size_t)j * (HBP + 1)]);
+            for (int d = 1; d <= HBP; ++d) {
+                if (j + d < N) m = dmax2(m, dabs(W.Pb[(size_t)j * (HBP + 1) + d]));
+                if (j - d >= 0) m = dmax2(m, dabs(W.Pb[(size_t)(j - d) * (HBP + 1) + d]));
             }
             psum += m;
             qmax = dmax2(qmax, dabs(W.q[j]));
@@ -315,7 +383,7 @@ PQS_HD void scale_data(const Ctx &c, Work &W, int passes) {
         double ct = dmax2(psum / N, lim_scaling(qmax));
         ct = 1.0 / lim_scaling(ct);
         for (int j = c.lane(); j < N; j += c.lanes()) {
-            for (int d = 0; d <= kHBP; ++d) W.Pb[(size_t)j * (kHBP + 1) + d] *= ct;
+            for (int d = 0; d <= HBP; ++d) W.Pb[(size_t)j * (HBP + 1) + d] *= ct;
             W.q[j] *= ct;
         }
         cs *= ct;
@@ -342,17 +410,18 @@ PQS_HD void set_rho_vec(const Ctx &c, Work &W, bool classify) {
 }
 
 // band of P + sigma I + A' diag(rho) A, then LDL' in place; false on a non-positive pivot
-template <class Ctx>
+template <int HB, int HBP, class Ctx>
 PQS_HD bool factor(const Ctx &c, Work &W, double sigma) {
+    static_assert(HBP <= HB, "the band of P lies inside the band of the reduced matrix");
     const int N = W.N;
     for (int j = c.lane(); j < W.Np; j += c.lanes()) {
-        double *row = W.Lb + (size_t)j * (kHB + 1);
-        for (int d = 0; d <= kHB; ++d) row[d] = 0.0;
+        double *row = W.Lb + (size_t)j * (HB + 1);
+        for (int d = 0; d <= HB; ++d) row[d] = 0.0;
         if (j >= N) {
             row[0] = 1.0;  // padding rows: identity
             continue;
         }
-        for (int d = 0; d <= kHBP; ++d) row[d] = W.Pb[(size_t)j * (kHBP + 1) + d];
+        for (int d = 0; d <= HBP; ++d) row[d] = W.Pb[(size_t)j * (HBP + 1) + d];
         row[0] += sigma;
         for (int e = 0; e < kEll; ++e) {
             const int r = W.Cr[j * kEll + e];
@@ -360,46 +429,46 @@ PQS_HD bool factor(const Ctx &c, Work &W, double sigma) {
             const double aj = W.Av[r * kEll + W.Ce[j * kEll + e]] * W.rho_vec[r];
             for (int f = 0; f < kEll; ++f) {
                 const int col = W.Ac[r * kEll + f];
-                if (col >= j && col - j <= kHB) row[col - j] += aj * W.Av[r * kEll + f];
+                if (col >= j && col - j <= HB) row[col - j] += aj * W.Av[r * kEll + f];
             }
         }
     }
     c.sync();
     int ok = 1;
     for (int j = 0; j < N; ++j) {
-        double *row = W.Lb + (size_t)j * (kHB + 1);
+        double *row = W.Lb + (size_t)j * (HB + 1);
         const double dj = row[0];
         if (!(dj > 0.0)) ok = 0;
-        // lanes a = 1 .. kHB update row j + a with the multipliers of column j
-        for (int a = 1 + c.lane(); a <= kHB; a += c.lanes()) {
+        // lanes a = 1 .. HB update row j + a with the multipliers of column j
+        for (int a = 1 + c.lane(); a <= HB; a += c.lanes()) {
             const double la = row[a] / dj;
-            double *ra = W.Lb + (size_t)(j + a) * (kHB + 1);
-            for (int b = a; b <= kHB; ++b) ra[b - a] -= la * row[b];
+            double *ra = W.Lb + (size_t)(j + a) * (HB + 1);
+            for (int b = a; b <= HB; ++b) ra[b - a] -= la * row[b];
         }
         c.sync();
-        for (int a = 1 + c.lane(); a <= kHB; a += c.lanes()) row[a] /= dj;
+        for (int a = 1 + c.lane(); a <= HB; a += c.lanes()) row[a] /= dj;
         c.sync();
     }
     return c.all(ok) != 0;
 }
 
 // solve (LDL') w = w in place
-template <class Ctx>
+template <int HB, class Ctx>
 PQS_HD void band_solve(const Ctx &c, Work &W) {
     const int N = W.N;
     for (int j = 0; j < N; ++j) {
         const double bj = W.w[j];
-        const double *row = W.Lb + (size_t)j * (kHB + 1);
-        for (int i = 1 + c.lane(); i <= kHB; i += c.lanes()) W.w[j + i] -= row[i] * bj;
+        const double *row = W.Lb + (size_t)j * (HB + 1);
+        for (int i = 1 + c.lane(); i <= HB; i += c.lanes()) W.w[j + i] -= row[i] * bj;
         c.sync();
     }
-    for (int j = c.lane(); j < N; j += c.lanes()) W.w[j] /= W.Lb[(size_t)j * (kHB + 1)];
+    for (int j = c.lane(); j < N; j += c.lanes()) W.w[j] /= W.Lb[(size_t)j * (HB + 1)];
     c.sync();
     for (int j = N - 1; j >= 0; --j) {
-        const double *row = W.Lb + (size_t)j * (kHB + 1);
+        const double *row = W.Lb + (size_t)j * (HB + 1);
         if (c.lane() == 0) {
             double s = 0.0;
-            for (int i = 1; i <= kHB; ++i) s += row[i] * W.w[j + i];
+            for (int i = 1; i <= HB; ++i) s += row[i] * W.w[j + i];
             W.w[j] -= s;
         }
         c.sync();
@@ -408,23 +477,24 @@ PQS_HD void band_solve(const Ctx &c, Work &W) {
 
 struct Result { int status, iters, rho_updates; double pri_res, dua_res, obj; };
 
-// Sizes for a handle that holds QPs of up to p_max points / layers (tension: N = 4 p - 1, M = 3 p - 1; post: N = 3 p,
-// M = 3 p - 2), and the carving of one QP's working set out of a flat scratch block (8-byte aligned).
-PQS_HD int n_max_of(int p_max) { return 4 * p_max; }
-PQS_HD int m_max_of(int p_max) { return 3 * p_max + 2; }
-PQS_HD size_t band_doubles(int p_max) { return (size_t)(n_max_of(p_max) + kHB) * (kHB + 1) + (size_t)(n_max_of(p_max) + kHB); }  // Lb + w
-PQS_HD size_t scratch_bytes(int p_max) {
-    const size_t N = n_max_of(p_max), M = m_max_of(p_max), Np = N + kHB;
-    size_t d = Np * (kHBP + 1) + N /*q*/ + M * kEll /*Av*/ + 2 * M /*l,u*/ + N + M /*D,E*/ + M /*rho*/ + N + 2 * M /*x,z,y*/ + N /*xp*/ +
+// Sizes of a working set for QPs of up to n_max variables and m_max rows, and the carving of one QP's working set
+// out of a flat scratch block (8-byte aligned) plus its band block (Lb + w, shared memory in the kernel).
+template <int HB>
+PQS_HD size_t band_doubles(int n_max) { return (size_t)(n_max + HB) * (HB + 1) + (size_t)(n_max + HB); }  // Lb + w
+template <int HB, int HBP>
+PQS_HD size_t scratch_bytes(int n_max, int m_max) {
+    const size_t N = n_max, M = m_max, Np = N + HB;
+    size_t d = Np * (HBP + 1) + N /*q*/ + M * kEll /*Av*/ + 2 * M /*l,u*/ + N + M /*D,E*/ + M /*rho*/ + N + 2 * M /*x,z,y*/ + N /*xp*/ +
                M /*dy*/ + 2 * (N > M ? N : M) /*t1,t2*/;
     size_t b = d * sizeof(double) + (M * kEll + N * kEll) * sizeof(int16_t) + (N * kEll + N + M) * sizeof(int8_t);
     return (b + 15) & ~(size_t)15;
 }
-PQS_HD void carve(Work &W, unsigned char *base, int p_max, double *band) {
-    const size_t N = n_max_of(p_max), M = m_max_of(p_max), Np = N + kHB, T = N > M ? N : M;
+template <int HB, int HBP>
+PQS_HD void carve(Work &W, unsigned char *base, int n_max, int m_max, double *band) {
+    const size_t N = n_max, M = m_max, Np = N + HB, T = N > M ? N : M;
     W.Np = (int)Np;
     double *d = reinterpret_cast<double *>(base);
-    W.Pb = d; d += Np * (kHBP + 1);
+    W.Pb = d; d += Np * (HBP + 1);
     W.q = d; d += N;
     W.Av = d; d += M * kEll;
     W.l = d; d += M;
@@ -447,11 +517,26 @@ PQS_HD void carve(Work &W, unsigned char *base, int p_max, double *band) {
     W.cnt = b; b += N;
     W.ctype = b;
     W.Lb = band;
-    W.w = band + Np * (kHB + 1);
+    W.w = band + Np * (HB + 1);
+}
+
+// The two handle shapes. TENSION2 and post (bandwidth 4) share one working set of p_max points / layers (tension:
+// N = 4 p - 1, M = 3 p - 1; post: N = 3 p, M = 3 p - 2); the Cartesian QP (bandwidth 9) has N = M = 3 p.
+PQS_HD int n_max_of(int p_max) { return 4 * p_max; }
+PQS_HD int m_max_of(int p_max) { return 3 * p_max + 2; }
+PQS_HD size_t band_doubles(int p_max) { return band_doubles<kHB>(n_max_of(p_max)); }
+PQS_HD size_t scratch_bytes(int p_max) { return scratch_bytes<kHB, kHBP>(n_max_of(p_max), m_max_of(p_max)); }
+PQS_HD void carve(Work &W, unsigned char *base, int p_max, double *band) {
+    carve<kHB, kHBP>(W, base, n_max_of(p_max), m_max_of(p_max), band);
+}
+PQS_HD size_t cartesian_band_doubles(int p_max) { return band_doubles<kHBC>(3 * p_max); }
+PQS_HD size_t cartesian_scratch_bytes(int p_max) { return scratch_bytes<kHBC, kHBC>(3 * p_max, 3 * p_max); }
+PQS_HD void cartesian_carve(Work &W, unsigned char *base, int p_max, double *band) {
+    carve<kHBC, kHBC>(W, base, 3 * p_max, 3 * p_max, band);
 }
 
 // OSQP on the assembled working set (cold start). Follows oracle/osqp_generic.py step for step.
-template <class Ctx>
+template <int HB, int HBP, class Ctx>
 PQS_HD Result solve(const Ctx &c, Work &W, const Settings &st) {
     const int N = W.N, M = W.M;
     Result R;
@@ -460,7 +545,7 @@ PQS_HD Result solve(const Ctx &c, Work &W, const Settings &st) {
     R.rho_updates = 0;
     R.pri_res = R.dua_res = R.obj = 0.0;
     build_columns(c, W);
-    scale_data(c, W, st.scaling);
+    scale_data<HBP>(c, W, st.scaling);
     W.rho = dmin2(dmax2(st.rho, 1e-6), 1e6);
     set_rho_vec(c, W, true);
     for (int j = c.lane(); j < W.Np; j += c.lanes()) {
@@ -469,7 +554,7 @@ PQS_HD Result solve(const Ctx &c, Work &W, const Settings &st) {
     }
     for (int r = c.lane(); r < M; r += c.lanes()) W.z[r] = W.y[r] = W.dy[r] = 0.0;
     c.sync();
-    if (!factor(c, W, st.sigma)) {
+    if (!factor<HB, HBP>(c, W, st.sigma)) {
         R.status = kNumerical;
         return R;
     }
@@ -489,7 +574,7 @@ PQS_HD Result solve(const Ctx &c, Work &W, const Settings &st) {
             W.w[j] = st.sigma * W.x[j] - W.q[j] + W.t1[j];
         }
         c.sync();
-        band_solve(c, W);                 // w = x~
+        band_solve<HB>(c, W);             // w = x~
         mat_vec_A(c, W, W.w, W.t2);       // t2 = z~ = A x~
         c.sync();
         for (int j = c.lane(); j < N; j += c.lanes()) W.x[j] = st.alpha * W.w[j] + (1.0 - st.alpha) * W.xp[j];
@@ -506,7 +591,7 @@ PQS_HD Result solve(const Ctx &c, Work &W, const Settings &st) {
         if (!(can_check || can_adapt)) continue;
         // ---- info: residuals on unscaled quantities (t1 = P x, t2 = A x; A'y recomputed into w afterwards)
         mat_vec_A(c, W, W.x, W.t2);
-        mat_vec_P(c, W, W.x, W.t1);
+        mat_vec_P<HBP>(c, W, W.x, W.t1);
         c.sync();
         {
             double a = 0, b = 0, d = 0, e = 0, f = 0, g = 0, obj = 0;
@@ -572,7 +657,7 @@ PQS_HD Result solve(const Ctx &c, Work &W, const Settings &st) {
                 qdx = c.sum(qdx);
                 c.sync();
                 if (nrm > st.eps_dual_inf && qdx < -W.c * st.eps_dual_inf * nrm) {
-                    mat_vec_P(c, W, W.w, W.t1);
+                    mat_vec_P<HBP>(c, W, W.w, W.t1);
                     c.sync();
                     if (inf_norm_scaled(c, W.D, W.t1, N, true) < W.c * st.eps_dual_inf * nrm) {
                         mat_vec_A(c, W, W.w, W.t2);
@@ -597,7 +682,7 @@ PQS_HD Result solve(const Ctx &c, Work &W, const Settings &st) {
                 W.rho = est;
                 set_rho_vec(c, W, false);
                 ++R.rho_updates;
-                if (!factor(c, W, st.sigma)) { R.status = kNumerical; break; }
+                if (!factor<HB, HBP>(c, W, st.sigma)) { R.status = kNumerical; break; }
             }
         }
     }
@@ -605,7 +690,8 @@ PQS_HD Result solve(const Ctx &c, Work &W, const Settings &st) {
     if (R.status < 0) {
         // the 10x re-check of osqp_solve after the last iteration on the residuals of the last info (max_iter is
         // a multiple of the check interval with OSQP's defaults). The "inaccurate" infeasibility certificates are not
-        // re-evaluated: both QPs are feasible by construction (dynamics rows + a non-empty corridor).
+        // re-evaluated: the QPs are feasible by construction (dynamics rows + a non-empty corridor; in the Cartesian QP
+        // x_i, y_i absorb any d_i in its range, which contains 0).
         const double ep = 10 * (st.eps_abs + st.eps_rel * dmax2(u_z, u_ax));
         const double ed = 10 * (st.eps_abs + st.eps_rel * cinv * dmax2(u_q, dmax2(u_aty, u_px)));
         R.status = (u_rp < ep && u_rd < ed) ? kSolvedInacc : kMaxIter;
@@ -621,7 +707,7 @@ PQS_HD Result tension_smooth(const Ctx &c, Work &W, const Settings &st, const Te
                              const double *yl, const double *al, const double *kl, const double *sl, double *rx, double *ry,
                              double *rs, double *x_full) {
     assemble_tension(c, W, p, xl, yl, al, kl, sl, tw);
-    const Result R = solve(c, W, st);
+    const Result R = solve<kHB, kHBP>(c, W, st);
     for (int i = c.lane(); i < p; i += c.lanes()) {
         rx[i] = W.D[4 * i] * W.x[4 * i];
         ry[i] = W.D[4 * i + 1] * W.x[4 * i + 1];
@@ -650,7 +736,7 @@ template <class Ctx>
 PQS_HD Result post_smooth(const Ctx &c, Work &W, const Settings &st, const PostWeights &pw, int p, const double *layer_s,
                           const double *lower, const double *upper, double vehicle_l, double *offsets, double *x_full) {
     assemble_post(c, W, p, layer_s, lower, upper, vehicle_l, pw);
-    const Result R = solve(c, W, st);
+    const Result R = solve<kHB, kHBP>(c, W, st);
     for (int i = c.lane(); i < p; i += c.lanes()) {
         offsets[i] = W.D[3 * i] * W.x[3 * i];
         if (x_full) {
@@ -663,5 +749,36 @@ PQS_HD Result post_smooth(const Ctx &c, Work &W, const Settings &st, const PostW
     return R;
 }
 
+// One QP end to end: Cartesian tension smoother (TensionSmoother::osqpSmooth, tension_smoother.cpp:49-100). Inputs:
+// the resampled points, their headings and the obstacle distance at each point (Map::getObstacleDistance; read for
+// the interior points only). Outputs as tension_smooth: result_x / result_y (QPSolution(i), QPSolution(p + i)),
+// result_s re-accumulated from them, optionally the whole primal vector in the reference's index order (x block,
+// y block, d block).
+template <class Ctx>
+PQS_HD Result cartesian_tension_smooth(const Ctx &c, Work &W, const Settings &st, const CartesianWeights &cw, int p,
+                                       const double *xl, const double *yl, const double *al, const double *cl,
+                                       double *rx, double *ry, double *rs, double *x_full) {
+    assemble_cartesian(c, W, p, xl, yl, al, cl, cw);
+    const Result R = solve<kHBC, kHBC>(c, W, st);
+    for (int i = c.lane(); i < p; i += c.lanes()) {
+        rx[i] = W.D[3 * i] * W.x[3 * i];
+        ry[i] = W.D[3 * i + 1] * W.x[3 * i + 1];
+        if (x_full) {
+            x_full[i] = rx[i];
+            x_full[p + i] = ry[i];
+            x_full[2 * p + i] = W.D[3 * i + 2] * W.x[3 * i + 2];
+        }
+    }
+    c.sync();
+    if (c.lane() == 0) {
+        double tmp_s = 0;
+        for (int i = 0; i < p; ++i) {
+            if (i != 0) tmp_s += sqrt(pow(rx[i] - rx[i - 1], 2) + pow(ry[i] - ry[i - 1], 2));
+            rs[i] = tmp_s;
+        }
+    }
+    c.sync();
+    return R;
+}
 
 }  // namespace pqs

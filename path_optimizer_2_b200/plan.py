@@ -17,13 +17,17 @@ STATUS_NAMES = ("OK", "SPLINE_DEGENERATE", "TOO_MANY_POINTS", "TENSION_FAILED", 
  INIT_HEADING, TOO_MANY_KNOTS, BLOCKED_AT_START, PRE_SOLVE_FAILED, SOLVE_FAILED) = range(13)
 PATH_ROWS = ("x", "y", "heading", "k", "d_k", "l", "d_heading")
 STAGES = ("smoothing", "segmentation", "optimisation", "total")
+# PlanParams.smoothing_method: the reference's --smoothing_method
+SMOOTH_TENSION2, SMOOTH_TENSION = 0, 1
+SMOOTHING_METHODS = {"TENSION2": SMOOTH_TENSION2, "TENSION": SMOOTH_TENSION}
 
 
 class PlanParams(C.Structure):
     _fields_ = [("solver", abi.PqpParams), ("bounds", bounds.BoundsParams), ("dp", dp.DpParams),
                 ("smoother", smoother.SmootherParams), ("output_spacing", C.c_double),
                 ("precise_planning_length", C.c_double), ("dynamic_segmentation", C.c_int32),
-                ("rough_constraints_far_away", C.c_int32), ("constraint_end_heading", C.c_int32), ("reserved", C.c_int32)]
+                ("rough_constraints_far_away", C.c_int32), ("constraint_end_heading", C.c_int32),
+                ("smoothing_method", C.c_int32)]
 
 
 class PlanIn(C.Structure):
@@ -58,6 +62,7 @@ _TRACE = [
     ("z_full1", np.float64, lambda P, L, N, R: (6 * N + 2,)),
     ("x_full2", np.float64, lambda P, L, N, R: (6 * N - 1,)), ("y_full2", np.float64, lambda P, L, N, R: (6 * N + 2,)),
     ("z_full2", np.float64, lambda P, L, N, R: (6 * N + 2,)),
+    ("tension_clearance", np.float64, lambda P, L, N, R: (P,)),
 ]
 
 
@@ -89,9 +94,12 @@ def _lib():
     return L
 
 
-def default_params():
+def default_params(smoothing_method=None):
+    """Library defaults; `smoothing_method` ("TENSION2", "TENSION" or SMOOTH_*) overrides the default TENSION2."""
     p = PlanParams()
     _lib().pqp_plan_default_params(C.byref(p))
+    if smoothing_method is not None:
+        p.smoothing_method = SMOOTHING_METHODS.get(smoothing_method, smoothing_method)
     return p
 
 

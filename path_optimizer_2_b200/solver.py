@@ -37,7 +37,7 @@ def build_library(force=False, verbose=False):
     cu = [os.path.join(_CSRC, f) for f in ("pqp_api.cu", "pqp_bounds.cu", "pqp_multi.cu", "pqp_smoother.cu")]
     deps = cu + [os.path.join(_CSRC, f) for f in ("pqp_kernel.cuh", "pqp_host_common.h", "pqp_bounds_core.cuh", "pqp_device_guard.h",
                                                   "pqp_dp.cu", "pqp_dp_core.cuh", "pqp_bounds_internal.h", "pqp_smoother_core.cuh",
-                                                  "pqp_plan.cu", "pqp_plan_core.cuh")]
+                                                  "pqp_plan.cu", "pqp_plan_core.cuh", "pqp_smoother_internal.h")]
     deps += [os.path.join(root, "include", f) for f in ("pqp.h", "pqp_bounds.h", "pqp_multi.h", "pqp_dp.h", "pqp_smoother.h",
                                                         "pqp_plan.h")]
     stale = not os.path.exists(LIB_PATH) or any(
