@@ -4,19 +4,20 @@
  * reference interface replaced:
  *   PathOptimizer::solve                         src/path_optimizer.cpp:34-71
  *     ReferencePathSmoother::solve               src/reference_path_smoother/reference_path_smoother.cpp:17-45
+ *       bSpline() (pqp_plan_points only)          :31-36, :490-524, tools.cpp:46-48
  *       segmentRawReference + s_list_             :47-85, :519-523
  *       TensionSmoother2::osqpSmooth + spline     tension_smoother_2.cpp:20-72, tension_smoother.cpp:36-41
  *       or TensionSmoother::osqpSmooth (TENSION)  tension_smoother.cpp:20-177, clearance Map.cpp:16-22
  *       graphSearchDp, postSmooth                 reference_path_smoother.cpp:142-295, :526-580
  *     processReferencePath                        src/path_optimizer.cpp:73-122, src/tools/tools.cpp:57-126
  *     optimizePath (solve, re-solve, path)        src/path_optimizer.cpp:124-161, src/solver/base_solver.cpp
- * from the bSpline() samples of each path to its final path, device-resident on one stream. The stage
- * kernels are those of pqp_smoother.h, pqp_dp.h, pqp_bounds.h and pqp.h; this handle adds the steps that
- * connect them (natural spline fits, the 1 m resampling, the two smoother epilogues, the start / target
- * decisions and the solver's per-instance block) and reports per path which stage failed.
+ * device-resident on one stream, from either the bSpline() samples of each path (pqp_plan) or its reference
+ * points, PathOptimizer::solve's own input (pqp_plan_points), to its final path. The stage kernels are those of
+ * pqp_smoother.h, pqp_dp.h, pqp_bounds.h and pqp.h; this handle adds the steps that connect them (the B-spline
+ * sampling of the reference points, natural spline fits, the 1 m resampling, the two smoother epilogues, the
+ * start / target decisions and the solver's per-instance block) and reports per path which stage failed.
  *
- * bSpline() itself (tinyspline) and its "fewer than 4 reference points" check stay with the caller. There is
- * no CPU fallback. Every function returns a PQP_* code from pqp.h and never throws.
+ * There is no CPU fallback. Every function returns a PQP_* code from pqp.h and never throws.
  */
 #ifndef PQP_PLAN_H
 #define PQP_PLAN_H
@@ -33,11 +34,13 @@ extern "C" {
 #endif
 
 /* status[b]: the first stage that failed. Each code is one `return false` of the reference, except
- * SPLINE_DEGENERATE and the capacity codes, where the reference asserts or grows its vectors. */
+ * SPLINE_DEGENERATE and the capacity codes, where the reference asserts or grows its vectors, and BSPLINE_DEGREE,
+ * where tinyspline throws. */
 enum {
     PQP_PLAN_OK = 0,
     PQP_PLAN_SPLINE_DEGENERATE = 1, /* fewer than 3 samples, or abscissae (arc lengths) not increasing */
-    PQP_PLAN_TOO_MANY_POINTS = 2,   /* resampled list longer than p_max, or more DP layers than layers_max */
+    PQP_PLAN_TOO_MANY_POINTS = 2,   /* more bSpline() samples than r_max (pqp_plan_points), resampled list longer
+                                       than p_max, or more DP layers than layers_max */
     PQP_PLAN_TENSION_FAILED = 3,    /* tension QP (either method) not solved (tension_smoother.cpp:32-35) */
     PQP_PLAN_DP_VEHICLE_FAR = 4,    /* graphSearchDp: |vehicle offset| > lateral range */
     PQP_PLAN_POST_TOO_SHORT = 5,    /* postSmooth: fewer than 4 DP layers kept */
@@ -47,14 +50,19 @@ enum {
     PQP_PLAN_TOO_MANY_KNOTS = 9,    /* more reference states than n_max (reported, never truncated) */
     PQP_PLAN_BLOCKED_AT_START = 10, /* fewer than 2 states before the first blocked one */
     PQP_PLAN_PRE_SOLVE_FAILED = 11, /* first solve not PQP_SOLVED (path_optimizer.cpp:142-146) */
-    PQP_PLAN_SOLVE_FAILED = 12      /* re-solve not PQP_SOLVED (:153-157) */
+    PQP_PLAN_SOLVE_FAILED = 12,     /* re-solve not PQP_SOLVED (:153-157) */
+    PQP_PLAN_POINT_COUNT = 13,      /* pqp_plan_points: fewer than 4 reference points (reference_path_smoother.cpp:33-36),
+                                       or more than the row stride m_max */
+    PQP_PLAN_BSPLINE_DEGREE = 14    /* pqp_plan_points: B-spline degree >= the number of points (tinyspline's
+                                       TS_DEG_GE_NCTRLP, an exception in the reference) */
 };
 
 #define PQP_PLAN_PATH_ROWS 7 /* x, y, heading, k, d_k, l, d_heading: the SlState fields getOptimizedPath sets */
 
 /* pqp_plan_last_stage_ms: the TimeRecorder stages of PathOptimizer::solve (path_optimizer.cpp:41-69) */
 enum {
-    PQP_PLAN_STAGE_SMOOTHING = 0,    /* segmentation, tension QP, DP, post-smooth QP, reference spline */
+    PQP_PLAN_STAGE_SMOOTHING = 0,    /* B-spline (pqp_plan_points), segmentation, tension QP, DP, post-smooth QP,
+                                        reference spline */
     PQP_PLAN_STAGE_SEGMENTATION = 1, /* processReferencePath: start / target, reference states, bounds */
     PQP_PLAN_STAGE_OPTIMISATION = 2, /* both solves and the final path */
     PQP_PLAN_STAGE_TOTAL = 3,
@@ -93,6 +101,17 @@ typedef struct pqp_plan_in {
     const double *target;   /* [b][3] x, y, heading of the target state */
 } pqp_plan_in;
 
+/* Reference points instead of samples (pqp_plan_points): PathOptimizer::solve's reference_points. Host pointers
+ * for pqp_plan_points, device pointers for pqp_plan_points_device. */
+typedef struct pqp_plan_points_in {
+    int32_t batch, m_max;   /* m_max: row stride of ref_x / ref_y, 1 <= m_max <= the handle's r_max */
+    const double *ref_x;    /* [b][m_max] reference_points[i].x */
+    const double *ref_y;    /* [b][m_max] reference_points[i].y */
+    const int32_t *m;       /* [b] points per path (points beyond m[b] are never read) */
+    const double *start;    /* [b][4] as pqp_plan_in */
+    const double *target;   /* [b][3] as pqp_plan_in */
+} pqp_plan_points_in;
+
 /* Intermediate results per stage; every pointer is optional (NULL = not written). Same memory space as the
  * call's buffers. P = p_max, L = layers_max, N = n_max, R = r_max of the handle. A path that failed before a
  * stage has unspecified entries for that stage. */
@@ -126,6 +145,9 @@ typedef struct pqp_plan_trace {
     double *x_full2, *y_full2, *z_full2; /* second solve */
     double *tension_clearance; /* [b][P] obstacle distance at the seg_x / seg_y points (TENSION only; untouched
                                   under TENSION2) */
+    int32_t *raw_r;          /* [b] bSpline() samples (R + 1: more than R; 0: points rejected). pqp_plan_points only;
+                                the samples themselves are raw_spline rows 4 (x) and 8 (y) */
+    int32_t *bspline_degree; /* [b] B-spline degree, 3 to 5 (0: point count rejected). pqp_plan_points only */
 } pqp_plan_trace;
 
 typedef struct pqp_plan_out {
@@ -151,6 +173,13 @@ int pqp_plan(pqp_plan_handle *h, const pqp_plan_in *in, const pqp_plan_out *out)
  * allocation. Solves are FP32 without the FP64 re-solve (pqp.h, *_device): an infeasible instance the FP32
  * certificate cannot resolve ends as PQP_PLAN_PRE_SOLVE_FAILED. pqp_plan uses this same path. */
 int pqp_plan_device(pqp_plan_handle *h, const pqp_plan_in *in, const pqp_plan_out *out, void *stream);
+/* The whole of PathOptimizer::solve: bSpline() on the GPU (a clamped B-spline of degree 3 to 5 over the points,
+ * sampled about once per metre of the control polygon) into the handle's [B][r_max] sample storage, then the
+ * pqp_plan chain. pqp_plan_points: host buffers, synchronous; pqp_plan_points_device: device buffers, asynchronous on
+ * `stream`, no allocation. Per-path failures: POINT_COUNT, BSPLINE_DEGREE, TOO_MANY_POINTS (more samples than
+ * r_max), and SPLINE_DEGENERATE from the samples (a polygon shorter than 1 m, of zero length, or with NaN points). */
+int pqp_plan_points(pqp_plan_handle *h, const pqp_plan_points_in *in, const pqp_plan_out *out);
+int pqp_plan_points_device(pqp_plan_handle *h, const pqp_plan_points_in *in, const pqp_plan_out *out, void *stream);
 /* ms[PQP_PLAN_NSTAGES] of the last call (CUDA events; waits for that call to finish). */
 int pqp_plan_last_stage_ms(pqp_plan_handle *h, float *ms);
 /* Kernel launches issued by the handle so far: the glue kernels plus those of every stage handle it owns. */

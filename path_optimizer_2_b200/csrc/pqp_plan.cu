@@ -33,10 +33,42 @@ struct Dims {
     int B, R, P, L, N, in_r;
 };
 
-// raw samples -> s_list_ (chord length) into the raw spline rows, sample count of segmentRawReference
+// bSpline() up to its sample parameters (pqp_plan_points), one thread per path: the point-count and degree checks,
+// the control polygon's length and degree, and the t accumulation into the path's row of t_all (at most R values)
+__global__ void bspline_prep_kernel(Dims d, int m_max, const double *__restrict__ px, const double *__restrict__ py,
+                                    const int32_t *__restrict__ m, double *t_all, int32_t *raw_r, int32_t *degree,
+                                    int32_t *status) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= d.B) return;
+    int r, deg;
+    status[b] = pqpl::bspline_prepare(px + (size_t)b * m_max, py + (size_t)b * m_max, m[b], m_max, d.R,
+                                      t_all + (size_t)b * d.R, r, deg);
+    raw_r[b] = r;
+    degree[b] = deg;
+}
+
+// bSpline()'s samples (pqp_plan_points): de Boor at each parameter, one thread per (path, sample), into the [B][R]
+// rows the raw prep reads
+__global__ void bspline_eval_kernel(Dims d, int m_max, const double *__restrict__ px, const double *__restrict__ py,
+                                    const int32_t *__restrict__ m, const double *__restrict__ t_all,
+                                    const int32_t *__restrict__ raw_r, const int32_t *__restrict__ degree,
+                                    const int32_t *__restrict__ status, double *out_x, double *out_y) {
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (long long)d.B * d.R) return;
+    const int b = (int)(t / d.R), j = (int)(t % d.R);
+    if (status[b] != pqpl::kOk || j >= raw_r[b]) return;
+    const size_t o = (size_t)b * d.R + j;
+    double x, y;
+    pqpl::bspline_eval(px + (size_t)b * m_max, py + (size_t)b * m_max, m[b], degree[b], t_all[o], x, y);
+    out_x[o] = x;
+    out_y[o] = y;
+}
+
+// raw samples -> s_list_ (chord length) into the raw spline rows, sample count of segmentRawReference. `prior`
+// (pqp_plan_points: the B-spline stage's status, possibly `status` itself) keeps an earlier failure; NULL under pqp_plan.
 __global__ void raw_prep_kernel(Dims d, const double *__restrict__ raw_x, const double *__restrict__ raw_y,
-                                const int32_t *__restrict__ r, const double *__restrict__ start, double *raw_rows,
-                                int32_t *raw_k, int32_t *seg_p, int32_t *status, double *start3) {
+                                const int32_t *__restrict__ r, const double *__restrict__ start, const int32_t *prior,
+                                double *raw_rows, int32_t *raw_k, int32_t *seg_p, int32_t *status, double *start3) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= d.B) return;
     start3[3 * b] = start[4 * b];
@@ -44,11 +76,11 @@ __global__ void raw_prep_kernel(Dims d, const double *__restrict__ raw_x, const 
     start3[3 * b + 2] = start[4 * b + 2];
     double *rows = raw_rows + (size_t)b * pqpl::kSplineRows * d.R;
     double *sx = rows, *x = rows + 4 * (size_t)d.R, *y = rows + 8 * (size_t)d.R;
-    const int rb = r[b];
-    int st = pqpl::kOk, p = 0;
-    if (rb < 3 || rb > d.R) {
+    int st = prior ? prior[b] : pqpl::kOk, p = 0;
+    const int rb = st == pqpl::kOk ? r[b] : 0;  // a path that failed before its samples has none to read
+    if (st == pqpl::kOk && (rb < 3 || rb > d.R)) {
         st = pqpl::kSplineDegenerate;
-    } else {
+    } else if (st == pqpl::kOk) {
         for (int i = 0; i < rb; ++i) {
             x[i] = raw_x[(size_t)b * d.in_r + i];
             y[i] = raw_y[(size_t)b * d.in_r + i];
@@ -342,6 +374,10 @@ struct pqp_plan_handle {
     int32_t *post_p = nullptr, *post_status = nullptr, *post_iters = nullptr, *rk = nullptr;
     double *post_off = nullptr, *r_rows = nullptr, *r_len = nullptr, *max_s = nullptr;
     double *t_clear = nullptr;  // [B][P] clearance of the Cartesian tension QP (TENSION only)
+    // pqp_plan_points: the host call's staged points, the sample parameters, samples and degree per path (the samples
+    // themselves go to in_x / in_y)
+    double *pt_x = nullptr, *pt_y = nullptr, *bs_t = nullptr;
+    int32_t *pt_m = nullptr, *raw_r = nullptr, *bs_deg = nullptr;
     double *states = nullptr, *curv = nullptr, *bnd = nullptr, *knots = nullptr, *knots2 = nullptr, *inst = nullptr,
            *ref_xyh = nullptr, *xyh = nullptr;
     int32_t *n_states = nullptr, *total = nullptr, *n_valid = nullptr, *n1 = nullptr, *n2 = nullptr, *p = nullptr;
@@ -390,12 +426,22 @@ int validate(pqp_plan_handle *h, const pqp_plan_in *in, const pqp_plan_out *out)
     return PQP_OK;
 }
 
+int validate_points(pqp_plan_handle *h, const pqp_plan_points_in *in, const pqp_plan_out *out) {
+    if (!h) return PQP_E_INVALID;
+    if (!in || !out) return pfail(h, PQP_E_INVALID, "null batch");
+    if (!in->ref_x || !in->ref_y || !in->m || !in->start || !in->target) return pfail(h, PQP_E_INVALID, "null input buffer");
+    if (!out->status || !out->n || !out->path || !out->cost || !out->iters) return pfail(h, PQP_E_INVALID, "null output buffer");
+    if (in->batch < 1 || in->batch > h->batch_max) return pfail(h, PQP_E_INVALID, "batch out of range");
+    if (in->m_max < 1 || in->m_max > h->R) return pfail(h, PQP_E_INVALID, "m_max must be in [1, the handle's r_max]");
+    return PQP_OK;
+}
+
 int copy_out(pqp_plan_handle *h, void *dst, const void *src, size_t bytes, cudaStream_t s) {
     if (dst) PQL_CUDA(h, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, s));
     return PQP_OK;
 }
 
-int copy_trace(pqp_plan_handle *h, const pqp_plan_trace *t, int B, cudaStream_t s) {
+int copy_trace(pqp_plan_handle *h, const pqp_plan_trace *t, int B, bool points, cudaStream_t s) {
     if (!t) return PQP_OK;
     const size_t b = B, d = sizeof(double), i4 = sizeof(int32_t), P = h->P, L = h->L, N = h->N, R = h->R;
     int rc = PQP_OK;
@@ -446,19 +492,47 @@ int copy_trace(pqp_plan_handle *h, const pqp_plan_trace *t, int B, cudaStream_t 
     PQL_T(t->y_full2, h->full[4], b * m * d);
     PQL_T(t->z_full2, h->full[5], b * m * d);
     if (h->t_clear) PQL_T(t->tension_clearance, h->t_clear, b * P * d);
+    if (points) {
+        PQL_T(t->raw_r, h->raw_r, b * i4);
+        PQL_T(t->bspline_degree, h->bs_deg, b * i4);
+    }
 #undef PQL_T
     return PQP_OK;
 }
 
-int run(pqp_plan_handle *h, const pqp_plan_in *in, const pqp_plan_out *out, cudaStream_t s) {
+// the host calls' outputs from the handle's staging buffers; waits for the call to finish
+int copy_results(pqp_plan_handle *h, const pqp_plan_out *out, int batch, cudaStream_t s) {
+    const size_t B = batch, N = h->N;
+    PQL_CUDA(h, cudaMemcpyAsync(out->status, h->o_status, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    PQL_CUDA(h, cudaMemcpyAsync(out->n, h->o_n, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    PQL_CUDA(h, cudaMemcpyAsync(out->iters, h->o_iters, B * 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    PQL_CUDA(h, cudaMemcpyAsync(out->cost, h->o_cost, B * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PQL_CUDA(h, cudaMemcpyAsync(out->path, h->o_path, B * PQP_PLAN_PATH_ROWS * N * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PQL_CUDA(h, cudaStreamSynchronize(s));
+    return PQP_OK;
+}
+
+// `pts` (pqp_plan_points, device pointers): bSpline() first writes the samples of those points into `in`'s raw_x,
+// raw_y and r (the handle's in_x, in_y and raw_r) and its status into h->status
+int run(pqp_plan_handle *h, const pqp_plan_in *in, const pqp_plan_out *out, cudaStream_t s,
+        const pqp_plan_points_in *pts = nullptr) {
     const int B = in->batch;
     const Dims d{B, h->R, h->P, h->L, h->N, in->r_max};
     const pqp_plan_trace *tr = out->trace;
     h->timed = true;
     PQL_CUDA(h, cudaEventRecord(h->ev[0], s));
     // ---- reference path smoothing (ReferencePathSmoother::solve) ----
-    raw_prep_kernel<<<blocks_for(B), kThreads, 0, s>>>(d, in->raw_x, in->raw_y, in->r, in->start, h->raw_rows, h->raw_k,
-                                                        h->seg_p, h->status, h->start3);
+    if (pts) {
+        bspline_prep_kernel<<<blocks_for(B), kThreads, 0, s>>>(d, pts->m_max, pts->ref_x, pts->ref_y, pts->m, h->bs_t,
+                                                                h->raw_r, h->bs_deg, h->status);
+        PQL_LAUNCH(h);
+        bspline_eval_kernel<<<blocks_for((long long)B * h->R), kThreads, 0, s>>>(
+            d, pts->m_max, pts->ref_x, pts->ref_y, pts->m, h->bs_t, h->raw_r, h->bs_deg, h->status, h->in_x, h->in_y);
+        PQL_LAUNCH(h);
+    }
+    raw_prep_kernel<<<blocks_for(B), kThreads, 0, s>>>(d, in->raw_x, in->raw_y, in->r, in->start,
+                                                        pts ? h->status : nullptr, h->raw_rows, h->raw_k, h->seg_p,
+                                                        h->status, h->start3);
     PQL_LAUNCH(h);
     fit_kernel<<<blocks_for(2LL * B), kThreads, 0, s>>>(B, h->R, h->raw_rows, h->raw_k);
     PQL_LAUNCH(h);
@@ -585,7 +659,13 @@ int run(pqp_plan_handle *h, const pqp_plan_in *in, const pqp_plan_out *out, cuda
     }
     PQL_CUDA(h, cudaEventRecord(h->ev[3], s));
     h->launches += kStageLaunches;
-    return copy_trace(h, tr, B, s);
+    return copy_trace(h, tr, B, pts != nullptr, s);
+}
+
+// pqp_plan_points(_device) on device points: the samples go to the handle's [B][R] sample storage
+int run_points(pqp_plan_handle *h, const pqp_plan_points_in *pts, const pqp_plan_out *out, cudaStream_t s) {
+    const pqp_plan_in din = {pts->batch, h->R, h->in_x, h->in_y, h->raw_r, pts->start, pts->target};
+    return run(h, &din, out, s, pts);
 }
 
 }  // namespace
@@ -734,6 +814,12 @@ int pqp_plan_create(const pqp_bounds_map *map, const pqp_plan_params *params, in
     if (e == cudaSuccess) e = dalloc(&h->iters2, B);
     for (int i = 0; i < 6 && e == cudaSuccess; ++i) e = dalloc(&h->full[i], B * (i % 3 == 0 ? 6 * N - 1 : 6 * N + 2));
     if (e == cudaSuccess && h->prm.smoothing_method == PQP_PLAN_SMOOTH_TENSION) e = dalloc(&h->t_clear, B * P);
+    if (e == cudaSuccess) e = dalloc(&h->pt_x, B * R);
+    if (e == cudaSuccess) e = dalloc(&h->pt_y, B * R);
+    if (e == cudaSuccess) e = dalloc(&h->pt_m, B);
+    if (e == cudaSuccess) e = dalloc(&h->bs_t, B * R);
+    if (e == cudaSuccess) e = dalloc(&h->raw_r, B);
+    if (e == cudaSuccess) e = dalloc(&h->bs_deg, B);
     // spline rows are zero beyond each path's k, so every row read past the end of a fit is defined
     if (e == cudaSuccess) e = cudaMemset(h->raw_rows, 0, B * S * R * sizeof(double));
     if (e == cudaSuccess) e = cudaMemset(h->t_rows, 0, B * S * P * sizeof(double));
@@ -764,7 +850,7 @@ void pqp_plan_destroy(pqp_plan_handle *h) {
                         h->states, h->curv, h->bnd, h->knots, h->knots2, h->inst, h->ref_xyh, h->xyh, h->n_states,
                         h->total, h->n_valid, h->n1, h->n2, h->p, h->sol1, h->sol2, h->cost1, h->cost2, h->status1,
                         h->iters1, h->status2, h->iters2, h->full[0], h->full[1], h->full[2], h->full[3], h->full[4],
-                        h->full[5], h->t_clear};
+                        h->full[5], h->t_clear, h->pt_x, h->pt_y, h->pt_m, h->bs_t, h->raw_r, h->bs_deg};
         for (void *p : bufs) cudaFree(p);
         for (cudaEvent_t ev : h->ev)
             if (ev) cudaEventDestroy(ev);
@@ -790,7 +876,7 @@ int pqp_plan(pqp_plan_handle *h, const pqp_plan_in *in, const pqp_plan_out *out)
     if (rc != PQP_OK) return rc;
     pqp::DeviceGuard guard_(h->device);
     cudaStream_t s = h->stream;
-    const size_t B = in->batch, R = in->r_max, N = h->N;
+    const size_t B = in->batch, R = in->r_max;
     PQL_CUDA(h, cudaMemcpyAsync(h->in_x, in->raw_x, B * R * sizeof(double), cudaMemcpyHostToDevice, s));
     PQL_CUDA(h, cudaMemcpyAsync(h->in_y, in->raw_y, B * R * sizeof(double), cudaMemcpyHostToDevice, s));
     PQL_CUDA(h, cudaMemcpyAsync(h->in_r, in->r, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
@@ -800,13 +886,32 @@ int pqp_plan(pqp_plan_handle *h, const pqp_plan_in *in, const pqp_plan_out *out)
     const pqp_plan_out dout = {h->o_status, h->o_n, h->o_path, h->o_cost, h->o_iters, out->trace};
     rc = run(h, &din, &dout, s);
     if (rc != PQP_OK) return rc;
-    PQL_CUDA(h, cudaMemcpyAsync(out->status, h->o_status, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    PQL_CUDA(h, cudaMemcpyAsync(out->n, h->o_n, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    PQL_CUDA(h, cudaMemcpyAsync(out->iters, h->o_iters, B * 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    PQL_CUDA(h, cudaMemcpyAsync(out->cost, h->o_cost, B * sizeof(double), cudaMemcpyDeviceToHost, s));
-    PQL_CUDA(h, cudaMemcpyAsync(out->path, h->o_path, B * PQP_PLAN_PATH_ROWS * N * sizeof(double), cudaMemcpyDeviceToHost, s));
-    PQL_CUDA(h, cudaStreamSynchronize(s));
-    return PQP_OK;
+    return copy_results(h, out, in->batch, s);
+}
+
+int pqp_plan_points_device(pqp_plan_handle *h, const pqp_plan_points_in *in, const pqp_plan_out *out, void *stream) {
+    int rc = validate_points(h, in, out);
+    if (rc != PQP_OK) return rc;
+    pqp::DeviceGuard guard_(h->device);
+    return run_points(h, in, out, static_cast<cudaStream_t>(stream));
+}
+
+int pqp_plan_points(pqp_plan_handle *h, const pqp_plan_points_in *in, const pqp_plan_out *out) {
+    int rc = validate_points(h, in, out);
+    if (rc != PQP_OK) return rc;
+    pqp::DeviceGuard guard_(h->device);
+    cudaStream_t s = h->stream;
+    const size_t B = in->batch, M = in->m_max;
+    PQL_CUDA(h, cudaMemcpyAsync(h->pt_x, in->ref_x, B * M * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQL_CUDA(h, cudaMemcpyAsync(h->pt_y, in->ref_y, B * M * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQL_CUDA(h, cudaMemcpyAsync(h->pt_m, in->m, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    PQL_CUDA(h, cudaMemcpyAsync(h->in_start, in->start, B * 4 * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQL_CUDA(h, cudaMemcpyAsync(h->in_target, in->target, B * 3 * sizeof(double), cudaMemcpyHostToDevice, s));
+    const pqp_plan_points_in din = {in->batch, in->m_max, h->pt_x, h->pt_y, h->pt_m, h->in_start, h->in_target};
+    const pqp_plan_out dout = {h->o_status, h->o_n, h->o_path, h->o_cost, h->o_iters, out->trace};
+    rc = run_points(h, &din, &dout, s);
+    if (rc != PQP_OK) return rc;
+    return copy_results(h, out, in->batch, s);
 }
 
 int pqp_plan_last_stage_ms(pqp_plan_handle *h, float *ms) {

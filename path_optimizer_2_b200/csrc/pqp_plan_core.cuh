@@ -18,7 +18,7 @@ namespace pqpl {
 enum {
     kOk = 0, kSplineDegenerate = 1, kTooManyPoints = 2, kTensionFailed = 3, kDpVehicleFar = 4, kPostTooShort = 5,
     kPostFailed = 6, kEmptyReference = 7, kInitHeading = 8, kTooManyKnots = 9, kBlockedAtStart = 10,
-    kPreSolveFailed = 11, kSolveFailed = 12
+    kPreSolveFailed = 11, kSolveFailed = 12, kPointCount = 13, kBsplineDegree = 14
 };
 
 constexpr int kSplineRows = 9;  // PQP_SPLINE_ROWS
@@ -76,6 +76,111 @@ PQB_HD bool increasing(const double *s, int k) {
     for (int i = 1; i < k; ++i)
         if (!(s[i] > s[i - 1])) return false;
     return true;
+}
+
+// ---- bSpline() (reference_path_smoother.cpp:490-524): a clamped B-spline whose control points are the reference
+// points, sampled at t = 0, delta_t, 2 delta_t (accumulated), ... below 1, then at t = 1 ----
+
+// Length of the control polygon: the sequential sum of the point distances (tools.cpp:46-48), squares as d * d.
+PQB_HD double polygon_length(const double *x, const double *y, int m) {
+    double length = 0.0;
+    for (int i = 0; i + 1 < m; ++i) {
+        const double dx = x[i] - x[i + 1], dy = y[i] - y[i + 1];
+        length += sqrt(dx * dx + dy * dy);
+    }
+    return length;
+}
+
+// 3 when the average point spacing is above 10 m, 4 above 5 m, else 5 (strict comparisons: NaN gives 5).
+PQB_HD int bspline_degree(double length, int m) {
+    const double average = length / (double)(m - 1);
+    if (average > 10.0) return 3;
+    if (average > 5.0) return 4;
+    return 5;
+}
+
+// The sample parameters: t = 0, then t += 1 / length while t < 1, then t = 1. Writes at most `cap` values into t[]
+// and returns their count, or cap + 1 when there would be more (an infinite length gives delta_t = 0, on which the
+// reference loops forever). A NaN length, a zero length or one below 1 m gives the two samples t = 0 and t = 1.
+PQB_HD int bspline_abscissae(double length, int cap, double *t) {
+    const double delta_t = 1.0 / length;
+    double tmp_t = 0.0;
+    int count = 0;
+    while (tmp_t < 1.0) {
+        if (count == cap) return cap + 1;
+        t[count++] = tmp_t;
+        tmp_t += delta_t;
+    }
+    if (count == cap) return cap + 1;
+    t[count++] = 1.0;
+    return count;
+}
+
+// Knot i of the clamped uniform vector of m control points: degree + 1 zeros, (i - degree) / (m - degree), degree + 1
+// ones. Computed the same way wherever it is compared, so the span choice is a pure function of (t, degree, m).
+PQB_HD double bspline_knot(int i, int degree, int m) {
+    if (i <= degree) return 0.0;
+    if (i >= m) return 1.0;
+    return (double)(i - degree) / (double)(m - degree);
+}
+
+// The span k in [degree, m - 1] with knot(k) <= t < knot(k + 1); t = 1 falls in the last non-empty span, m - 1.
+PQB_HD int bspline_span(double t, int degree, int m) {
+    int lo = degree, hi = m - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (bspline_knot(mid, degree, m) <= t) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
+// de Boor's algorithm at t for degree D (unrolled, so the working points stay in registers). At t = 0 every alpha is
+// 0 and at t = 1 every alpha is 1, so the end samples are the first and the last point exactly.
+template <int D>
+PQB_HD void de_boor(const double *px, const double *py, int m, double t, double &x, double &y) {
+    const int k = bspline_span(t, D, m);
+    double dx[D + 1], dy[D + 1];
+#pragma unroll
+    for (int j = 0; j <= D; ++j) {
+        dx[j] = px[j + k - D];
+        dy[j] = py[j + k - D];
+    }
+#pragma unroll
+    for (int r = 1; r <= D; ++r) {
+#pragma unroll
+        for (int j = D; j >= r; --j) {
+            const double ua = bspline_knot(j + k - D, D, m);
+            const double ub = bspline_knot(j + 1 + k - r, D, m);
+            const double alpha = (t - ua) / (ub - ua);
+            dx[j] = (1.0 - alpha) * dx[j - 1] + alpha * dx[j];
+            dy[j] = (1.0 - alpha) * dy[j - 1] + alpha * dy[j];
+        }
+    }
+    x = dx[D];
+    y = dy[D];
+}
+
+// One sample of the curve of degree 3, 4 or 5 over the m points (px, py).
+PQB_HD void bspline_eval(const double *px, const double *py, int m, int degree, double t, double &x, double &y) {
+    if (degree == 3) de_boor<3>(px, py, m, t, x, y);
+    else if (degree == 4) de_boor<4>(px, py, m, t, x, y);
+    else de_boor<5>(px, py, m, t, x, y);
+}
+
+// bSpline()'s checks and sample parameters for one path: kPointCount for fewer than 4 points (reference_path_smoother
+// .cpp:33-36) or more than the row holds, kBsplineDegree when degree >= m (tinyspline refuses the spline),
+// kTooManyPoints when there are more than `cap` samples. r = samples written to t[] (cap + 1 when over capacity, 0 when
+// the points were rejected), degree = 0 when the count was rejected.
+PQB_HD int bspline_prepare(const double *x, const double *y, int m, int m_max, int cap, double *t, int &r, int &degree) {
+    r = 0;
+    degree = 0;
+    if (m < 4 || m > m_max) return kPointCount;
+    const double length = polygon_length(x, y, m);
+    degree = bspline_degree(length, m);
+    if (degree >= m) return kBsplineDegree;
+    r = bspline_abscissae(length, cap, t);
+    return r > cap ? kTooManyPoints : kOk;
 }
 
 // s_list_ of bSpline() (reference_path_smoother.cpp:519-523): cumulative chord length, squares written as d * d.

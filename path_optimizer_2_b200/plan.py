@@ -1,6 +1,7 @@
 """ctypes binding of include/pqp_plan.h: PathOptimizer::solve (path_optimizer.cpp:34-71) for a batch of paths on the
-GPU, from the bSpline() samples of each path to its final path. `Planner` owns one handle: the map, the stage handles
-and all scratch. No CPU path."""
+GPU, from the bSpline() samples of each path (`plan`) or from its reference points, PathOptimizer::solve's own input
+(`plan_points`), to its final path. `Planner` owns one handle: the map, the stage handles and all scratch. No CPU
+path."""
 import ctypes as C
 
 import numpy as np
@@ -8,13 +9,14 @@ import numpy as np
 from . import abi, bounds, dp, smoother, solver
 
 EXPORTED_SYMBOLS = ["pqp_plan_default_params", "pqp_plan_create", "pqp_plan_destroy", "pqp_plan", "pqp_plan_device",
-                    "pqp_plan_last_stage_ms", "pqp_plan_launch_count", "pqp_plan_last_error"]
+                    "pqp_plan_points", "pqp_plan_points_device", "pqp_plan_last_stage_ms", "pqp_plan_launch_count",
+                    "pqp_plan_last_error"]
 
 STATUS_NAMES = ("OK", "SPLINE_DEGENERATE", "TOO_MANY_POINTS", "TENSION_FAILED", "DP_VEHICLE_FAR", "POST_TOO_SHORT",
                 "POST_FAILED", "EMPTY_REFERENCE", "INIT_HEADING", "TOO_MANY_KNOTS", "BLOCKED_AT_START",
-                "PRE_SOLVE_FAILED", "SOLVE_FAILED")
+                "PRE_SOLVE_FAILED", "SOLVE_FAILED", "POINT_COUNT", "BSPLINE_DEGREE")
 (OK, SPLINE_DEGENERATE, TOO_MANY_POINTS, TENSION_FAILED, DP_VEHICLE_FAR, POST_TOO_SHORT, POST_FAILED, EMPTY_REFERENCE,
- INIT_HEADING, TOO_MANY_KNOTS, BLOCKED_AT_START, PRE_SOLVE_FAILED, SOLVE_FAILED) = range(13)
+ INIT_HEADING, TOO_MANY_KNOTS, BLOCKED_AT_START, PRE_SOLVE_FAILED, SOLVE_FAILED, POINT_COUNT, BSPLINE_DEGREE) = range(15)
 PATH_ROWS = ("x", "y", "heading", "k", "d_k", "l", "d_heading")
 STAGES = ("smoothing", "segmentation", "optimisation", "total")
 # PlanParams.smoothing_method: the reference's --smoothing_method
@@ -33,6 +35,11 @@ class PlanParams(C.Structure):
 class PlanIn(C.Structure):
     _fields_ = [("batch", C.c_int32), ("r_max", C.c_int32)] + [
         (n, C.c_void_p) for n in ("raw_x", "raw_y", "r", "start", "target")]
+
+
+class PlanPointsIn(C.Structure):
+    _fields_ = [("batch", C.c_int32), ("m_max", C.c_int32)] + [
+        (n, C.c_void_p) for n in ("ref_x", "ref_y", "m", "start", "target")]
 
 
 # (name, dtype, shape given (P, L, N, R)) in the order of pqp_plan_trace
@@ -63,6 +70,7 @@ _TRACE = [
     ("x_full2", np.float64, lambda P, L, N, R: (6 * N - 1,)), ("y_full2", np.float64, lambda P, L, N, R: (6 * N + 2,)),
     ("z_full2", np.float64, lambda P, L, N, R: (6 * N + 2,)),
     ("tension_clearance", np.float64, lambda P, L, N, R: (P,)),
+    ("raw_r", np.int32, lambda *d: ()), ("bspline_degree", np.int32, lambda *d: ()),  # plan_points only
 ]
 
 
@@ -86,6 +94,8 @@ def _lib():
         L.pqp_plan_destroy.restype = None
         L.pqp_plan.argtypes = [vp, C.POINTER(PlanIn), C.POINTER(PlanOut)]
         L.pqp_plan_device.argtypes = [vp, C.POINTER(PlanIn), C.POINTER(PlanOut), vp]
+        L.pqp_plan_points.argtypes = [vp, C.POINTER(PlanPointsIn), C.POINTER(PlanOut)]
+        L.pqp_plan_points_device.argtypes = [vp, C.POINTER(PlanPointsIn), C.POINTER(PlanOut), vp]
         L.pqp_plan_last_stage_ms.argtypes = [vp, C.POINTER(C.c_float)]
         L.pqp_plan_launch_count.argtypes = [vp, C.POINTER(C.c_int64)]
         L.pqp_plan_last_error.argtypes = [vp]
@@ -165,35 +175,56 @@ class Planner:
     def dims(self):
         return self.p_max, self.layers_max, self.n_max, self.r_max
 
-    def plan(self, raw_x, raw_y, start, target, trace=False) -> PlanResult:
-        """Host call. raw_x, raw_y: lists of per-path sample arrays (x_list_, y_list_ of bSpline()); start [B][4]
-        (x, y, heading, k); target [B][3] (x, y, heading)."""
-        B = len(raw_x)
-        r = np.array([len(v) for v in raw_x], dtype=np.int32)
-        rx, ry = np.zeros((B, self.r_max)), np.zeros((B, self.r_max))
+    def _host_call(self, fn, make_in, xs, ys, start, target, trace, stride, clip=False):
+        B = len(xs)
+        cnt = np.array([len(v) for v in xs], dtype=np.int32)
+        rx, ry = np.zeros((B, stride)), np.zeros((B, stride))
         for b in range(B):
-            rx[b, :r[b]], ry[b, :r[b]] = raw_x[b], raw_y[b]
+            k = min(int(cnt[b]), stride) if clip else int(cnt[b])  # clip: a longer row is rejected by its count
+            rx[b, :k], ry[b, :k] = xs[b][:k], ys[b][:k]
         start = np.ascontiguousarray(start, dtype=np.float64).reshape(B, 4)
         target = np.ascontiguousarray(target, dtype=np.float64).reshape(B, 3)
         res = PlanResult(B, self.n_max)
-        pin = PlanIn(B, self.r_max, rx.ctypes.data, ry.ctypes.data, r.ctypes.data, start.ctypes.data, target.ctypes.data)
+        pin = make_in(B, stride, rx.ctypes.data, ry.ctypes.data, cnt.ctypes.data, start.ctypes.data, target.ctypes.data)
         tr = None
         if trace:
             res.trace = _trace_arrays(B, self.dims, lambda shape, dt: np.zeros(shape, dtype=dt))
             tr = _trace_struct(res.trace, lambda a: a.ctypes.data)
         pout = PlanOut(res.status.ctypes.data, res.n.ctypes.data, res.path.ctypes.data, res.cost.ctypes.data,
                        res.iters.ctypes.data, C.pointer(tr) if tr is not None else None)
-        self._check(self.L.pqp_plan(self.h, C.byref(pin), C.byref(pout)))
+        self._check(fn(self.h, C.byref(pin), C.byref(pout)))
         return res
+
+    def plan(self, raw_x, raw_y, start, target, trace=False) -> PlanResult:
+        """Host call. raw_x, raw_y: lists of per-path sample arrays (x_list_, y_list_ of bSpline()); start [B][4]
+        (x, y, heading, k); target [B][3] (x, y, heading)."""
+        return self._host_call(self.L.pqp_plan, PlanIn, raw_x, raw_y, start, target, trace, self.r_max)
+
+    def plan_points(self, ref_x, ref_y, start, target, trace=False, m_max=None) -> PlanResult:
+        """Host call from the reference points (PathOptimizer::solve's reference_points): ref_x, ref_y are lists of
+        per-path point arrays; bSpline() runs on the GPU. `m_max` (default r_max) is the row stride; a path with more
+        points than that is reported as POINT_COUNT. start, target as `plan`."""
+        m_max = self.r_max if m_max is None else int(m_max)
+        return self._host_call(self.L.pqp_plan_points, PlanPointsIn, ref_x, ref_y, start, target, trace, m_max,
+                               clip=True)
 
     def plan_device(self, raw_x, raw_y, r, start, target, *, trace=False, stream=None):
         """Device call on torch tensors (cuda, contiguous): raw_x / raw_y float64 [B][r_max'], r int32 [B], start
         float64 [B][4], target float64 [B][3]. Asynchronous on `stream` (default: the current stream); returns a dict of
         output tensors (status, n, path, cost, iters, and `trace`: a dict of tensors when requested)."""
+        return self._device_call(self.L.pqp_plan_device, PlanIn, raw_x, raw_y, r, start, target, trace, stream)
+
+    def plan_points_device(self, ref_x, ref_y, m, start, target, *, trace=False, stream=None):
+        """Device call from the reference points on torch tensors (cuda, contiguous): ref_x / ref_y float64
+        [B][m_max], m int32 [B], start float64 [B][4], target float64 [B][3]; m_max <= r_max. As `plan_device`."""
+        return self._device_call(self.L.pqp_plan_points_device, PlanPointsIn, ref_x, ref_y, m, start, target, trace,
+                                 stream)
+
+    def _device_call(self, fn, make_in, xs, ys, cnt, start, target, trace, stream):
         import torch
-        B = int(raw_x.shape[0])
-        dev = raw_x.device
-        for t in (raw_x, raw_y, r, start, target):
+        B = int(xs.shape[0])
+        dev = xs.device
+        for t in (xs, ys, cnt, start, target):
             assert t.is_cuda and t.is_contiguous()
         out = {"status": torch.zeros(B, dtype=torch.int32, device=dev), "n": torch.zeros(B, dtype=torch.int32, device=dev),
                "path": torch.zeros((B, len(PATH_ROWS), self.n_max), dtype=torch.float64, device=dev),
@@ -204,12 +235,12 @@ class Planner:
         if trace:
             out["trace"] = _trace_arrays(B, self.dims, lambda shape, dt: torch.zeros(shape, dtype=tdt[dt], device=dev))
             tr = _trace_struct(out["trace"], lambda a: a.data_ptr())
-        pin = PlanIn(B, int(raw_x.shape[1]), raw_x.data_ptr(), raw_y.data_ptr(), r.data_ptr(), start.data_ptr(),
-                     target.data_ptr())
+        pin = make_in(B, int(xs.shape[1]), xs.data_ptr(), ys.data_ptr(), cnt.data_ptr(), start.data_ptr(),
+                      target.data_ptr())
         pout = PlanOut(out["status"].data_ptr(), out["n"].data_ptr(), out["path"].data_ptr(), out["cost"].data_ptr(),
                        out["iters"].data_ptr(), C.pointer(tr) if tr is not None else None)
         s = stream if stream is not None else torch.cuda.current_stream(dev)
-        self._check(self.L.pqp_plan_device(self.h, C.byref(pin), C.byref(pout), C.c_void_p(s.cuda_stream)))
+        self._check(fn(self.h, C.byref(pin), C.byref(pout), C.c_void_p(s.cuda_stream)))
         return out
 
     @property

@@ -169,12 +169,13 @@ class LineBatch:
         return np.ascontiguousarray(self.states[:, 1:4])
 
 
-def make_plan_inputs(batch, n=120, first=0, dmap=None, seed=11, noise=0.03):
+def make_plan_inputs(batch, n=120, first=0, dmap=None, seed=11, noise=0.03, lines=None):
     """Inputs of a whole plan (include/pqp_plan.h) from the lines of `make_lines`: the line sampled about every 1 m
     with `noise` m of noise stands in for bSpline()'s samples; the start lies up to 1 m beside the line at s = 0.5
-    with its heading and curvature, the target on the line 1 m before its end. -> (raw_x, raw_y lists, start [B][4],
-    target [B][3])."""
-    lines = make_lines(batch, n, first=first, dmap=dmap)
+    with its heading and curvature, the target on the line 1 m before its end. `lines`: make_lines(batch, n, first,
+    dmap=dmap) when already built. -> (raw_x, raw_y lists, start [B][4], target [B][3])."""
+    if lines is None:
+        lines = make_lines(batch, n, first=first, dmap=dmap)
     rng = np.random.default_rng(seed + first)
     raw_x, raw_y = [], []
     start, target = np.zeros((batch, 4)), np.zeros((batch, 3))
@@ -195,6 +196,31 @@ def make_plan_inputs(batch, n=120, first=0, dmap=None, seed=11, noise=0.03):
         ye, dye, _ = (float(v) for v in _eval(rows, end - 1.0, 1))
         target[b] = xe, ye, math.atan2(dye, dxe)
     return raw_x, raw_y, start, target
+
+
+def make_plan_points(batch, n=120, first=0, dmap=None, seed=11, spacing=(3.0, 14.0), noise=0.2):
+    """Inputs of a whole plan from the reference points (pqp_plan_points): "clicked" points along the lines of
+    `make_lines`, evenly spaced per path at a spacing drawn from `spacing` (m) - so that the B-spline degrees 3
+    (average spacing above 10 m), 4 (above 5 m) and 5 all occur - from the line's start to its end, each moved up to
+    `noise` m (normal, sigma noise / 2) sideways. Start and target are those of `make_plan_inputs`.
+    -> (ref_x, ref_y lists, start [B][4], target [B][3])."""
+    dmap = dmap or DistanceMap()
+    lines = make_lines(batch, n, first=first, dmap=dmap)
+    _, _, start, target = make_plan_inputs(batch, n, first=first, dmap=dmap, seed=seed, lines=lines)
+    rng = np.random.default_rng(seed + 7919 + first)
+    ref_x, ref_y = [], []
+    for b in range(batch):
+        rows = lines.spline_rows(b)
+        end = float(rows[0, -1])
+        m = max(int(round(end / rng.uniform(*spacing))), 3) + 1
+        s = np.linspace(0.0, end, m)
+        x, dx, _ = _eval(rows, s, 0)
+        y, dy, _ = _eval(rows, s, 1)
+        h = np.arctan2(dy, dx)
+        off = np.clip(rng.normal(0.0, noise / 2, m), -noise, noise)
+        ref_x.append(x - off * np.sin(h))
+        ref_y.append(y + off * np.cos(h))
+    return ref_x, ref_y, start, target
 
 
 def make_lines(batch, n=120, first=0, cfg_id=2, dmap=None):
