@@ -176,7 +176,12 @@ int pqp_default_params(pqp_params *params);
 /* Create a solver bound to CUDA device `device` able to hold `batch_max` instances of up
  * to `n_max` knots (2 <= n_max <= 511; the reference itself has no cap, see INTEGRATION.md). Owns device buffers for inputs, outputs and the
  * per-instance warm state (scaled x, z, y and rho; the OSQP workspace of
- * base_solver.hpp:62). */
+ * base_solver.hpp:62). Returns PQP_E_INVALID, before looking for a device, for params that
+ * OSQP's settings validation refuses (rho, sigma <= 0; alpha outside (0, 2); eps_abs or
+ * eps_rel < 0, or both 0; eps_prim_inf, eps_dual_inf <= 0; adaptive_rho not 0 or 1;
+ * adaptive_rho_tolerance < 1; max_iter <= 0; negative check_termination, scaling or
+ * adaptive_rho_interval), for any non-finite double, for a negative weight, for
+ * wheel_base <= 0 and for max_steering_angle outside (0, pi/2). */
 int pqp_create(const pqp_params *params, int32_t n_max, int32_t batch_max, int32_t device,
                pqp_handle **out);
 int pqp_destroy(pqp_handle *h);

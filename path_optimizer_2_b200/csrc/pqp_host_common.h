@@ -79,10 +79,23 @@ inline size_t warm_floats(int c) { return (size_t)NWARM * c * 32; }
 inline size_t scal_floats(int c) { return (size_t)NSCAL * c * 32; }
 inline size_t dy_floats(int c) { return (size_t)NDY * c * 32; }
 
+// The OSQP settings are checked as OSQP 0.6's validate_settings checks them (as recalled from its sources, which
+// are not in this tree); the vehicle and weight fields as the QP needs them: a positive curvature limit
+// tan(max_steering_angle) / wheel_base and a positive semidefinite P.
 inline bool params_valid(const pqp_params &p) {
-    return p.wheel_base > 0 && p.rho > 0 && p.sigma > 0 && p.alpha > 0 && p.alpha < 2 &&
+    const double fields[] = {p.front_length, p.rear_length, p.wheel_base, p.max_steering_angle,
+                             p.expected_safety_margin, p.weight_l, p.weight_kappa, p.weight_dkappa, p.weight_slack,
+                             p.end_l_lb, p.end_l_ub, p.rho, p.sigma, p.alpha, p.eps_abs, p.eps_rel, p.eps_prim_inf,
+                             p.eps_dual_inf, p.adaptive_rho_tolerance};
+    for (double v : fields)
+        if (!std::isfinite(v)) return false;
+    return p.wheel_base > 0 && p.max_steering_angle > 0 && p.max_steering_angle < M_PI / 2 &&
+           p.weight_l >= 0 && p.weight_kappa >= 0 && p.weight_dkappa >= 0 && p.weight_slack >= 0 &&
+           p.rho > 0 && p.sigma > 0 && p.alpha > 0 && p.alpha < 2 &&
+           p.eps_abs >= 0 && p.eps_rel >= 0 && (p.eps_abs > 0 || p.eps_rel > 0) &&
+           p.eps_prim_inf > 0 && p.eps_dual_inf > 0 && p.adaptive_rho_tolerance >= 1 &&
            p.max_iter > 0 && p.check_termination >= 0 && p.scaling >= 0 &&
-           p.adaptive_rho_interval >= 0 && p.eps_abs >= 0 && p.eps_rel >= 0;
+           (p.adaptive_rho == 0 || p.adaptive_rho == 1) && p.adaptive_rho_interval >= 0;
 }
 
 }  // namespace pqp

@@ -251,12 +251,18 @@ template <typename T> PQP_DEV void mul_abt_sym(const T (&a)[9], const T (&b)[9],
 }
 
 // ------------------------------------------------------------------ per-stage predicates
-struct StagePred {
+// gn and a22 are 0 or +-1; the clearance rows' lever arms h0, h1 are in the kernel's scalar type R (rounded to
+// FP32 they would put the FP64 instantiation's A 1e-7 relative off the oracle's whenever front_length or
+// rear_length is not a float)
+template <typename R>
+struct StagePredT {
     bool real, mid, last, act0, act1;
-    float gn, a22, h0, h1;
+    float gn, a22;
+    R h0, h1;
 };
-PQP_DEV StagePred stage_pred(int g, int n, int p, float lf, float lr) {
-    StagePred s;
+template <typename R>
+PQP_DEV StagePredT<R> stage_pred(int g, int n, int p, R lf, R lr) {
+    StagePredT<R> s;
     s.real = (g >= 1) && (g <= n);
     s.mid = (g >= 1) && (g <= n - 1);
     s.last = (g == n);
@@ -264,8 +270,8 @@ PQP_DEV StagePred stage_pred(int g, int n, int p, float lf, float lr) {
     s.act1 = (g >= 1) && (g <= p);
     s.gn = (g <= n - 1) ? -1.0f : 0.0f;
     s.a22 = s.mid ? 1.0f : 0.0f;
-    s.h0 = s.act1 ? lf : 0.0f;  // front row for precise stages, centre row (h = 0) otherwise
-    s.h1 = s.act1 ? lr : 0.0f;
+    s.h0 = s.act1 ? lf : R(0);  // front row for precise stages, centre row (h = 0) otherwise
+    s.h1 = s.act1 ? lr : R(0);
     return s;
 }
 
@@ -342,6 +348,7 @@ struct SmemStore {
 template <int C, typename real, typename Store = SmemStore<C, real>, bool Incr = false>
 struct QpWarp {
     typedef typename Vec4T<real>::type Vec4;
+    typedef StagePredT<real> StagePred;
     const KernelArgs &ka;
     Store store;
     const int lane, qp;
@@ -2012,9 +2019,14 @@ struct QpWarp {
                 nr = residuals();
                 if (can_check) {
                     status = check_termination(nr, last);
-                    // at the iteration cap the statuses of the final 10x re-check are decided on the same
-                    // residuals, but OSQP reaches that re-check only after the loop body's rho update
-                    const bool capped = last && (status == kMaxIter || status == kSolvedInacc || status == kPrimInfInacc);
+                    // OSQP stops before the rho update only where the scheduled check inside its loop body decides
+                    // the run (SOLVED, PRIMAL_INFEASIBLE). At the cap, osqp_solve's after-loop check (made when the
+                    // last iteration had no scheduled one) and its 10x re-check follow that update; they see the
+                    // same residuals and certificate terms, which the rescaling leaves unchanged. A scheduled check
+                    // has just reset to_check to check_every, which an unscheduled iteration never leaves it at.
+                    const bool scheduled = to_check == P.check_every;
+                    const bool capped = last && status != kNumerical &&
+                                        (!scheduled || status == kMaxIter || status == kSolvedInacc || status == kPrimInfInacc);
                     if (status != kUnsolved && !(capped && can_adapt)) break;
                 }
                 if (can_adapt && adapt_rho(nr)) {
