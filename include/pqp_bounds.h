@@ -27,7 +27,8 @@ extern "C" {
 /* The map's "distance" layer as grid_map holds it (demo.cpp:98-113): float, rows x cols,
  * row-major [i * cols + j]; cell (i, j) is centred at
  *   (center_x + length_x / 2 - (i + 1/2) resolution, center_y + length_y / 2 - (j + 1/2) resolution)
- * with length_x = rows * resolution, length_y = cols * resolution. Host pointer; copied at create. */
+ * with length_x = rows * resolution, length_y = cols * resolution. Host pointer; copied at create (and replaceable
+ * later, pqp_bounds_set_map below). */
 typedef struct pqp_bounds_map {
     int32_t rows, cols;
     double resolution;
@@ -107,6 +108,46 @@ int pqp_bounds_build_states_device(pqp_bounds_handle *h, const pqp_states_in *in
                                    void *stream);
 int pqp_bounds_last_kernel_ms(pqp_bounds_handle *h, float *ms);
 const char *pqp_bounds_last_error(pqp_bounds_handle *h);
+
+/* An occupancy image, from which the set_occupancy calls compute the distance layer on the GPU. cells is
+ * uint8, rows x cols, row-major, in the cell convention of pqp_bounds_map; cell k is an obstacle when
+ * cells[k] <= obstacle_max (0: obstacles are the zero pixels, as demo.cpp:98-113 measures them; 127: what
+ * sharedmap.DistanceMap thresholds). */
+typedef struct pqp_occupancy_map {
+    int32_t rows, cols;
+    double resolution;
+    double center_x, center_y;
+    const uint8_t *cells;     /* [rows * cols]: host pointer for pqp_bounds_set_occupancy, device pointer for
+                                 pqp_bounds_set_occupancy_device */
+    int32_t obstacle_max;
+} pqp_occupancy_map;
+
+/* Replacing the map of a live handle (a receding-horizon host gets a new map every tick). No call
+ * allocates. rows, cols, resolution and the centre may all change; the map must have rows, cols >= 2,
+ * rows * cols no more than the cells the handle was created with, a finite resolution > 0, finite centres
+ * and non-NULL pointers. A refused map returns PQP_E_INVALID with last_error set and leaves the handle's map
+ * (metadata and layer) untouched.
+ *
+ * The *_device calls are ordered on `stream`: work already enqueued there sees the old map, work enqueued
+ * after it the new one. Across streams the caller orders, as for every other *_device call. The host calls
+ * run on the handle's own stream and return when the new map is in place.
+ *
+ * set_map: the float distance layer as pqp_bounds_create takes it, copied.
+ * set_occupancy: the exact Euclidean distance transform of the image, on the GPU:
+ *     d2(i, j) = min over obstacle cells (i', j') of (i - i')^2 + (j - j')^2   (exact, integer)
+ *     layer    = (float)sqrt((double)d2) * (float)resolution
+ *   i.e. scipy.ndimage.distance_transform_edt(cells > obstacle_max).astype(float32) * float32(resolution) bit
+ *   for bit; obstacle cells are 0; an image with no obstacle at all gives (float)2^64 * (float)resolution per
+ *   cell, as OpenCV's precise transform does. rows, cols <= 16384. Two kernel launches, in place in the
+ *   distance layer; the host call first copies the image into a staging buffer allocated at create (1 byte
+ *   per cell).
+ * get_map: the current metadata (meta->distance is set to NULL) and, when distance is not NULL, a copy of the
+ *   layer into distance[rows * cols]; waits for all work on the device first. */
+int pqp_bounds_set_map(pqp_bounds_handle *h, const pqp_bounds_map *map);
+int pqp_bounds_set_map_device(pqp_bounds_handle *h, const pqp_bounds_map *map, void *stream);
+int pqp_bounds_set_occupancy(pqp_bounds_handle *h, const pqp_occupancy_map *occ);
+int pqp_bounds_set_occupancy_device(pqp_bounds_handle *h, const pqp_occupancy_map *occ, void *stream);
+int pqp_bounds_get_map(pqp_bounds_handle *h, pqp_bounds_map *meta, float *distance);
 
 #ifdef __cplusplus
 }

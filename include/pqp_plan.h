@@ -162,7 +162,7 @@ typedef struct pqp_plan_out {
 typedef struct pqp_plan_handle pqp_plan_handle;
 
 void pqp_plan_default_params(pqp_plan_params *p);
-/* One map (copied), 1 <= batch_max, r_max >= 3, p_max >= 4, layers_max >= 4, 2 <= n_max <= 511. All device
+/* One map (copied; replaceable with pqp_plan_set_map / pqp_plan_set_occupancy), 1 <= batch_max, r_max >= 3, p_max >= 4, layers_max >= 4, 2 <= n_max <= 511. All device
  * memory is allocated here; the plan calls allocate nothing. */
 int pqp_plan_create(const pqp_bounds_map *map, const pqp_plan_params *params, int32_t r_max, int32_t p_max,
                     int32_t layers_max, int32_t n_max, int32_t batch_max, int32_t device, pqp_plan_handle **out);
@@ -180,6 +180,19 @@ int pqp_plan_device(pqp_plan_handle *h, const pqp_plan_in *in, const pqp_plan_ou
  * r_max), and SPLINE_DEGENERATE from the samples (a polygon shorter than 1 m, of zero length, or with NaN points). */
 int pqp_plan_points(pqp_plan_handle *h, const pqp_plan_points_in *in, const pqp_plan_out *out);
 int pqp_plan_points_device(pqp_plan_handle *h, const pqp_plan_points_in *in, const pqp_plan_out *out, void *stream);
+/* Replace the map of the handle (its bounds handle's: the DP, the TENSION clearance and the bounds all read it) with
+ * no re-allocation, as pqp_bounds.h describes: a distance layer (set_map) or an occupancy image whose exact
+ * Euclidean distance transform is computed on the GPU (set_occupancy, 2 kernel launches, counted by
+ * pqp_plan_launch_count). The *_device calls are ordered on `stream` like pqp_plan_device: a plan enqueued before
+ * sees the old map, one enqueued after the new one. The host calls run on the handle's own stream and return when
+ * the map is in place. rows * cols may not exceed the cells of the map the handle was created with. get_map: the
+ * current metadata and, when distance is not NULL, a copy of the layer (waits for the device). None of these changes
+ * what pqp_plan_last_stage_ms reports. */
+int pqp_plan_set_map(pqp_plan_handle *h, const pqp_bounds_map *map);
+int pqp_plan_set_map_device(pqp_plan_handle *h, const pqp_bounds_map *map, void *stream);
+int pqp_plan_set_occupancy(pqp_plan_handle *h, const pqp_occupancy_map *occ);
+int pqp_plan_set_occupancy_device(pqp_plan_handle *h, const pqp_occupancy_map *occ, void *stream);
+int pqp_plan_get_map(pqp_plan_handle *h, pqp_bounds_map *meta, float *distance);
 /* ms[PQP_PLAN_NSTAGES] of the last call (CUDA events; waits for that call to finish). */
 int pqp_plan_last_stage_ms(pqp_plan_handle *h, float *ms);
 /* Kernel launches issued by the handle so far: the glue kernels plus those of every stage handle it owns. */

@@ -55,6 +55,22 @@ class ReferenceFrontEndT {
 
     const std::string &lastError() const { return error_; }
 
+    // Replace the map (ReferencePath::updateBounds(const Map &) takes one per call): a float distance layer, or an
+    // occupancy image (obstacle where a pixel is <= obstacle_max; 0 = demo.cpp's zero pixels) whose exact Euclidean
+    // distance transform runs on the GPU. rows * cols may not exceed the constructor's. Synchronous; false with
+    // lastError() on a refused map, which leaves the current one in place.
+    bool setMap(const float *distance, int rows, int cols, double resolution, double center_x, double center_y) {
+        if (!handle_) return false;
+        pqp_bounds_map m = {rows, cols, resolution, center_x, center_y, distance};
+        return pqp_bounds_set_map(handle_, &m) == PQP_OK || fail();
+    }
+    bool setOccupancy(const unsigned char *cells, int rows, int cols, double resolution, double center_x,
+                      double center_y, int obstacle_max = 0) {
+        if (!handle_) return false;
+        pqp_occupancy_map m = {rows, cols, resolution, center_x, center_y, cells, obstacle_max};
+        return pqp_bounds_set_occupancy(handle_, &m) == PQP_OK || fail();
+    }
+
     // buildReferenceFromSpline (reference_path_impl.cpp:314-338). `dynamic_segmentation` is
     // FLAGS_enable_dynamic_segmentation. Returns false for a zero-length reference (:316-319).
     bool buildReferenceFromSpline(const SplineRows &x_s, const SplineRows &y_s, double max_s, double delta_s_smaller,

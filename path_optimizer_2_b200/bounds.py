@@ -18,13 +18,46 @@ SPLINE_ROWS, STATE_ROWS, BOUND_ROWS = 9, 4, 6
 EXPORTED_SYMBOLS = [
     "pqp_bounds_default_params", "pqp_bounds_create", "pqp_bounds_destroy", "pqp_bounds_compute",
     "pqp_bounds_compute_device", "pqp_bounds_build_states", "pqp_bounds_build_states_device",
-    "pqp_bounds_last_kernel_ms", "pqp_bounds_last_error",
+    "pqp_bounds_last_kernel_ms", "pqp_bounds_last_error", "pqp_bounds_set_map", "pqp_bounds_set_map_device",
+    "pqp_bounds_set_occupancy", "pqp_bounds_set_occupancy_device", "pqp_bounds_get_map",
 ]
 
 
 class BoundsMap(C.Structure):
     _fields_ = [("rows", C.c_int32), ("cols", C.c_int32), ("resolution", C.c_double),
                 ("center_x", C.c_double), ("center_y", C.c_double), ("distance", C.c_void_p)]
+
+
+class OccupancyMap(C.Structure):
+    """pqp_occupancy_map: uint8 image [rows, cols]; a cell is an obstacle when its value <= obstacle_max."""
+    _fields_ = [("rows", C.c_int32), ("cols", C.c_int32), ("resolution", C.c_double),
+                ("center_x", C.c_double), ("center_y", C.c_double), ("cells", C.c_void_p),
+                ("obstacle_max", C.c_int32)]
+
+
+def distance_map(dist, resolution, center):
+    """(BoundsMap, the contiguous float32 layer it points at) for a host array."""
+    dist = np.ascontiguousarray(dist, dtype=np.float32)
+    assert dist.ndim == 2
+    return BoundsMap(dist.shape[0], dist.shape[1], float(resolution), float(center[0]), float(center[1]),
+                     dist.ctypes.data), dist
+
+
+def occupancy_map(img, resolution, center, obstacle_max):
+    """(OccupancyMap, the contiguous uint8 image it points at) for a host array."""
+    img = np.ascontiguousarray(img, dtype=np.uint8)
+    assert img.ndim == 2
+    return OccupancyMap(img.shape[0], img.shape[1], float(resolution), float(center[0]), float(center[1]),
+                        img.ctypes.data, int(obstacle_max)), img
+
+
+def get_map(fn, h, check):
+    """`fn`(h, meta, layer) read-back -> (float32 layer [rows, cols], resolution, (center_x, center_y))."""
+    meta = BoundsMap()
+    check(fn(h, C.byref(meta), None))
+    dist = np.empty((meta.rows, meta.cols), dtype=np.float32)
+    check(fn(h, C.byref(meta), dist.ctypes.data))
+    return dist, meta.resolution, (meta.center_x, meta.center_y)
 
 
 class BoundsParams(C.Structure):
@@ -75,6 +108,11 @@ def _declare(L):
     L.pqp_bounds_last_kernel_ms.argtypes = [vp, C.POINTER(C.c_float)]
     L.pqp_bounds_last_error.argtypes = [vp]
     L.pqp_bounds_last_error.restype = C.c_char_p
+    L.pqp_bounds_set_map.argtypes = [vp, C.POINTER(BoundsMap)]
+    L.pqp_bounds_set_map_device.argtypes = [vp, C.POINTER(BoundsMap), vp]
+    L.pqp_bounds_set_occupancy.argtypes = [vp, C.POINTER(OccupancyMap)]
+    L.pqp_bounds_set_occupancy_device.argtypes = [vp, C.POINTER(OccupancyMap), vp]
+    L.pqp_bounds_get_map.argtypes = [vp, C.POINTER(BoundsMap), vp]
     L._pqp_bounds_declared = True
     return L
 
@@ -154,3 +192,18 @@ class PathBounds:
         ms = C.c_float(0)
         self._check(self.L.pqp_bounds_last_kernel_ms(self.h, C.byref(ms)))
         return ms.value
+
+    def set_map(self, dist, resolution, center=(0.0, 0.0)):
+        """Replace the map with a float32 distance layer [rows, cols] (rows * cols <= the cells at construction)."""
+        m, _keep = distance_map(dist, resolution, center)
+        self._check(self.L.pqp_bounds_set_map(self.h, C.byref(m)))
+
+    def set_occupancy(self, img, resolution, center=(0.0, 0.0), obstacle_max=0):
+        """Replace the map with the exact Euclidean distance transform of a uint8 image [rows, cols], computed on the
+        GPU: cells <= obstacle_max are obstacles (0: the demo's zero pixels)."""
+        m, _keep = occupancy_map(img, resolution, center, obstacle_max)
+        self._check(self.L.pqp_bounds_set_occupancy(self.h, C.byref(m)))
+
+    def get_map(self):
+        """-> (float32 distance layer [rows, cols], resolution, (center_x, center_y)) of the current map."""
+        return get_map(self.L.pqp_bounds_get_map, self.h, self._check)

@@ -7,6 +7,7 @@
 // 48 B of bounds - it is gather-latency bound, not HBM bound (DESIGN.md §5).
 #include <cuda_runtime.h>
 
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <new>
@@ -16,6 +17,7 @@
 #include "pqp_bounds_core.cuh"
 #include "pqp_bounds_internal.h"
 #include "pqp_device_guard.h"
+#include "pqp_map_core.cuh"
 
 namespace {
 
@@ -119,11 +121,53 @@ __global__ void __launch_bounds__(64) reference_states_kernel(const StatesArgs a
 
 }  // namespace
 
+// The exact Euclidean distance transform of pqp_bounds_set_occupancy* (pqp_map_core.cuh), in place in the
+// distance layer: the column pass writes int32 g over the layer, the row pass reads its row of g into shared
+// memory and writes the row's floats back. Named namespace: the kernels keep stable names in profiles.
+namespace pqm {
+
+constexpr int kEdtColumnThreads = 128;
+constexpr int kEdtRowThreads = 64;
+
+// one thread per column: consecutive threads read consecutive bytes of a row
+__global__ void __launch_bounds__(kEdtColumnThreads) edt_column_kernel(const uint8_t *__restrict__ img, int rows, int cols,
+                                                                        int obstacle_max, int32_t *__restrict__ g) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j < cols) pqm::column_pass(img, rows, cols, j, obstacle_max, g);
+}
+
+// one block per row: the block loads the row's g, thread 0 builds the lower envelope, the block fills d2 per
+// envelope parabola and converts it to the layer's floats
+__global__ void __launch_bounds__(kEdtRowThreads) edt_row_kernel(void *layer, int rows, int cols, float res) {
+    extern __shared__ int4 edt_smem[];
+    int32_t *g = reinterpret_cast<int32_t *>(edt_smem);
+    int32_t *h = g + cols;
+    int16_t *s = reinterpret_cast<int16_t *>(h + cols);
+    int16_t *t = s + cols;
+    __shared__ int n_env;
+    const size_t row = (size_t)blockIdx.x * cols;
+    const int32_t *gin = static_cast<const int32_t *>(layer) + row;
+    for (int u = threadIdx.x; u < cols; u += blockDim.x) g[u] = gin[u];
+    __syncthreads();
+    if (threadIdx.x == 0) n_env = pqm::envelope(g, cols, s, t, h);
+    __syncthreads();
+    const int n = n_env;
+    for (int k = threadIdx.x; k < n; k += blockDim.x) pqm::fill(s, t, h, n, cols, k, g);
+    __syncthreads();
+    const int32_t inf = pqm::inf_g(rows, cols);
+    float *out = static_cast<float *>(layer) + row;
+    for (int u = threadIdx.x; u < cols; u += blockDim.x) out[u] = pqm::layer_value(g[u], inf * inf, res);
+}
+
+}  // namespace pqm
+
 struct pqp_bounds_handle {
     int device = 0;
     pqb::MapView map{};
     pqb::Params prm{};
     float *d_dist = nullptr;
+    size_t cap_cells = 0;        // cells of the map the handle was created with: the most any later map may have
+    uint8_t *d_occ = nullptr;    // [cap_cells] staging of pqp_bounds_set_occupancy's host image
     cudaStream_t stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     // staging for the host-pointer call (grown on demand)
@@ -205,6 +249,67 @@ cudaError_t grow(T **p, size_t *cap, size_t need) {
     return e;
 }
 
+void set_meta(pqp_bounds_handle *h, int rows, int cols, double res, double cx, double cy) {
+    h->map.dist = h->d_dist;
+    h->map.rows = rows;
+    h->map.cols = cols;
+    h->map.res = res;
+    h->map.inv_res = 1.0 / res;
+    h->map.half_lx = 0.5 * rows * res;
+    h->map.half_ly = 0.5 * cols * res;
+    h->map.cx = cx;
+    h->map.cy = cy;
+}
+
+// what pqp_bounds_set_map* and pqp_bounds_set_occupancy* accept; a refused map leaves the handle's map untouched
+int validate_map(pqp_bounds_handle *h, const void *m, int rows, int cols, double res, double cx, double cy,
+                 const void *data, const char *what) {
+    if (!h) return PQP_E_INVALID;
+    std::string why;
+    if (!m || !data) why = "null map or layer";
+    else if (rows < 2 || cols < 2) why = "rows, cols >= 2 required";
+    else if ((size_t)rows * (size_t)cols > h->cap_cells) why = "rows * cols exceeds the cells the handle was created with";
+    else if (!(res > 0.0) || !std::isfinite(res)) why = "resolution must be finite and > 0";
+    else if (!std::isfinite(cx) || !std::isfinite(cy)) why = "centre must be finite";
+    if (why.empty()) return PQP_OK;
+    h->err = std::string(what) + ": " + why;
+    return PQP_E_INVALID;
+}
+
+int launch_edt(pqp_bounds_handle *h, const pqp_occupancy_map *occ, const uint8_t *cells, cudaStream_t s) {
+    const int rows = occ->rows, cols = occ->cols;
+    const size_t smem = (size_t)pqm::kRowSmemPerCol * cols;
+    // the dynamic share plus the kernel's static n_env may pass the 48 KB default at any width: always opt in
+    PQB_CUDA(h, cudaFuncSetAttribute(pqm::edt_row_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    pqm::edt_column_kernel<<<(cols + pqm::kEdtColumnThreads - 1) / pqm::kEdtColumnThreads, pqm::kEdtColumnThreads, 0,
+                             s>>>(cells, rows, cols, occ->obstacle_max, reinterpret_cast<int32_t *>(h->d_dist));
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) {
+        h->err = std::string("edt_column_kernel launch: ") + cudaGetErrorString(e);
+        return PQP_E_CUDA;
+    }
+    pqm::edt_row_kernel<<<rows, pqm::kEdtRowThreads, smem, s>>>(h->d_dist, rows, cols, (float)occ->resolution);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) {
+        h->err = std::string("edt_row_kernel launch: ") + cudaGetErrorString(e) + " (" + std::to_string(rows) + " x " +
+                 std::to_string(cols) + ", " + std::to_string(smem) + " B shared)";
+        return PQP_E_CUDA;
+    }
+    return PQP_OK;
+}
+
+int validate_occupancy(pqp_bounds_handle *h, const pqp_occupancy_map *occ, const char *what) {
+    const int rc = occ ? validate_map(h, occ, occ->rows, occ->cols, occ->resolution, occ->center_x, occ->center_y,
+                                      occ->cells, what)
+                       : validate_map(h, nullptr, 0, 0, 0.0, 0.0, 0.0, nullptr, what);
+    if (rc != PQP_OK) return rc;
+    if (occ->rows > pqm::kMaxSide || occ->cols > pqm::kMaxSide) {
+        h->err = std::string(what) + ": rows and cols must be <= 16384 for the distance transform";
+        return PQP_E_INVALID;
+    }
+    return PQP_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -247,6 +352,7 @@ int pqp_bounds_create(const pqp_bounds_map *map, const pqp_bounds_params *params
     cudaError_t e = cudaSuccess;
     if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void **>(&h->d_dist), cells * sizeof(float));
     if (e == cudaSuccess) e = cudaMemcpy(h->d_dist, map->distance, cells * sizeof(float), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void **>(&h->d_occ), cells);
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking);
     if (e == cudaSuccess) e = cudaEventCreate(&h->ev0);
     if (e == cudaSuccess) e = cudaEventCreate(&h->ev1);
@@ -255,15 +361,8 @@ int pqp_bounds_create(const pqp_bounds_map *map, const pqp_bounds_params *params
         pqp_bounds_destroy(h);
         return PQP_E_CUDA;
     }
-    h->map.dist = h->d_dist;
-    h->map.rows = map->rows;
-    h->map.cols = map->cols;
-    h->map.res = map->resolution;
-    h->map.inv_res = 1.0 / map->resolution;
-    h->map.half_lx = 0.5 * map->rows * map->resolution;
-    h->map.half_ly = 0.5 * map->cols * map->resolution;
-    h->map.cx = map->center_x;
-    h->map.cy = map->center_y;
+    h->cap_cells = cells;
+    set_meta(h, map->rows, map->cols, map->resolution, map->center_x, map->center_y);
     *out = h;
     return PQP_OK;
 }
@@ -272,6 +371,7 @@ void pqp_bounds_destroy(pqp_bounds_handle *h) {
     if (!h) return;
     pqp::DeviceGuard guard_(h->device);
     cudaFree(h->d_dist);
+    cudaFree(h->d_occ);
     cudaFree(h->d_states);
     cudaFree(h->d_spline);
     cudaFree(h->d_bounds);
@@ -428,5 +528,70 @@ int pqp_bounds_last_kernel_ms(pqp_bounds_handle *h, float *ms) {
 }
 
 const char *pqp_bounds_last_error(pqp_bounds_handle *h) { return h ? h->err.c_str() : g_bounds_create_error.c_str(); }
+
+int pqp_bounds_set_map_device(pqp_bounds_handle *h, const pqp_bounds_map *map, void *stream) {
+    const int rc = map ? validate_map(h, map, map->rows, map->cols, map->resolution, map->center_x, map->center_y,
+                                      map->distance, "pqp_bounds_set_map")
+                       : validate_map(h, nullptr, 0, 0, 0.0, 0.0, 0.0, nullptr, "pqp_bounds_set_map");
+    if (rc != PQP_OK) return rc;
+    pqp::DeviceGuard guard_(h->device);
+    const size_t cells = (size_t)map->rows * map->cols;
+    PQB_CUDA(h, cudaMemcpyAsync(h->d_dist, map->distance, cells * sizeof(float), cudaMemcpyDefault,
+                                static_cast<cudaStream_t>(stream)));
+    set_meta(h, map->rows, map->cols, map->resolution, map->center_x, map->center_y);
+    return PQP_OK;
+}
+
+int pqp_bounds_set_map(pqp_bounds_handle *h, const pqp_bounds_map *map) {
+    const int rc = pqp_bounds_set_map_device(h, map, h ? h->stream : nullptr);
+    if (rc != PQP_OK) return rc;
+    pqp::DeviceGuard guard_(h->device);
+    PQB_CUDA(h, cudaStreamSynchronize(h->stream));
+    return PQP_OK;
+}
+
+int pqp_bounds_set_occupancy_device(pqp_bounds_handle *h, const pqp_occupancy_map *occ, void *stream) {
+    const int rc = validate_occupancy(h, occ, "pqp_bounds_set_occupancy_device");
+    if (rc != PQP_OK) return rc;
+    pqp::DeviceGuard guard_(h->device);
+    const int lrc = launch_edt(h, occ, occ->cells, static_cast<cudaStream_t>(stream));
+    if (lrc != PQP_OK) return lrc;
+    set_meta(h, occ->rows, occ->cols, occ->resolution, occ->center_x, occ->center_y);
+    return PQP_OK;
+}
+
+int pqp_bounds_set_occupancy(pqp_bounds_handle *h, const pqp_occupancy_map *occ) {
+    const int rc = validate_occupancy(h, occ, "pqp_bounds_set_occupancy");
+    if (rc != PQP_OK) return rc;
+    pqp::DeviceGuard guard_(h->device);
+    const size_t cells = (size_t)occ->rows * occ->cols;
+    PQB_CUDA(h, cudaMemcpyAsync(h->d_occ, occ->cells, cells, cudaMemcpyHostToDevice, h->stream));
+    const int lrc = launch_edt(h, occ, h->d_occ, h->stream);
+    if (lrc != PQP_OK) return lrc;
+    set_meta(h, occ->rows, occ->cols, occ->resolution, occ->center_x, occ->center_y);
+    PQB_CUDA(h, cudaStreamSynchronize(h->stream));
+    return PQP_OK;
+}
+
+int pqp_bounds_get_map(pqp_bounds_handle *h, pqp_bounds_map *meta, float *distance) {
+    if (!h) return PQP_E_INVALID;
+    if (!meta) {
+        h->err = "pqp_bounds_get_map: null metadata";
+        return PQP_E_INVALID;
+    }
+    pqp::DeviceGuard guard_(h->device);
+    meta->rows = h->map.rows;
+    meta->cols = h->map.cols;
+    meta->resolution = h->map.res;
+    meta->center_x = h->map.cx;
+    meta->center_y = h->map.cy;
+    meta->distance = nullptr;
+    if (distance) {
+        PQB_CUDA(h, cudaDeviceSynchronize());
+        PQB_CUDA(h, cudaMemcpy(distance, h->d_dist, (size_t)h->map.rows * h->map.cols * sizeof(float),
+                               cudaMemcpyDeviceToHost));
+    }
+    return PQP_OK;
+}
 
 }  // extern "C"

@@ -914,6 +914,40 @@ int pqp_plan_points(pqp_plan_handle *h, const pqp_plan_points_in *in, const pqp_
     return copy_results(h, out, in->batch, s);
 }
 
+int pqp_plan_set_map_device(pqp_plan_handle *h, const pqp_bounds_map *map, void *stream) {
+    if (!h) return PQP_E_INVALID;
+    PQL_SUB(h, pqp_bounds_set_map_device(h->bounds, map, stream), pqp_bounds_last_error, h->bounds);
+    return PQP_OK;
+}
+
+int pqp_plan_set_map(pqp_plan_handle *h, const pqp_bounds_map *map) {
+    if (!h) return PQP_E_INVALID;
+    PQL_SUB(h, pqp_plan_set_map_device(h, map, h->stream), pqp_plan_last_error, h);
+    pqp::DeviceGuard guard_(h->device);
+    PQL_CUDA(h, cudaStreamSynchronize(h->stream));
+    return PQP_OK;
+}
+
+int pqp_plan_set_occupancy_device(pqp_plan_handle *h, const pqp_occupancy_map *occ, void *stream) {
+    if (!h) return PQP_E_INVALID;
+    PQL_SUB(h, pqp_bounds_set_occupancy_device(h->bounds, occ, stream), pqp_bounds_last_error, h->bounds);
+    h->launches += 2;  // column and row pass of the distance transform
+    return PQP_OK;
+}
+
+int pqp_plan_set_occupancy(pqp_plan_handle *h, const pqp_occupancy_map *occ) {
+    if (!h) return PQP_E_INVALID;
+    PQL_SUB(h, pqp_bounds_set_occupancy(h->bounds, occ), pqp_bounds_last_error, h->bounds);
+    h->launches += 2;
+    return PQP_OK;
+}
+
+int pqp_plan_get_map(pqp_plan_handle *h, pqp_bounds_map *meta, float *distance) {
+    if (!h) return PQP_E_INVALID;
+    PQL_SUB(h, pqp_bounds_get_map(h->bounds, meta, distance), pqp_bounds_last_error, h->bounds);
+    return PQP_OK;
+}
+
 int pqp_plan_last_stage_ms(pqp_plan_handle *h, float *ms) {
     if (!h || !ms) return PQP_E_INVALID;
     if (!h->timed) return pfail(h, PQP_E_STATE, "no plan has run yet");

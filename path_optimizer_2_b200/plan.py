@@ -10,7 +10,10 @@ from . import abi, bounds, dp, smoother, solver
 
 EXPORTED_SYMBOLS = ["pqp_plan_default_params", "pqp_plan_create", "pqp_plan_destroy", "pqp_plan", "pqp_plan_device",
                     "pqp_plan_points", "pqp_plan_points_device", "pqp_plan_last_stage_ms", "pqp_plan_launch_count",
-                    "pqp_plan_last_error"]
+                    "pqp_plan_last_error", "pqp_plan_set_map", "pqp_plan_set_map_device", "pqp_plan_set_occupancy",
+                    "pqp_plan_set_occupancy_device", "pqp_plan_get_map"]
+# kernel launches of one set_occupancy call (the distance transform's column and row pass)
+OCCUPANCY_LAUNCHES = 2
 
 STATUS_NAMES = ("OK", "SPLINE_DEGENERATE", "TOO_MANY_POINTS", "TENSION_FAILED", "DP_VEHICLE_FAR", "POST_TOO_SHORT",
                 "POST_FAILED", "EMPTY_REFERENCE", "INIT_HEADING", "TOO_MANY_KNOTS", "BLOCKED_AT_START",
@@ -100,6 +103,11 @@ def _lib():
         L.pqp_plan_launch_count.argtypes = [vp, C.POINTER(C.c_int64)]
         L.pqp_plan_last_error.argtypes = [vp]
         L.pqp_plan_last_error.restype = C.c_char_p
+        L.pqp_plan_set_map.argtypes = [vp, C.POINTER(bounds.BoundsMap)]
+        L.pqp_plan_set_map_device.argtypes = [vp, C.POINTER(bounds.BoundsMap), vp]
+        L.pqp_plan_set_occupancy.argtypes = [vp, C.POINTER(bounds.OccupancyMap)]
+        L.pqp_plan_set_occupancy_device.argtypes = [vp, C.POINTER(bounds.OccupancyMap), vp]
+        L.pqp_plan_get_map.argtypes = [vp, C.POINTER(bounds.BoundsMap), vp]
         L._plan_declared = True
     return L
 
@@ -242,6 +250,43 @@ class Planner:
         s = stream if stream is not None else torch.cuda.current_stream(dev)
         self._check(fn(self.h, C.byref(pin), C.byref(pout), C.c_void_p(s.cuda_stream)))
         return out
+
+    def set_map(self, dist, resolution, center=(0.0, 0.0)):
+        """Replace the map with a float32 distance layer [rows, cols] (host, synchronous); rows * cols may not exceed
+        the cells of the map the planner was created with."""
+        m, _keep = bounds.distance_map(dist, resolution, center)
+        self._check(self.L.pqp_plan_set_map(self.h, C.byref(m)))
+
+    def set_occupancy(self, img, resolution, center=(0.0, 0.0), obstacle_max=0):
+        """Replace the map with the exact Euclidean distance transform, computed on the GPU, of a uint8 image
+        [rows, cols] (host, synchronous): cells <= obstacle_max are obstacles (0: the demo's zero pixels)."""
+        m, _keep = bounds.occupancy_map(img, resolution, center, obstacle_max)
+        self._check(self.L.pqp_plan_set_occupancy(self.h, C.byref(m)))
+
+    def set_map_device(self, dist, resolution, center=(0.0, 0.0), *, stream=None):
+        """As `set_map` from a torch float32 CUDA tensor [rows, cols], asynchronous on `stream` (default: the
+        current stream): plans enqueued before see the old map, plans enqueued after the new one."""
+        import torch
+        assert dist.is_cuda and dist.is_contiguous() and dist.dtype == torch.float32 and dist.dim() == 2
+        m = bounds.BoundsMap(int(dist.shape[0]), int(dist.shape[1]), float(resolution), float(center[0]),
+                             float(center[1]), dist.data_ptr())
+        s = stream if stream is not None else torch.cuda.current_stream(dist.device)
+        self._check(self.L.pqp_plan_set_map_device(self.h, C.byref(m), C.c_void_p(s.cuda_stream)))
+
+    def set_occupancy_device(self, img, resolution, center=(0.0, 0.0), obstacle_max=0, *, stream=None):
+        """As `set_occupancy` from a torch uint8 CUDA tensor [rows, cols], asynchronous on `stream` (default: the
+        current stream); the image must stay alive until the stream has run the transform."""
+        import torch
+        assert img.is_cuda and img.is_contiguous() and img.dtype == torch.uint8 and img.dim() == 2
+        m = bounds.OccupancyMap(int(img.shape[0]), int(img.shape[1]), float(resolution), float(center[0]),
+                                float(center[1]), img.data_ptr(), int(obstacle_max))
+        s = stream if stream is not None else torch.cuda.current_stream(img.device)
+        self._check(self.L.pqp_plan_set_occupancy_device(self.h, C.byref(m), C.c_void_p(s.cuda_stream)))
+
+    def get_map(self):
+        """-> (float32 distance layer [rows, cols], resolution, (center_x, center_y)) of the current map; waits for
+        the device."""
+        return bounds.get_map(self.L.pqp_plan_get_map, self.h, self._check)
 
     @property
     def last_stage_ms(self):
