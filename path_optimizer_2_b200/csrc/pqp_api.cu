@@ -19,8 +19,8 @@
 #include <vector>
 
 #include "../../include/pqp_multi.h"
-#include "pqp_device_guard.h"
 #include "pqp_host_common.h"
+#include "pqp_host_handle.h"
 
 namespace {
 
@@ -325,25 +325,13 @@ struct pqp_handle {
     float last_ms = 0.0f;
     long long launches = 0;
     std::string err;
+    pqp::Resources res;  // last member: releasing clears the members above
 };
 
 namespace {
 
 using pqp::DeviceGuard;
-
-int fail(pqp_handle *h, int code, const std::string &msg) {
-    if (h) h->err = msg;
-    else g_create_error = msg;
-    return code;
-}
-int cuda_fail(pqp_handle *h, cudaError_t e, const char *what) {
-    return fail(h, PQP_E_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
-}
-#define PQP_CUDA(h, call)                                         \
-    do {                                                          \
-        cudaError_t e_ = (call);                                  \
-        if (e_ != cudaSuccess) return cuda_fail((h), e_, #call);  \
-    } while (0)
+using pqp::fail;
 
 // the increment form is only instantiated for FP32 (the FP64 kernel is exact in either form)
 template <int C, typename real, bool Incr>
@@ -437,16 +425,11 @@ cudaError_t prepare_persistent_chunk(int chunk, size_t smem, int *bps, bool incr
 
 int validate_batch(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *out) {
     if (!h) return PQP_E_INVALID;
-    if (!in || !out) return fail(h, PQP_E_INVALID, "null batch");
-    if (!in->knots || !in->inst || !in->n || !out->sol) return fail(h, PQP_E_INVALID, "null buffer");
-    if (in->batch < 1 || in->batch > h->batch_max) return fail(h, PQP_E_INVALID, "batch out of range");
-    if (in->n_max != h->n_max) return fail(h, PQP_E_INVALID, "n_max differs from the handle's");
+    if (!in || !out) return fail(h->err, PQP_E_INVALID, "null batch");
+    if (!in->knots || !in->inst || !in->n || !out->sol) return fail(h->err, PQP_E_INVALID, "null buffer");
+    if (in->batch < 1 || in->batch > h->batch_max) return fail(h->err, PQP_E_INVALID, "batch out of range");
+    if (in->n_max != h->n_max) return fail(h->err, PQP_E_INVALID, "n_max differs from the handle's");
     return PQP_OK;
-}
-
-template <typename T>
-cudaError_t dmalloc(T **p, size_t count) {
-    return cudaMalloc(reinterpret_cast<void **>(p), count * sizeof(T));
 }
 
 // device pointers in `in`/`out`; asynchronous
@@ -491,37 +474,64 @@ int run_device(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *out, 
     ka.scal = esc ? h->e_scal : h->d_scal;
     ka.dy = esc ? h->e_dy : h->d_dy;
     ka.rho_state = esc ? h->e_rho : h->d_rho;
-    if (timed) PQP_CUDA(h, cudaEventRecord(h->ev0, s));
+    if (timed) PQP_CUDA(h->err, cudaEventRecord(h->ev0, s));
     if (esc || h->fp64) {
         if (!h->prepared64) {
             int bps = 0;
-            PQP_CUDA(h, prepare_chunk<double>(h->chunk, h->smem_bytes64, &bps));
+            PQP_CUDA(h->err, prepare_chunk<double>(h->chunk, h->smem_bytes64, &bps));
             h->prepared64 = true;
         }
         if (h->chunk == 16) {
             const int ctas = std::min(ka.batch, 2 * h->sm_count);
-            if (!h->d_state64) PQP_CUDA(h, dmalloc(&h->d_state64, (size_t)2 * h->sm_count * pqp::smem_floats(16)));
+            if (!h->d_state64) PQP_CUDA(h->err, h->res.alloc(h->d_state64, (size_t)2 * h->sm_count * pqp::smem_floats(16)));
             pqp_admm_kernel_gmem<16, double, false><<<ctas, 32, 0, s>>>(ka, h->d_state64);
-            PQP_CUDA(h, cudaGetLastError());
+            PQP_CUDA(h->err, cudaGetLastError());
         } else {
-            PQP_CUDA(h, launch_chunk<double>(h->chunk, ka, h->smem_bytes64, s));
+            PQP_CUDA(h->err, launch_chunk<double>(h->chunk, ka, h->smem_bytes64, s));
         }
     } else if (h->persistent) {
         // one work counter per concurrently running launch (pipeline chunk); counters rotate
         int *ctr = h->d_counters + (h->counter_next++ % pqp_handle::kCounters);
-        PQP_CUDA(h, cudaMemsetAsync(ctr, 0, sizeof(int), s));
+        PQP_CUDA(h->err, cudaMemsetAsync(ctr, 0, sizeof(int), s));
         ka.work_counter = ctr;
-        PQP_CUDA(h, launch_persistent_chunk(h->chunk, ka, h->smem_bytes, s, h->sm_count * h->warps_per_sm, h->incr));
+        PQP_CUDA(h->err, launch_persistent_chunk(h->chunk, ka, h->smem_bytes, s, h->sm_count * h->warps_per_sm, h->incr));
     } else {
-        PQP_CUDA(h, launch_chunk<float>(h->chunk, ka, h->smem_bytes, s, h->incr));
+        PQP_CUDA(h->err, launch_chunk<float>(h->chunk, ka, h->smem_bytes, s, h->incr));
     }
-    if (timed) PQP_CUDA(h, cudaEventRecord(h->ev1, s));
+    if (timed) PQP_CUDA(h->err, cudaEventRecord(h->ev1, s));
     h->launches++;
     if (!esc) {
         h->solved = true;
         if (qp0 == 0) h->last_batch = in->batch;
     }
     return PQP_OK;
+}
+
+// The FP64 escalation's side batch of esc_cap instances, all or nothing: after a failed allocation it has no
+// buffers, so the next escalation allocates again instead of running with a missing one.
+cudaError_t alloc_escalation(pqp_handle *h) {
+    const size_t E = h->esc_cap, nmax = h->n_max, c = h->chunk, nvm = 6 * nmax - 1, mm = 6 * nmax + 2;
+    pqp::Resources &r = h->res;
+    return r.group([&] {
+        cudaError_t e = r.alloc(h->e_knots, E * PQP_NFIELDS * nmax);
+        if (e == cudaSuccess) e = r.alloc(h->e_inst, E * PQP_NINST);
+        if (e == cudaSuccess) e = r.alloc(h->e_n, E);
+        if (e == cudaSuccess) e = r.alloc(h->e_p, E);
+        if (e == cudaSuccess) e = r.alloc(h->e_sol, E * 4 * nmax);
+        if (e == cudaSuccess) e = r.alloc(h->e_cost, E);
+        if (e == cudaSuccess) e = r.alloc(h->e_status, E);
+        if (e == cudaSuccess) e = r.alloc(h->e_iters, E);
+        if (e == cudaSuccess) e = r.alloc(h->e_info, E * PQP_NINFO);
+        if (e == cudaSuccess) e = r.alloc(h->e_xf, E * nvm);
+        if (e == cudaSuccess) e = r.alloc(h->e_yf, E * mm);
+        if (e == cudaSuccess) e = r.alloc(h->e_zf, E * mm);
+        if (e == cudaSuccess) e = r.alloc(h->e_warm, E * pqp::warm_floats(c) * sizeof(double));
+        if (e == cudaSuccess) e = r.alloc(h->e_scal, E * pqp::scal_floats(c) * sizeof(double));
+        if (e == cudaSuccess) e = r.alloc(h->e_dy, E * pqp::dy_floats(c) * sizeof(double));
+        if (e == cudaSuccess) e = r.alloc(h->e_rho, E * sizeof(double));
+        if (e == cudaSuccess) e = r.alloc(h->e_slots, E);
+        return e;
+    });
 }
 
 // Instances the FP32 kernel could neither solve nor certify (iteration cap reached while the
@@ -543,24 +553,7 @@ int escalate_fp64(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *ou
     const size_t nvm = 6 * (size_t)nmax - 1, mm = 6 * (size_t)nmax + 2;
     if (!h->e_knots) {
         h->esc_cap = h->batch_max < 256 ? h->batch_max : 256;
-        const size_t E = h->esc_cap;
-        PQP_CUDA(h, dmalloc(&h->e_knots, E * PQP_NFIELDS * nmax));
-        PQP_CUDA(h, dmalloc(&h->e_inst, E * PQP_NINST));
-        PQP_CUDA(h, dmalloc(&h->e_n, E));
-        PQP_CUDA(h, dmalloc(&h->e_p, E));
-        PQP_CUDA(h, dmalloc(&h->e_sol, E * 4 * nmax));
-        PQP_CUDA(h, dmalloc(&h->e_cost, E));
-        PQP_CUDA(h, dmalloc(&h->e_status, E));
-        PQP_CUDA(h, dmalloc(&h->e_iters, E));
-        PQP_CUDA(h, dmalloc(&h->e_info, E * PQP_NINFO));
-        PQP_CUDA(h, dmalloc(&h->e_xf, E * nvm));
-        PQP_CUDA(h, dmalloc(&h->e_yf, E * mm));
-        PQP_CUDA(h, dmalloc(&h->e_zf, E * mm));
-        PQP_CUDA(h, cudaMalloc(&h->e_warm, E * pqp::warm_floats(c) * sizeof(double)));
-        PQP_CUDA(h, cudaMalloc(&h->e_scal, E * pqp::scal_floats(c) * sizeof(double)));
-        PQP_CUDA(h, cudaMalloc(&h->e_dy, E * pqp::dy_floats(c) * sizeof(double)));
-        PQP_CUDA(h, cudaMalloc(&h->e_rho, E * sizeof(double)));
-        PQP_CUDA(h, dmalloc(&h->e_slots, E));
+        PQP_CUDA(h->err, alloc_escalation(h));
     }
     cudaStream_t s = h->stream;
     const size_t kb = (size_t)PQP_NFIELDS * nmax;
@@ -569,44 +562,44 @@ int escalate_fp64(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *ou
         for (int j = 0; j < E; ++j) {
             const int b = idx[start + j];
             // inputs come from the handle's device copy (valid for both host-batch and NULL-batch calls)
-            PQP_CUDA(h, cudaMemcpyAsync(h->e_knots + j * kb, h->d_knots + b * kb, kb * sizeof(double), cudaMemcpyDeviceToDevice, s));
-            PQP_CUDA(h, cudaMemcpyAsync(h->e_inst + (size_t)j * PQP_NINST, h->d_inst + (size_t)b * PQP_NINST, PQP_NINST * sizeof(double), cudaMemcpyDeviceToDevice, s));
-            PQP_CUDA(h, cudaMemcpyAsync(h->e_n + j, h->d_n + b, sizeof(int), cudaMemcpyDeviceToDevice, s));
-            if (h->d_p_valid) PQP_CUDA(h, cudaMemcpyAsync(h->e_p + j, h->d_p + b, sizeof(int), cudaMemcpyDeviceToDevice, s));
+            PQP_CUDA(h->err, cudaMemcpyAsync(h->e_knots + j * kb, h->d_knots + b * kb, kb * sizeof(double), cudaMemcpyDeviceToDevice, s));
+            PQP_CUDA(h->err, cudaMemcpyAsync(h->e_inst + (size_t)j * PQP_NINST, h->d_inst + (size_t)b * PQP_NINST, PQP_NINST * sizeof(double), cudaMemcpyDeviceToDevice, s));
+            PQP_CUDA(h->err, cudaMemcpyAsync(h->e_n + j, h->d_n + b, sizeof(int), cudaMemcpyDeviceToDevice, s));
+            if (h->d_p_valid) PQP_CUDA(h->err, cudaMemcpyAsync(h->e_p + j, h->d_p + b, sizeof(int), cudaMemcpyDeviceToDevice, s));
         }
-        PQP_CUDA(h, cudaMemsetAsync(h->e_xf, 0, (size_t)E * nvm * sizeof(double), s));
-        PQP_CUDA(h, cudaMemsetAsync(h->e_yf, 0, (size_t)E * mm * sizeof(double), s));
-        PQP_CUDA(h, cudaMemsetAsync(h->e_zf, 0, (size_t)E * mm * sizeof(double), s));
+        PQP_CUDA(h->err, cudaMemsetAsync(h->e_xf, 0, (size_t)E * nvm * sizeof(double), s));
+        PQP_CUDA(h->err, cudaMemsetAsync(h->e_yf, 0, (size_t)E * mm * sizeof(double), s));
+        PQP_CUDA(h->err, cudaMemsetAsync(h->e_zf, 0, (size_t)E * mm * sizeof(double), s));
         pqp_batch_in din = {E, nmax, h->e_knots, h->e_inst, h->e_n, h->d_p_valid ? h->e_p : nullptr};
         pqp_batch_out dout = {h->e_sol, h->e_cost, h->e_status, h->e_iters, h->e_xf, h->e_yf, h->e_zf, h->e_info};
         int rc = run_device(h, &din, &dout, 0, s, false, 0, true, nullptr);
         if (rc) return rc;
         for (int j = 0; j < E; ++j) {
             const int b = idx[start + j];
-            PQP_CUDA(h, cudaMemcpyAsync(out->sol + (size_t)b * 4 * nmax, h->e_sol + (size_t)j * 4 * nmax, 4 * (size_t)nmax * sizeof(double), cudaMemcpyDeviceToHost, s));
-            if (out->cost) PQP_CUDA(h, cudaMemcpyAsync(out->cost + b, h->e_cost + j, sizeof(double), cudaMemcpyDeviceToHost, s));
-            if (out->status) PQP_CUDA(h, cudaMemcpyAsync(out->status + b, h->e_status + j, sizeof(int), cudaMemcpyDeviceToHost, s));
-            if (out->iters) PQP_CUDA(h, cudaMemcpyAsync(out->iters + b, h->e_iters + j, sizeof(int), cudaMemcpyDeviceToHost, s));
-            if (out->info) PQP_CUDA(h, cudaMemcpyAsync(out->info + (size_t)b * PQP_NINFO, h->e_info + (size_t)j * PQP_NINFO, PQP_NINFO * sizeof(double), cudaMemcpyDeviceToHost, s));
-            if (out->x_full) PQP_CUDA(h, cudaMemcpyAsync(out->x_full + b * nvm, h->e_xf + j * nvm, nvm * sizeof(double), cudaMemcpyDeviceToHost, s));
-            if (out->y_full) PQP_CUDA(h, cudaMemcpyAsync(out->y_full + b * mm, h->e_yf + j * mm, mm * sizeof(double), cudaMemcpyDeviceToHost, s));
-            if (out->z_full) PQP_CUDA(h, cudaMemcpyAsync(out->z_full + b * mm, h->e_zf + j * mm, mm * sizeof(double), cudaMemcpyDeviceToHost, s));
+            PQP_CUDA(h->err, cudaMemcpyAsync(out->sol + (size_t)b * 4 * nmax, h->e_sol + (size_t)j * 4 * nmax, 4 * (size_t)nmax * sizeof(double), cudaMemcpyDeviceToHost, s));
+            if (out->cost) PQP_CUDA(h->err, cudaMemcpyAsync(out->cost + b, h->e_cost + j, sizeof(double), cudaMemcpyDeviceToHost, s));
+            if (out->status) PQP_CUDA(h->err, cudaMemcpyAsync(out->status + b, h->e_status + j, sizeof(int), cudaMemcpyDeviceToHost, s));
+            if (out->iters) PQP_CUDA(h->err, cudaMemcpyAsync(out->iters + b, h->e_iters + j, sizeof(int), cudaMemcpyDeviceToHost, s));
+            if (out->info) PQP_CUDA(h->err, cudaMemcpyAsync(out->info + (size_t)b * PQP_NINFO, h->e_info + (size_t)j * PQP_NINFO, PQP_NINFO * sizeof(double), cudaMemcpyDeviceToHost, s));
+            if (out->x_full) PQP_CUDA(h->err, cudaMemcpyAsync(out->x_full + b * nvm, h->e_xf + j * nvm, nvm * sizeof(double), cudaMemcpyDeviceToHost, s));
+            if (out->y_full) PQP_CUDA(h->err, cudaMemcpyAsync(out->y_full + b * mm, h->e_yf + j * mm, mm * sizeof(double), cudaMemcpyDeviceToHost, s));
+            if (out->z_full) PQP_CUDA(h->err, cudaMemcpyAsync(out->z_full + b * mm, h->e_zf + j * mm, mm * sizeof(double), cudaMemcpyDeviceToHost, s));
             // keep the device-resident results coherent too (resolve(NULL) linearises about d_sol)
-            PQP_CUDA(h, cudaMemcpyAsync(h->d_sol + (size_t)b * 4 * nmax, h->e_sol + (size_t)j * 4 * nmax, 4 * (size_t)nmax * sizeof(double), cudaMemcpyDeviceToDevice, s));
-            PQP_CUDA(h, cudaMemcpyAsync(h->d_status + b, h->e_status + j, sizeof(int), cudaMemcpyDeviceToDevice, s));
-            PQP_CUDA(h, cudaMemcpyAsync(h->d_cost + b, h->e_cost + j, sizeof(double), cudaMemcpyDeviceToDevice, s));
-            PQP_CUDA(h, cudaMemcpyAsync(h->d_iters + b, h->e_iters + j, sizeof(int), cudaMemcpyDeviceToDevice, s));
+            PQP_CUDA(h->err, cudaMemcpyAsync(h->d_sol + (size_t)b * 4 * nmax, h->e_sol + (size_t)j * 4 * nmax, 4 * (size_t)nmax * sizeof(double), cudaMemcpyDeviceToDevice, s));
+            PQP_CUDA(h->err, cudaMemcpyAsync(h->d_status + b, h->e_status + j, sizeof(int), cudaMemcpyDeviceToDevice, s));
+            PQP_CUDA(h->err, cudaMemcpyAsync(h->d_cost + b, h->e_cost + j, sizeof(double), cudaMemcpyDeviceToDevice, s));
+            PQP_CUDA(h->err, cudaMemcpyAsync(h->d_iters + b, h->e_iters + j, sizeof(int), cudaMemcpyDeviceToDevice, s));
         }
         // the warm slots of these instances adopt the FP64 run's scaled iterates and rho
         if (!h->cold_only) {
-            PQP_CUDA(h, cudaMemcpyAsync(h->e_slots, idx.data() + start, (size_t)E * sizeof(int), cudaMemcpyHostToDevice, s));
+            PQP_CUDA(h->err, cudaMemcpyAsync(h->e_slots, idx.data() + start, (size_t)E * sizeof(int), cudaMemcpyHostToDevice, s));
             const size_t wf = pqp::warm_floats(c);
             adopt_warm_kernel<<<dim3((unsigned)((wf + 255) / 256), (unsigned)E), 256, 0, s>>>(
                 E, wf, h->e_slots, static_cast<const double *>(h->e_warm), static_cast<const double *>(h->e_rho),
                 static_cast<float *>(h->d_warm), static_cast<float *>(h->d_rho));
-            PQP_CUDA(h, cudaGetLastError());
+            PQP_CUDA(h->err, cudaGetLastError());
         }
-        PQP_CUDA(h, cudaStreamSynchronize(s));
+        PQP_CUDA(h->err, cudaStreamSynchronize(s));
         h->escalated += E;
     }
     return PQP_OK;
@@ -646,14 +639,14 @@ int run_host_streamed(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out
     }
     cudaStream_t sk = h->streams[0], sc = h->streams[1], sd = h->streams[2];
     for (int c = 0; c < pqp_handle::kStreams; ++c) h->h_done[c] = 0;
-    PQP_CUDA(h, cudaMemsetAsync(h->d_ready, 0, pqp_handle::kStreams * sizeof(int), sk));
-    PQP_CUDA(h, cudaMemsetAsync(h->d_done, 0, pqp_handle::kStreams * sizeof(int), sk));
-    if (out->x_full) PQP_CUDA(h, cudaMemsetAsync(h->d_xf, 0, (size_t)B * nvm * sizeof(double), sk));
-    if (out->y_full) PQP_CUDA(h, cudaMemsetAsync(h->d_yf, 0, (size_t)B * mm * sizeof(double), sk));
-    if (out->z_full) PQP_CUDA(h, cudaMemsetAsync(h->d_zf, 0, (size_t)B * mm * sizeof(double), sk));
-    PQP_CUDA(h, cudaEventRecord(h->ev0, sk));
-    PQP_CUDA(h, cudaStreamWaitEvent(sc, h->ev0, 0));
-    PQP_CUDA(h, cudaStreamWaitEvent(sd, h->ev0, 0));
+    PQP_CUDA(h->err, cudaMemsetAsync(h->d_ready, 0, pqp_handle::kStreams * sizeof(int), sk));
+    PQP_CUDA(h->err, cudaMemsetAsync(h->d_done, 0, pqp_handle::kStreams * sizeof(int), sk));
+    if (out->x_full) PQP_CUDA(h->err, cudaMemsetAsync(h->d_xf, 0, (size_t)B * nvm * sizeof(double), sk));
+    if (out->y_full) PQP_CUDA(h->err, cudaMemsetAsync(h->d_yf, 0, (size_t)B * mm * sizeof(double), sk));
+    if (out->z_full) PQP_CUDA(h->err, cudaMemsetAsync(h->d_zf, 0, (size_t)B * mm * sizeof(double), sk));
+    PQP_CUDA(h->err, cudaEventRecord(h->ev0, sk));
+    PQP_CUDA(h->err, cudaStreamWaitEvent(sc, h->ev0, 0));
+    PQP_CUDA(h->err, cudaStreamWaitEvent(sd, h->ev0, 0));
     pqp_batch_in din = {B, nmax, h->d_knots, h->d_inst, h->d_n, (h->d_p_valid = in->p != nullptr) ? h->d_p : nullptr};
     pqp_batch_out dout = {h->d_sol, h->d_cost, h->d_status, h->d_iters, out->x_full ? h->d_xf : nullptr,
                           out->y_full ? h->d_yf : nullptr, out->z_full ? h->d_zf : nullptr, h->d_info};
@@ -669,13 +662,13 @@ int run_host_streamed(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out
     for (int c = 0; c < nchunks; ++c) {
         const int lo = lo_of[c], hi = lo_of[c + 1];
         const size_t nb = (size_t)(hi - lo);
-        PQP_CUDA(h, cudaMemcpyAsync(h->d_knots + (size_t)lo * PQP_NFIELDS * nmax, in->knots + (size_t)lo * PQP_NFIELDS * nmax,
+        PQP_CUDA(h->err, cudaMemcpyAsync(h->d_knots + (size_t)lo * PQP_NFIELDS * nmax, in->knots + (size_t)lo * PQP_NFIELDS * nmax,
                                     nb * PQP_NFIELDS * nmax * sizeof(double), cudaMemcpyHostToDevice, sc));
-        PQP_CUDA(h, cudaMemcpyAsync(h->d_inst + (size_t)lo * PQP_NINST, in->inst + (size_t)lo * PQP_NINST,
+        PQP_CUDA(h->err, cudaMemcpyAsync(h->d_inst + (size_t)lo * PQP_NINST, in->inst + (size_t)lo * PQP_NINST,
                                     nb * PQP_NINST * sizeof(double), cudaMemcpyHostToDevice, sc));
-        PQP_CUDA(h, cudaMemcpyAsync(h->d_n + lo, in->n + lo, nb * sizeof(int), cudaMemcpyHostToDevice, sc));
-        if (in->p) PQP_CUDA(h, cudaMemcpyAsync(h->d_p + lo, in->p + lo, nb * sizeof(int), cudaMemcpyHostToDevice, sc));
-        PQP_CUDA(h, cudaMemsetAsync(h->d_ready + c, 1, sizeof(int), sc));  // "chunk c has landed"
+        PQP_CUDA(h->err, cudaMemcpyAsync(h->d_n + lo, in->n + lo, nb * sizeof(int), cudaMemcpyHostToDevice, sc));
+        if (in->p) PQP_CUDA(h->err, cudaMemcpyAsync(h->d_p + lo, in->p + lo, nb * sizeof(int), cudaMemcpyHostToDevice, sc));
+        PQP_CUDA(h->err, cudaMemsetAsync(h->d_ready + c, 1, sizeof(int), sc));  // "chunk c has landed"
     }
     int rc = run_device(h, &din, &dout, mode, sk, false, 0, false, h->d_flags, &sl);
     if (rc) return rc;
@@ -693,27 +686,40 @@ int run_host_streamed(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out
             const struct timespec nap = {0, 20000};
             nanosleep(&nap, nullptr);
         }
-        PQP_CUDA(h, cudaMemcpyAsync(h->h_status + lo, h->d_status + lo, nb * sizeof(int), cudaMemcpyDeviceToHost, sd));
-        PQP_CUDA(h, cudaMemcpyAsync(h->h_flags + lo, h->d_flags + lo, nb * sizeof(int), cudaMemcpyDeviceToHost, sd));
-        PQP_CUDA(h, cudaMemcpyAsync(out->sol + (size_t)lo * 4 * nmax, h->d_sol + (size_t)lo * 4 * nmax, nb * 4 * nmax * sizeof(double), cudaMemcpyDeviceToHost, sd));
-        if (out->cost) PQP_CUDA(h, cudaMemcpyAsync(out->cost + lo, h->d_cost + lo, nb * sizeof(double), cudaMemcpyDeviceToHost, sd));
-        if (out->status) PQP_CUDA(h, cudaMemcpyAsync(out->status + lo, h->d_status + lo, nb * sizeof(int), cudaMemcpyDeviceToHost, sd));
-        if (out->iters) PQP_CUDA(h, cudaMemcpyAsync(out->iters + lo, h->d_iters + lo, nb * sizeof(int), cudaMemcpyDeviceToHost, sd));
-        if (out->info) PQP_CUDA(h, cudaMemcpyAsync(out->info + (size_t)lo * PQP_NINFO, h->d_info + (size_t)lo * PQP_NINFO, nb * PQP_NINFO * sizeof(double), cudaMemcpyDeviceToHost, sd));
-        if (out->x_full) PQP_CUDA(h, cudaMemcpyAsync(out->x_full + lo * nvm, h->d_xf + lo * nvm, nb * nvm * sizeof(double), cudaMemcpyDeviceToHost, sd));
-        if (out->y_full) PQP_CUDA(h, cudaMemcpyAsync(out->y_full + lo * mm, h->d_yf + lo * mm, nb * mm * sizeof(double), cudaMemcpyDeviceToHost, sd));
-        if (out->z_full) PQP_CUDA(h, cudaMemcpyAsync(out->z_full + lo * mm, h->d_zf + lo * mm, nb * mm * sizeof(double), cudaMemcpyDeviceToHost, sd));
+        PQP_CUDA(h->err, cudaMemcpyAsync(h->h_status + lo, h->d_status + lo, nb * sizeof(int), cudaMemcpyDeviceToHost, sd));
+        PQP_CUDA(h->err, cudaMemcpyAsync(h->h_flags + lo, h->d_flags + lo, nb * sizeof(int), cudaMemcpyDeviceToHost, sd));
+        PQP_CUDA(h->err, cudaMemcpyAsync(out->sol + (size_t)lo * 4 * nmax, h->d_sol + (size_t)lo * 4 * nmax, nb * 4 * nmax * sizeof(double), cudaMemcpyDeviceToHost, sd));
+        if (out->cost) PQP_CUDA(h->err, cudaMemcpyAsync(out->cost + lo, h->d_cost + lo, nb * sizeof(double), cudaMemcpyDeviceToHost, sd));
+        if (out->status) PQP_CUDA(h->err, cudaMemcpyAsync(out->status + lo, h->d_status + lo, nb * sizeof(int), cudaMemcpyDeviceToHost, sd));
+        if (out->iters) PQP_CUDA(h->err, cudaMemcpyAsync(out->iters + lo, h->d_iters + lo, nb * sizeof(int), cudaMemcpyDeviceToHost, sd));
+        if (out->info) PQP_CUDA(h->err, cudaMemcpyAsync(out->info + (size_t)lo * PQP_NINFO, h->d_info + (size_t)lo * PQP_NINFO, nb * PQP_NINFO * sizeof(double), cudaMemcpyDeviceToHost, sd));
+        if (out->x_full) PQP_CUDA(h->err, cudaMemcpyAsync(out->x_full + lo * nvm, h->d_xf + lo * nvm, nb * nvm * sizeof(double), cudaMemcpyDeviceToHost, sd));
+        if (out->y_full) PQP_CUDA(h->err, cudaMemcpyAsync(out->y_full + lo * mm, h->d_yf + lo * mm, nb * mm * sizeof(double), cudaMemcpyDeviceToHost, sd));
+        if (out->z_full) PQP_CUDA(h->err, cudaMemcpyAsync(out->z_full + lo * mm, h->d_zf + lo * mm, nb * mm * sizeof(double), cudaMemcpyDeviceToHost, sd));
     }
     h->last_batch = B;
-    PQP_CUDA(h, cudaStreamSynchronize(sk));
-    PQP_CUDA(h, cudaStreamSynchronize(sc));
-    PQP_CUDA(h, cudaEventRecord(h->ev1, sd));
-    PQP_CUDA(h, cudaStreamSynchronize(sd));
-    PQP_CUDA(h, cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1));
+    PQP_CUDA(h->err, cudaStreamSynchronize(sk));
+    PQP_CUDA(h->err, cudaStreamSynchronize(sc));
+    PQP_CUDA(h->err, cudaEventRecord(h->ev1, sd));
+    PQP_CUDA(h->err, cudaStreamSynchronize(sd));
+    PQP_CUDA(h->err, cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1));
     for (int i = 0; i < PQP_NSTAGES; ++i) h->stage_ms[i] = -1.0f;  // copies and kernel overlap: only the total is defined
     h->stage_ms[PQP_STAGE_TOTAL] = h->last_ms;
     if (!h->fp64 && h->escalate && mode == 0) return escalate_fp64(h, in, out, B);
     return PQP_OK;
+}
+
+// staging of the host-pointer pqp_frenet_to_cartesian, all or nothing (allocated on its first call)
+cudaError_t alloc_frenet_staging(pqp_handle *h) {
+    const size_t B = h->batch_max, nm = h->n_max;
+    pqp::Resources &r = h->res;
+    return r.group([&] {
+        cudaError_t e = r.alloc(h->d_ref, B * 3 * nm);
+        if (e == cudaSuccess) e = r.alloc(h->d_xy, B * 3 * nm);
+        if (e == cudaSuccess) e = r.alloc(h->d_sol2, B * 4 * nm);
+        if (e == cudaSuccess) e = r.alloc(h->d_n2, B);
+        return e;
+    });
 }
 
 int run_host(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *out, int mode) {
@@ -727,36 +733,36 @@ int run_host(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *out, in
         if (rc) return rc;
         B = in->batch;
         for (int b = 0; b < B; ++b) {
-            if (in->n[b] < 2 || in->n[b] > nmax) return fail(h, PQP_E_INVALID, "n[b] must be in [2, n_max]");
-            if (in->p && (in->p[b] < 0 || in->p[b] > in->n[b])) return fail(h, PQP_E_INVALID, "p[b] must be in [0, n[b]]");
+            if (in->n[b] < 2 || in->n[b] > nmax) return fail(h->err, PQP_E_INVALID, "n[b] must be in [2, n_max]");
+            if (in->p && (in->p[b] < 0 || in->p[b] > in->n[b])) return fail(h->err, PQP_E_INVALID, "p[b] must be in [0, n[b]]");
         }
-        if (mode == 1 && h->cold_only) return fail(h, PQP_E_STATE, "cold-only handle (option bit 128) keeps no warm state");
-        if (mode == 1 && (!h->solved || B != h->last_batch)) return fail(h, PQP_E_STATE, "resolve needs a previous solve of the same batch");
+        if (mode == 1 && h->cold_only) return fail(h->err, PQP_E_STATE, "cold-only handle (option bit 128) keeps no warm state");
+        if (mode == 1 && (!h->solved || B != h->last_batch)) return fail(h->err, PQP_E_STATE, "resolve needs a previous solve of the same batch");
         h->host_inputs_resident = true;
         h->d_p_valid = in->p != nullptr;
         if (h->persistent && B >= 512) {
             const size_t nvm0 = 6 * (size_t)nmax - 1, mm0 = 6 * (size_t)nmax + 2;
-            if (out->x_full && !h->d_xf) PQP_CUDA(h, dmalloc(&h->d_xf, (size_t)h->batch_max * nvm0));
-            if (out->y_full && !h->d_yf) PQP_CUDA(h, dmalloc(&h->d_yf, (size_t)h->batch_max * mm0));
-            if (out->z_full && !h->d_zf) PQP_CUDA(h, dmalloc(&h->d_zf, (size_t)h->batch_max * mm0));
+            if (out->x_full && !h->d_xf) PQP_CUDA(h->err, h->res.alloc(h->d_xf, (size_t)h->batch_max * nvm0));
+            if (out->y_full && !h->d_yf) PQP_CUDA(h->err, h->res.alloc(h->d_yf, (size_t)h->batch_max * mm0));
+            if (out->z_full && !h->d_zf) PQP_CUDA(h->err, h->res.alloc(h->d_zf, (size_t)h->batch_max * mm0));
             return run_host_streamed(h, in, out, mode, B);
         }
     } else {
-        if (mode != 1) return fail(h, PQP_E_INVALID, "null batch");
-        if (h->cold_only) return fail(h, PQP_E_STATE, "cold-only handle (option bit 128) keeps no warm state");
-        if (!out || !out->sol) return fail(h, PQP_E_INVALID, "null output");
-        if (!h->solved || !h->host_inputs_resident) return fail(h, PQP_E_STATE, "resolve(NULL) needs a previous host-API solve");
+        if (mode != 1) return fail(h->err, PQP_E_INVALID, "null batch");
+        if (h->cold_only) return fail(h->err, PQP_E_STATE, "cold-only handle (option bit 128) keeps no warm state");
+        if (!out || !out->sol) return fail(h->err, PQP_E_INVALID, "null output");
+        if (!h->solved || !h->host_inputs_resident) return fail(h->err, PQP_E_STATE, "resolve(NULL) needs a previous host-API solve");
         B = h->last_batch;
         const int threads = 256, blocks = (B * nmax + threads - 1) / threads;
         relinearise_kernel<<<blocks, threads, 0, s>>>(B, nmax, h->d_sol, h->d_knots);
-        PQP_CUDA(h, cudaGetLastError());
+        PQP_CUDA(h->err, cudaGetLastError());
         h->launches++;
     }
     // optional full outputs are allocated on first use
     const size_t nvm = 6 * (size_t)nmax - 1, mm = 6 * (size_t)nmax + 2;
-    if (out->x_full && !h->d_xf) PQP_CUDA(h, dmalloc(&h->d_xf, (size_t)h->batch_max * nvm));
-    if (out->y_full && !h->d_yf) PQP_CUDA(h, dmalloc(&h->d_yf, (size_t)h->batch_max * mm));
-    if (out->z_full && !h->d_zf) PQP_CUDA(h, dmalloc(&h->d_zf, (size_t)h->batch_max * mm));
+    if (out->x_full && !h->d_xf) PQP_CUDA(h->err, h->res.alloc(h->d_xf, (size_t)h->batch_max * nvm));
+    if (out->y_full && !h->d_yf) PQP_CUDA(h->err, h->res.alloc(h->d_yf, (size_t)h->batch_max * mm));
+    if (out->z_full && !h->d_zf) PQP_CUDA(h->err, h->res.alloc(h->d_zf, (size_t)h->batch_max * mm));
     // Chunked pipeline, one stream per chunk: chunk c+1's H2D copy and chunk c-1's D2H copy
     // overlap chunk c's kernel (fully asynchronous when the caller's buffers are pinned), and
     // because every chunk's kernel sits in its own stream the block scheduler back-fills SMs
@@ -770,25 +776,25 @@ int run_host(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *out, in
     const int per = (B + nchunks - 1) / nchunks;
     cudaStream_t *streams = h->streams;
     // every chunk stream starts after whatever the handle's main stream has queued so far
-    PQP_CUDA(h, cudaEventRecord(h->ev0, streams[0]));
-    for (int c = 1; c < nchunks; ++c) PQP_CUDA(h, cudaStreamWaitEvent(streams[c], h->ev0, 0));
+    PQP_CUDA(h->err, cudaEventRecord(h->ev0, streams[0]));
+    for (int c = 1; c < nchunks; ++c) PQP_CUDA(h->err, cudaStreamWaitEvent(streams[c], h->ev0, 0));
     for (int c = 0; c < nchunks; ++c) {
         const int lo = c * per, hi = (lo + per < B) ? lo + per : B;
         if (lo >= hi) break;
         const size_t nb = (size_t)(hi - lo);
         cudaStream_t s = streams[c];
         if (in) {
-            PQP_CUDA(h, cudaMemcpyAsync(h->d_knots + (size_t)lo * PQP_NFIELDS * nmax, in->knots + (size_t)lo * PQP_NFIELDS * nmax,
+            PQP_CUDA(h->err, cudaMemcpyAsync(h->d_knots + (size_t)lo * PQP_NFIELDS * nmax, in->knots + (size_t)lo * PQP_NFIELDS * nmax,
                                         nb * PQP_NFIELDS * nmax * sizeof(double), cudaMemcpyHostToDevice, s));
-            PQP_CUDA(h, cudaMemcpyAsync(h->d_inst + (size_t)lo * PQP_NINST, in->inst + (size_t)lo * PQP_NINST,
+            PQP_CUDA(h->err, cudaMemcpyAsync(h->d_inst + (size_t)lo * PQP_NINST, in->inst + (size_t)lo * PQP_NINST,
                                         nb * PQP_NINST * sizeof(double), cudaMemcpyHostToDevice, s));
-            PQP_CUDA(h, cudaMemcpyAsync(h->d_n + lo, in->n + lo, nb * sizeof(int), cudaMemcpyHostToDevice, s));
-            if (in->p) PQP_CUDA(h, cudaMemcpyAsync(h->d_p + lo, in->p + lo, nb * sizeof(int), cudaMemcpyHostToDevice, s));
+            PQP_CUDA(h->err, cudaMemcpyAsync(h->d_n + lo, in->n + lo, nb * sizeof(int), cudaMemcpyHostToDevice, s));
+            if (in->p) PQP_CUDA(h->err, cudaMemcpyAsync(h->d_p + lo, in->p + lo, nb * sizeof(int), cudaMemcpyHostToDevice, s));
         }
-        if (out->x_full) PQP_CUDA(h, cudaMemsetAsync(h->d_xf + lo * nvm, 0, nb * nvm * sizeof(double), s));
-        if (out->y_full) PQP_CUDA(h, cudaMemsetAsync(h->d_yf + lo * mm, 0, nb * mm * sizeof(double), s));
-        if (out->z_full) PQP_CUDA(h, cudaMemsetAsync(h->d_zf + lo * mm, 0, nb * mm * sizeof(double), s));
-        if (nchunks == 1) PQP_CUDA(h, cudaEventRecord(h->ev_st[0], s));
+        if (out->x_full) PQP_CUDA(h->err, cudaMemsetAsync(h->d_xf + lo * nvm, 0, nb * nvm * sizeof(double), s));
+        if (out->y_full) PQP_CUDA(h->err, cudaMemsetAsync(h->d_yf + lo * mm, 0, nb * mm * sizeof(double), s));
+        if (out->z_full) PQP_CUDA(h->err, cudaMemsetAsync(h->d_zf + lo * mm, 0, nb * mm * sizeof(double), s));
+        if (nchunks == 1) PQP_CUDA(h->err, cudaEventRecord(h->ev_st[0], s));
         pqp_batch_in din;
         din.batch = (int32_t)nb;
         din.n_max = nmax;
@@ -807,46 +813,46 @@ int run_host(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *out, in
         dout.info = h->d_info + (size_t)lo * PQP_NINFO;
         rc = run_device(h, &din, &dout, mode, s, false, lo, false, h->d_flags + lo);
         if (rc) return rc;
-        if (nchunks == 1) PQP_CUDA(h, cudaEventRecord(h->ev_st[1], s));
-        PQP_CUDA(h, cudaMemcpyAsync(h->h_status + lo, dout.status, nb * sizeof(int), cudaMemcpyDeviceToHost, s));
-        PQP_CUDA(h, cudaMemcpyAsync(h->h_flags + lo, h->d_flags + lo, nb * sizeof(int), cudaMemcpyDeviceToHost, s));
-        PQP_CUDA(h, cudaMemcpyAsync(out->sol + (size_t)lo * 4 * nmax, dout.sol, nb * 4 * nmax * sizeof(double), cudaMemcpyDeviceToHost, s));
-        if (out->cost) PQP_CUDA(h, cudaMemcpyAsync(out->cost + lo, dout.cost, nb * sizeof(double), cudaMemcpyDeviceToHost, s));
-        if (out->status) PQP_CUDA(h, cudaMemcpyAsync(out->status + lo, dout.status, nb * sizeof(int), cudaMemcpyDeviceToHost, s));
-        if (out->iters) PQP_CUDA(h, cudaMemcpyAsync(out->iters + lo, dout.iters, nb * sizeof(int), cudaMemcpyDeviceToHost, s));
-        if (out->info) PQP_CUDA(h, cudaMemcpyAsync(out->info + (size_t)lo * PQP_NINFO, dout.info, nb * PQP_NINFO * sizeof(double), cudaMemcpyDeviceToHost, s));
-        if (out->x_full) PQP_CUDA(h, cudaMemcpyAsync(out->x_full + lo * nvm, dout.x_full, nb * nvm * sizeof(double), cudaMemcpyDeviceToHost, s));
-        if (out->y_full) PQP_CUDA(h, cudaMemcpyAsync(out->y_full + lo * mm, dout.y_full, nb * mm * sizeof(double), cudaMemcpyDeviceToHost, s));
-        if (out->z_full) PQP_CUDA(h, cudaMemcpyAsync(out->z_full + lo * mm, dout.z_full, nb * mm * sizeof(double), cudaMemcpyDeviceToHost, s));
+        if (nchunks == 1) PQP_CUDA(h->err, cudaEventRecord(h->ev_st[1], s));
+        PQP_CUDA(h->err, cudaMemcpyAsync(h->h_status + lo, dout.status, nb * sizeof(int), cudaMemcpyDeviceToHost, s));
+        PQP_CUDA(h->err, cudaMemcpyAsync(h->h_flags + lo, h->d_flags + lo, nb * sizeof(int), cudaMemcpyDeviceToHost, s));
+        PQP_CUDA(h->err, cudaMemcpyAsync(out->sol + (size_t)lo * 4 * nmax, dout.sol, nb * 4 * nmax * sizeof(double), cudaMemcpyDeviceToHost, s));
+        if (out->cost) PQP_CUDA(h->err, cudaMemcpyAsync(out->cost + lo, dout.cost, nb * sizeof(double), cudaMemcpyDeviceToHost, s));
+        if (out->status) PQP_CUDA(h->err, cudaMemcpyAsync(out->status + lo, dout.status, nb * sizeof(int), cudaMemcpyDeviceToHost, s));
+        if (out->iters) PQP_CUDA(h->err, cudaMemcpyAsync(out->iters + lo, dout.iters, nb * sizeof(int), cudaMemcpyDeviceToHost, s));
+        if (out->info) PQP_CUDA(h->err, cudaMemcpyAsync(out->info + (size_t)lo * PQP_NINFO, dout.info, nb * PQP_NINFO * sizeof(double), cudaMemcpyDeviceToHost, s));
+        if (out->x_full) PQP_CUDA(h->err, cudaMemcpyAsync(out->x_full + lo * nvm, dout.x_full, nb * nvm * sizeof(double), cudaMemcpyDeviceToHost, s));
+        if (out->y_full) PQP_CUDA(h->err, cudaMemcpyAsync(out->y_full + lo * mm, dout.y_full, nb * mm * sizeof(double), cudaMemcpyDeviceToHost, s));
+        if (out->z_full) PQP_CUDA(h->err, cudaMemcpyAsync(out->z_full + lo * mm, dout.z_full, nb * mm * sizeof(double), cudaMemcpyDeviceToHost, s));
     }
     h->last_batch = B;
     // join: stream[0] waits for every chunk stream; ev1 marks the end of the whole pipeline
     for (int c = 1; c < nchunks; ++c) {
-        PQP_CUDA(h, cudaEventRecord(h->evs[c], streams[c]));
-        PQP_CUDA(h, cudaStreamWaitEvent(streams[0], h->evs[c], 0));
+        PQP_CUDA(h->err, cudaEventRecord(h->evs[c], streams[c]));
+        PQP_CUDA(h->err, cudaStreamWaitEvent(streams[0], h->evs[c], 0));
     }
-    PQP_CUDA(h, cudaEventRecord(h->ev1, streams[0]));
-    PQP_CUDA(h, cudaStreamSynchronize(streams[0]));
-    PQP_CUDA(h, cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1));
+    PQP_CUDA(h->err, cudaEventRecord(h->ev1, streams[0]));
+    PQP_CUDA(h->err, cudaStreamSynchronize(streams[0]));
+    PQP_CUDA(h->err, cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1));
     // per-stage device times of a single-stream call (the reference's TimeRecorder stages of
     // BaseSolver::solve, base_solver.cpp:57-93; here cost / constraints / solver set-up / ADMM are one kernel)
     for (int i = 0; i < PQP_NSTAGES; ++i) h->stage_ms[i] = -1.0f;
     if (nchunks == 1) {
-        PQP_CUDA(h, cudaEventElapsedTime(&h->stage_ms[PQP_STAGE_H2D], h->ev0, h->ev_st[0]));
-        PQP_CUDA(h, cudaEventElapsedTime(&h->stage_ms[PQP_STAGE_KERNEL], h->ev_st[0], h->ev_st[1]));
-        PQP_CUDA(h, cudaEventElapsedTime(&h->stage_ms[PQP_STAGE_D2H], h->ev_st[1], h->ev1));
+        PQP_CUDA(h->err, cudaEventElapsedTime(&h->stage_ms[PQP_STAGE_H2D], h->ev0, h->ev_st[0]));
+        PQP_CUDA(h->err, cudaEventElapsedTime(&h->stage_ms[PQP_STAGE_KERNEL], h->ev_st[0], h->ev_st[1]));
+        PQP_CUDA(h->err, cudaEventElapsedTime(&h->stage_ms[PQP_STAGE_D2H], h->ev_st[1], h->ev1));
     }
     h->stage_ms[PQP_STAGE_TOTAL] = h->last_ms;
     h->stage_ms[PQP_STAGE_ESCALATION] = 0.0f;
     // cold solves only: the FP64 re-solve starts cold, which is not what a warm re-solve under an iteration
     // cap (receding horizon) is; the increment-form kernel certifies infeasibility by itself there
     if (!h->fp64 && h->escalate && mode == 0) {
-        PQP_CUDA(h, cudaEventRecord(h->ev_st[2], streams[0]));
+        PQP_CUDA(h->err, cudaEventRecord(h->ev_st[2], streams[0]));
         rc = escalate_fp64(h, in, out, B);
         if (rc) return rc;
-        PQP_CUDA(h, cudaEventRecord(h->ev_st[3], streams[0]));
-        PQP_CUDA(h, cudaEventSynchronize(h->ev_st[3]));
-        PQP_CUDA(h, cudaEventElapsedTime(&h->stage_ms[PQP_STAGE_ESCALATION], h->ev_st[2], h->ev_st[3]));
+        PQP_CUDA(h->err, cudaEventRecord(h->ev_st[3], streams[0]));
+        PQP_CUDA(h->err, cudaEventSynchronize(h->ev_st[3]));
+        PQP_CUDA(h->err, cudaEventElapsedTime(&h->stage_ms[PQP_STAGE_ESCALATION], h->ev_st[2], h->ev_st[3]));
     }
     return PQP_OK;
 }
@@ -868,112 +874,106 @@ const char *pqp_last_error(const pqp_handle *h) { return h ? h->err.c_str() : g_
 
 int pqp_create(const pqp_params *params, int32_t n_max, int32_t batch_max, int32_t device,
                pqp_handle **out) {
-    if (!out) return fail(nullptr, PQP_E_INVALID, "out is null");
+    if (!out) return fail(g_create_error, PQP_E_INVALID, "out is null");
     *out = nullptr;
-    if (!params || !pqp::params_valid(*params)) return fail(nullptr, PQP_E_INVALID, "invalid params");
-    if (n_max < 2 || n_max > 32 * pqp::kMaxChunk - 1) return fail(nullptr, PQP_E_INVALID, "n_max must be in [2, 511]");
-    if (batch_max < 1) return fail(nullptr, PQP_E_INVALID, "batch_max must be >= 1");
+    if (!params || !pqp::params_valid(*params)) return fail(g_create_error, PQP_E_INVALID, "invalid params");
+    if (n_max < 2 || n_max > 32 * pqp::kMaxChunk - 1) return fail(g_create_error, PQP_E_INVALID, "n_max must be in [2, 511]");
+    if (batch_max < 1) return fail(g_create_error, PQP_E_INVALID, "batch_max must be >= 1");
     int ndev = 0;
     cudaError_t e = cudaGetDeviceCount(&ndev);
     if (e != cudaSuccess || ndev == 0)
-        return fail(nullptr, PQP_E_NO_DEVICE, std::string("no CUDA device: ") + cudaGetErrorString(e));
-    if (device < 0 || device >= ndev) return fail(nullptr, PQP_E_NO_DEVICE, "device index out of range");
+        return fail(g_create_error, PQP_E_NO_DEVICE, std::string("no CUDA device: ") + cudaGetErrorString(e));
+    if (device < 0 || device >= ndev) return fail(g_create_error, PQP_E_NO_DEVICE, "device index out of range");
     cudaDeviceProp prop;
-    if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) return cuda_fail(nullptr, e, "cudaGetDeviceProperties");
+    PQP_CUDA(g_create_error, cudaGetDeviceProperties(&prop, device));
     if (prop.major != 9 || prop.minor != 0)
-        return fail(nullptr, PQP_E_NO_DEVICE, "this library is built for sm_90a (H100) only; found sm_" +
+        return fail(g_create_error, PQP_E_NO_DEVICE, "this library is built for sm_90a (H100) only; found sm_" +
                                                   std::to_string(prop.major) + std::to_string(prop.minor));
     pqp_handle *h = new (std::nothrow) pqp_handle;
-    if (!h) return fail(nullptr, PQP_E_INVALID, "out of host memory");
+    if (!h) return fail(g_create_error, PQP_E_INVALID, "out of host memory");
     h->prm = *params;
     h->n_max = n_max;
     h->batch_max = batch_max;
-    h->device = device;
+    h->device = h->res.device = device;
     h->chunk = pqp::chunk_for(n_max);
     h->sm_count = prop.multiProcessorCount;
     h->smem_bytes = pqp::smem_floats(h->chunk) * sizeof(float) + 16;
-#define PQP_CREATE_CUDA(call)                                                     \
-    do {                                                                          \
-        cudaError_t e_ = (call);                                                  \
-        if (e_ != cudaSuccess) {                                                  \
-            g_create_error = std::string(#call) + ": " + cudaGetErrorString(e_);  \
-            pqp_destroy(h);                                                       \
-            return PQP_E_CUDA;                                                    \
-        }                                                                         \
-    } while (0)
     DeviceGuard guard_(device);
-    h->fp64 = (params->reserved & 2) != 0;
-    h->escalate = (params->reserved & 4) == 0;
-    h->cold_only = (params->reserved & 128) != 0;
-    // launch of the FP32 kernel (measured on H100, 8192 instances, DESIGN.md §5): persistent (work counter, one
-    // streamed launch per host call) for n_max >= 128, where three QPs fill an SM's shared memory (n = 240: 0.5-1 %
-    // ahead); one CTA per instance below (n = 120: 2.7 % ahead, n = 60: equal). Both keep the state in shared
-    // memory. Bits 8 / 16 force one or the other.
-    const bool auto_persistent = h->chunk >= 8;
-    h->persistent = !h->fp64 && ((params->reserved & 8) != 0 || (auto_persistent && (params->reserved & 16) == 0));
-    // form of the ADMM step (FP32 kernels): the increment form (dx solve, row values A x carried and
-    // advanced by alpha A dx) follows the FP64 oracle's rho schedule - the same iteration count in almost
-    // every instance, fewer iterations on average - for a few per cent more work per iteration. Default:
-    // increment form for n_max >= 64, textbook form below; bits 32 / 64 force one or the other.
-    h->incr = !h->fp64 && ((params->reserved & 32) != 0 || ((params->reserved & 64) == 0 && h->chunk >= 4));
-    h->smem_bytes64 = pqp::smem_floats(h->chunk) * sizeof(double) + 16;
-    int bps = 0;
-    if (h->fp64) {
-        PQP_CREATE_CUDA(prepare_chunk<double>(h->chunk, h->smem_bytes64, &bps));
-        h->prepared64 = true;
-    } else if (h->persistent) {
-        PQP_CREATE_CUDA(prepare_persistent_chunk(h->chunk, h->smem_bytes, &bps, h->incr));
-    } else {
-        PQP_CREATE_CUDA(prepare_chunk<float>(h->chunk, h->smem_bytes, &bps, h->incr));
-    }
-    if (bps < 1) {
-        g_create_error = "the solve kernel does not fit on an SM";
+    const int rc = [&]() -> int {
+        h->fp64 = (params->reserved & 2) != 0;
+        h->escalate = (params->reserved & 4) == 0;
+        h->cold_only = (params->reserved & 128) != 0;
+        // launch of the FP32 kernel (measured on H100, 8192 instances, DESIGN.md §5): persistent (work counter, one
+        // streamed launch per host call) for n_max >= 128, where three QPs fill an SM's shared memory (n = 240: 0.5-1 %
+        // ahead); one CTA per instance below (n = 120: 2.7 % ahead, n = 60: equal). Both keep the state in shared
+        // memory. Bits 8 / 16 force one or the other.
+        const bool auto_persistent = h->chunk >= 8;
+        h->persistent = !h->fp64 && ((params->reserved & 8) != 0 || (auto_persistent && (params->reserved & 16) == 0));
+        // form of the ADMM step (FP32 kernels): the increment form (dx solve, row values A x carried and
+        // advanced by alpha A dx) follows the FP64 oracle's rho schedule - the same iteration count in almost
+        // every instance, fewer iterations on average - for a few per cent more work per iteration. Default:
+        // increment form for n_max >= 64, textbook form below; bits 32 / 64 force one or the other.
+        h->incr = !h->fp64 && ((params->reserved & 32) != 0 || ((params->reserved & 64) == 0 && h->chunk >= 4));
+        h->smem_bytes64 = pqp::smem_floats(h->chunk) * sizeof(double) + 16;
+        int bps = 0;
+        if (h->fp64) {
+            PQP_CUDA(g_create_error, prepare_chunk<double>(h->chunk, h->smem_bytes64, &bps));
+            h->prepared64 = true;
+        } else if (h->persistent) {
+            PQP_CUDA(g_create_error, prepare_persistent_chunk(h->chunk, h->smem_bytes, &bps, h->incr));
+        } else {
+            PQP_CUDA(g_create_error, prepare_chunk<float>(h->chunk, h->smem_bytes, &bps, h->incr));
+        }
+        if (bps < 1) return fail(g_create_error, PQP_E_CUDA, "the solve kernel does not fit on an SM");
+        h->warps_per_sm = bps;
+        pqp::Resources &r = h->res;
+        for (int i = 0; i < pqp_handle::kStreams; ++i) {
+            PQP_CUDA(g_create_error, r.stream(h->streams[i]));
+            PQP_CUDA(g_create_error, r.event(h->evs[i], cudaEventDisableTiming));
+        }
+        h->stream = h->streams[0];
+        PQP_CUDA(g_create_error, r.event(h->ev0));
+        PQP_CUDA(g_create_error, r.event(h->ev1));
+        const size_t B = batch_max, c = h->chunk;
+        PQP_CUDA(g_create_error, r.alloc(h->d_knots, B * PQP_NFIELDS * n_max));
+        PQP_CUDA(g_create_error, r.alloc(h->d_inst, B * PQP_NINST));
+        PQP_CUDA(g_create_error, r.alloc(h->d_n, B));
+        PQP_CUDA(g_create_error, r.alloc(h->d_p, B));
+        PQP_CUDA(g_create_error, r.alloc(h->d_sol, B * 4 * n_max));
+        PQP_CUDA(g_create_error, r.alloc(h->d_cost, B));
+        PQP_CUDA(g_create_error, r.alloc(h->d_status, B));
+        PQP_CUDA(g_create_error, r.alloc(h->d_iters, B));
+        PQP_CUDA(g_create_error, r.alloc(h->d_info, B * PQP_NINFO));
+        const size_t esz = h->fp64 ? sizeof(double) : sizeof(float);
+        // Warm state (scaled x, z, y and rho: the OSQP workspace that persists between solve and
+        // updateProblemFormulationAndSolve) is per instance; a cold-only handle keeps none. The Ruiz
+        // factors and delta_y are scratch of one solve: per instance under the one-CTA-per-instance
+        // launch, per resident warp under the persistent launch.
+        if (!h->cold_only) {
+            PQP_CUDA(g_create_error, r.alloc(h->d_warm, B * pqp::warm_floats(c) * esz));
+            PQP_CUDA(g_create_error, cudaMemset(h->d_warm, 0, B * pqp::warm_floats(c) * esz));
+            PQP_CUDA(g_create_error, r.alloc(h->d_rho, B * esz));
+        }
+        const size_t slots = h->persistent ? (size_t)h->sm_count * h->warps_per_sm : B;
+        PQP_CUDA(g_create_error, r.alloc(h->d_scal, slots * pqp::scal_floats(c) * esz));
+        PQP_CUDA(g_create_error, r.alloc(h->d_dy, slots * pqp::dy_floats(c) * esz));
+        for (int i = 0; i < 4; ++i) PQP_CUDA(g_create_error, r.event(h->ev_st[i]));
+        PQP_CUDA(g_create_error, r.alloc(h->d_counters, (size_t)pqp_handle::kCounters));
+        PQP_CUDA(g_create_error, r.alloc(h->d_ready, (size_t)pqp_handle::kStreams));
+        PQP_CUDA(g_create_error, r.alloc(h->d_done, (size_t)pqp_handle::kStreams));
+        PQP_CUDA(g_create_error, r.alloc_host(h->h_done, (size_t)pqp_handle::kStreams, cudaHostAllocMapped));
+        PQP_CUDA(g_create_error, cudaHostGetDevicePointer(reinterpret_cast<void **>(&h->d_hdone), h->h_done, 0));
+        PQP_CUDA(g_create_error, r.alloc(h->d_flags, B));
+        PQP_CUDA(g_create_error, cudaMemset(h->d_flags, 0, B * sizeof(int)));
+        PQP_CUDA(g_create_error, r.alloc_host(h->h_status, B));
+        PQP_CUDA(g_create_error, r.alloc_host(h->h_flags, B));
+        PQP_CUDA(g_create_error, cudaMemset(h->d_sol, 0, B * 4 * n_max * sizeof(double)));
+        return PQP_OK;
+    }();
+    if (rc != PQP_OK) {
         pqp_destroy(h);
-        return PQP_E_CUDA;
+        return rc;
     }
-    h->warps_per_sm = bps;
-    for (int i = 0; i < pqp_handle::kStreams; ++i) {
-        PQP_CREATE_CUDA(cudaStreamCreateWithFlags(&h->streams[i], cudaStreamNonBlocking));
-        PQP_CREATE_CUDA(cudaEventCreateWithFlags(&h->evs[i], cudaEventDisableTiming));
-    }
-    h->stream = h->streams[0];
-    PQP_CREATE_CUDA(cudaEventCreate(&h->ev0));
-    PQP_CREATE_CUDA(cudaEventCreate(&h->ev1));
-    const size_t B = batch_max, c = h->chunk;
-    PQP_CREATE_CUDA(dmalloc(&h->d_knots, B * PQP_NFIELDS * n_max));
-    PQP_CREATE_CUDA(dmalloc(&h->d_inst, B * PQP_NINST));
-    PQP_CREATE_CUDA(dmalloc(&h->d_n, B));
-    PQP_CREATE_CUDA(dmalloc(&h->d_p, B));
-    PQP_CREATE_CUDA(dmalloc(&h->d_sol, B * 4 * n_max));
-    PQP_CREATE_CUDA(dmalloc(&h->d_cost, B));
-    PQP_CREATE_CUDA(dmalloc(&h->d_status, B));
-    PQP_CREATE_CUDA(dmalloc(&h->d_iters, B));
-    PQP_CREATE_CUDA(dmalloc(&h->d_info, B * PQP_NINFO));
-    const size_t esz = h->fp64 ? sizeof(double) : sizeof(float);
-    // Warm state (scaled x, z, y and rho: the OSQP workspace that persists between solve and
-    // updateProblemFormulationAndSolve) is per instance; a cold-only handle keeps none. The Ruiz
-    // factors and delta_y are scratch of one solve: per instance under the one-CTA-per-instance
-    // launch, per resident warp under the persistent launch.
-    if (!h->cold_only) {
-        PQP_CREATE_CUDA(cudaMalloc(&h->d_warm, B * pqp::warm_floats(c) * esz));
-        PQP_CREATE_CUDA(cudaMemset(h->d_warm, 0, B * pqp::warm_floats(c) * esz));
-        PQP_CREATE_CUDA(cudaMalloc(&h->d_rho, B * esz));
-    }
-    const size_t slots = h->persistent ? (size_t)h->sm_count * h->warps_per_sm : B;
-    PQP_CREATE_CUDA(cudaMalloc(&h->d_scal, slots * pqp::scal_floats(c) * esz));
-    PQP_CREATE_CUDA(cudaMalloc(&h->d_dy, slots * pqp::dy_floats(c) * esz));
-    for (int i = 0; i < 4; ++i) PQP_CREATE_CUDA(cudaEventCreate(&h->ev_st[i]));
-    PQP_CREATE_CUDA(dmalloc(&h->d_counters, (size_t)pqp_handle::kCounters));
-    PQP_CREATE_CUDA(dmalloc(&h->d_ready, (size_t)pqp_handle::kStreams));
-    PQP_CREATE_CUDA(dmalloc(&h->d_done, (size_t)pqp_handle::kStreams));
-    PQP_CREATE_CUDA(cudaHostAlloc(reinterpret_cast<void **>(&h->h_done), pqp_handle::kStreams * sizeof(int), cudaHostAllocMapped));
-    PQP_CREATE_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void **>(&h->d_hdone), h->h_done, 0));
-    PQP_CREATE_CUDA(dmalloc(&h->d_flags, B));
-    PQP_CREATE_CUDA(cudaMemset(h->d_flags, 0, B * sizeof(int)));
-    PQP_CREATE_CUDA(cudaMallocHost(reinterpret_cast<void **>(&h->h_status), B * sizeof(int)));
-    PQP_CREATE_CUDA(cudaMallocHost(reinterpret_cast<void **>(&h->h_flags), B * sizeof(int)));
-    PQP_CREATE_CUDA(cudaMemset(h->d_sol, 0, B * 4 * n_max * sizeof(double)));
-#undef PQP_CREATE_CUDA
     *out = h;
     return PQP_OK;
 }
@@ -982,36 +982,13 @@ int pqp_destroy(pqp_handle *h) {
     if (!h) return PQP_OK;
     DeviceGuard guard_(h->device);
     for (int i = 0; i < pqp_handle::kStreams; ++i) if (h->streams[i]) cudaStreamSynchronize(h->streams[i]);
-    cudaFree(h->d_knots); cudaFree(h->d_inst); cudaFree(h->d_n); cudaFree(h->d_p);
-    cudaFree(h->d_sol); cudaFree(h->d_cost); cudaFree(h->d_status); cudaFree(h->d_iters);
-    cudaFree(h->d_info); cudaFree(h->d_xf); cudaFree(h->d_yf); cudaFree(h->d_zf);
-    cudaFree(h->d_ref); cudaFree(h->d_xy); cudaFree(h->d_sol2); cudaFree(h->d_n2);
-    cudaFree(h->d_warm); cudaFree(h->d_scal); cudaFree(h->d_dy); cudaFree(h->d_rho);
-    cudaFree(h->d_flags);
-    cudaFree(h->d_state64);
-    cudaFree(h->d_counters);
-    cudaFree(h->d_ready);
-    cudaFree(h->d_done);
-    if (h->h_done) cudaFreeHost(h->h_done);
-    if (h->h_status) cudaFreeHost(h->h_status);
-    if (h->h_flags) cudaFreeHost(h->h_flags);
-    cudaFree(h->e_knots); cudaFree(h->e_inst); cudaFree(h->e_sol); cudaFree(h->e_cost); cudaFree(h->e_info);
-    cudaFree(h->e_xf); cudaFree(h->e_yf); cudaFree(h->e_zf); cudaFree(h->e_n); cudaFree(h->e_p);
-    cudaFree(h->e_slots); cudaFree(h->e_status); cudaFree(h->e_iters); cudaFree(h->e_warm); cudaFree(h->e_scal); cudaFree(h->e_dy); cudaFree(h->e_rho);
-    if (h->ev0) cudaEventDestroy(h->ev0);
-    if (h->ev1) cudaEventDestroy(h->ev1);
-    for (int i = 0; i < 4; ++i) if (h->ev_st[i]) cudaEventDestroy(h->ev_st[i]);
-    for (int i = 0; i < pqp_handle::kStreams; ++i) {
-        if (h->streams[i]) cudaStreamDestroy(h->streams[i]);
-        if (h->evs[i]) cudaEventDestroy(h->evs[i]);
-    }
     delete h;
     return PQP_OK;
 }
 
 int pqp_solve(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *out) {
     if (!h) return PQP_E_INVALID;
-    if (!in) return fail(h, PQP_E_INVALID, "null batch");
+    if (!in) return fail(h->err, PQP_E_INVALID, "null batch");
     return run_host(h, in, out, 0);
 }
 
@@ -1031,8 +1008,8 @@ int pqp_solve_device(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out 
 int pqp_resolve_device(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *out, void *stream) {
     int rc = validate_batch(h, in, out);
     if (rc) return rc;
-    if (h->cold_only) return fail(h, PQP_E_STATE, "cold-only handle (option bit 128) keeps no warm state");
-    if (!h->solved || in->batch != h->last_batch) return fail(h, PQP_E_STATE, "resolve needs a previous solve of the same batch");
+    if (h->cold_only) return fail(h->err, PQP_E_STATE, "cold-only handle (option bit 128) keeps no warm state");
+    if (!h->solved || in->batch != h->last_batch) return fail(h->err, PQP_E_STATE, "resolve needs a previous solve of the same batch");
     DeviceGuard guard_(h->device);
     return run_device(h, in, out, 1, static_cast<cudaStream_t>(stream), false);
 }
@@ -1040,22 +1017,22 @@ int pqp_resolve_device(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_ou
 int pqp_frenet_to_cartesian_device(pqp_handle *h, int32_t batch, const int32_t *n, const double *ref_xyh,
                                    const double *sol, double *out_xyh, void *stream) {
     if (!h) return PQP_E_INVALID;
-    if (!n || !ref_xyh || !sol || !out_xyh || batch < 1) return fail(h, PQP_E_INVALID, "null buffer");
+    if (!n || !ref_xyh || !sol || !out_xyh || batch < 1) return fail(h->err, PQP_E_INVALID, "null buffer");
     DeviceGuard guard_(h->device);
     const int threads = 256, blocks = (batch * h->n_max + threads - 1) / threads;
     frenet_to_cartesian_kernel<<<blocks, threads, 0, static_cast<cudaStream_t>(stream)>>>(batch, h->n_max, n, ref_xyh, sol, out_xyh);
-    PQP_CUDA(h, cudaGetLastError());
+    PQP_CUDA(h->err, cudaGetLastError());
     h->launches++;
     return PQP_OK;
 }
 
 int pqp_relinearise_device(pqp_handle *h, int32_t batch, const double *sol, double *knots, void *stream) {
     if (!h) return PQP_E_INVALID;
-    if (!sol || !knots || batch < 1) return fail(h, PQP_E_INVALID, "null buffer");
+    if (!sol || !knots || batch < 1) return fail(h->err, PQP_E_INVALID, "null buffer");
     DeviceGuard guard_(h->device);
     const int threads = 256, blocks = (batch * h->n_max + threads - 1) / threads;
     relinearise_kernel<<<blocks, threads, 0, static_cast<cudaStream_t>(stream)>>>(batch, h->n_max, sol, knots);
-    PQP_CUDA(h, cudaGetLastError());
+    PQP_CUDA(h->err, cudaGetLastError());
     h->launches++;
     return PQP_OK;
 }
@@ -1063,13 +1040,13 @@ int pqp_relinearise_device(pqp_handle *h, int32_t batch, const double *sol, doub
 int pqp_advance_window_device(pqp_handle *h, int32_t batch, int32_t ext_len, int32_t tick, const double *ext_knots,
                               const double *sol, double *knots, double *inst, void *stream) {
     if (!h) return PQP_E_INVALID;
-    if (!ext_knots || !sol || !knots || !inst || batch < 1) return fail(h, PQP_E_INVALID, "null buffer");
-    if (tick < 0 || tick + h->n_max > ext_len) return fail(h, PQP_E_INVALID, "window [tick, tick + n_max) leaves the extended reference");
+    if (!ext_knots || !sol || !knots || !inst || batch < 1) return fail(h->err, PQP_E_INVALID, "null buffer");
+    if (tick < 0 || tick + h->n_max > ext_len) return fail(h->err, PQP_E_INVALID, "window [tick, tick + n_max) leaves the extended reference");
     DeviceGuard guard_(h->device);
     const int threads = 256, blocks = (batch * h->n_max + threads - 1) / threads;
     advance_window_kernel<<<blocks, threads, 0, static_cast<cudaStream_t>(stream)>>>(batch, h->n_max, ext_len, tick, ext_knots, sol,
                                                                                    knots, inst);
-    PQP_CUDA(h, cudaGetLastError());
+    PQP_CUDA(h->err, cudaGetLastError());
     h->launches++;
     return PQP_OK;
 }
@@ -1077,22 +1054,19 @@ int pqp_advance_window_device(pqp_handle *h, int32_t batch, int32_t ext_len, int
 int pqp_frenet_to_cartesian(pqp_handle *h, int32_t batch, const int32_t *n, const double *ref_xyh,
                             const double *sol, double *out_xyh) {
     if (!h) return PQP_E_INVALID;
-    if (!n || !ref_xyh || !sol || !out_xyh || batch < 1 || batch > h->batch_max) return fail(h, PQP_E_INVALID, "bad arguments");
+    if (!n || !ref_xyh || !sol || !out_xyh || batch < 1 || batch > h->batch_max) return fail(h->err, PQP_E_INVALID, "bad arguments");
     DeviceGuard guard_(h->device);
     const size_t B = batch, nm = h->n_max;
-    if (!h->d_ref) PQP_CUDA(h, dmalloc(&h->d_ref, (size_t)h->batch_max * 3 * nm));
-    if (!h->d_xy) PQP_CUDA(h, dmalloc(&h->d_xy, (size_t)h->batch_max * 3 * nm));
-    if (!h->d_sol2) PQP_CUDA(h, dmalloc(&h->d_sol2, (size_t)h->batch_max * 4 * nm));
-    if (!h->d_n2) PQP_CUDA(h, dmalloc(&h->d_n2, (size_t)h->batch_max));
+    if (!h->d_ref) PQP_CUDA(h->err, alloc_frenet_staging(h));
     cudaStream_t s = h->stream;
-    PQP_CUDA(h, cudaMemcpyAsync(h->d_ref, ref_xyh, B * 3 * nm * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQP_CUDA(h, cudaMemcpyAsync(h->d_sol2, sol, B * 4 * nm * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQP_CUDA(h, cudaMemcpyAsync(h->d_n2, n, B * sizeof(int), cudaMemcpyHostToDevice, s));
-    PQP_CUDA(h, cudaMemsetAsync(h->d_xy, 0, B * 3 * nm * sizeof(double), s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_ref, ref_xyh, B * 3 * nm * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_sol2, sol, B * 4 * nm * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_n2, n, B * sizeof(int), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemsetAsync(h->d_xy, 0, B * 3 * nm * sizeof(double), s));
     int rc = pqp_frenet_to_cartesian_device(h, batch, h->d_n2, h->d_ref, h->d_sol2, h->d_xy, s);
     if (rc) return rc;
-    PQP_CUDA(h, cudaMemcpyAsync(out_xyh, h->d_xy, B * 3 * nm * sizeof(double), cudaMemcpyDeviceToHost, s));
-    PQP_CUDA(h, cudaStreamSynchronize(s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(out_xyh, h->d_xy, B * 3 * nm * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaStreamSynchronize(s));
     return PQP_OK;
 }
 
@@ -1105,10 +1079,10 @@ int pqp_last_kernel_ms(pqp_handle *h, float *ms) {
 int pqp_pack_results_device(pqp_handle *h, int32_t batch, const double *cost, const int32_t *status,
                             const int32_t *iters, pqp_result_rec *packed, void *stream) {
     if (!h) return PQP_E_INVALID;
-    if (!cost || !status || !iters || !packed || batch < 1) return fail(h, PQP_E_INVALID, "null buffer");
+    if (!cost || !status || !iters || !packed || batch < 1) return fail(h->err, PQP_E_INVALID, "null buffer");
     DeviceGuard guard_(h->device);
     pack_results_kernel<<<(batch + 255) / 256, 256, 0, static_cast<cudaStream_t>(stream)>>>(batch, cost, status, iters, packed);
-    PQP_CUDA(h, cudaGetLastError());
+    PQP_CUDA(h->err, cudaGetLastError());
     h->launches++;
     return PQP_OK;
 }
@@ -1116,7 +1090,7 @@ int pqp_pack_results_device(pqp_handle *h, int32_t batch, const double *cost, co
 int pqp_resident_results(pqp_handle *h, const double **sol, const double **cost, const int32_t **status,
                          const int32_t **iters) {
     if (!h) return PQP_E_INVALID;
-    if (!h->solved || !h->host_inputs_resident) return fail(h, PQP_E_STATE, "no host-pointer solve has run on this handle");
+    if (!h->solved || !h->host_inputs_resident) return fail(h->err, PQP_E_STATE, "no host-pointer solve has run on this handle");
     if (sol) *sol = h->d_sol;
     if (cost) *cost = h->d_cost;
     if (status) *status = h->d_status;

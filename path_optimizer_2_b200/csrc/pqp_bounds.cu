@@ -16,7 +16,7 @@
 #include "../../include/pqp_bounds.h"
 #include "pqp_bounds_core.cuh"
 #include "pqp_bounds_internal.h"
-#include "pqp_device_guard.h"
+#include "pqp_host_handle.h"
 #include "pqp_map_core.cuh"
 
 namespace {
@@ -175,10 +175,9 @@ struct pqp_bounds_handle {
     int32_t *d_n = nullptr, *d_k = nullptr, *d_nvalid = nullptr;
     double *d_maxs = nullptr, *d_curv = nullptr;
     int32_t *d_total = nullptr;
-    size_t cap_maxs = 0, cap_curv = 0, cap_total = 0;
-    size_t cap_states = 0, cap_bounds = 0, cap_spline = 0, cap_knots = 0, cap_n = 0, cap_k = 0, cap_nvalid = 0;
     bool timed = false;
     std::string err;
+    pqp::Resources res;  // last member: releasing clears the members above
 };
 
 namespace pqb {
@@ -190,22 +189,13 @@ namespace {
 
 thread_local std::string g_bounds_create_error;
 
-#define PQB_CUDA(h, call)                                                          \
-    do {                                                                           \
-        cudaError_t e_ = (call);                                                   \
-        if (e_ != cudaSuccess) {                                                   \
-            (h)->err = std::string(#call) + ": " + cudaGetErrorString(e_);         \
-            return PQP_E_CUDA;                                                     \
-        }                                                                          \
-    } while (0)
+using pqp::fail;
 
 int validate(pqp_bounds_handle *h, const pqp_bounds_in *in, const pqp_bounds_out *out) {
     if (!h) return PQP_E_INVALID;
     if (!in || !out || in->batch <= 0 || in->n_max <= 0 || in->k_max < 3 || !in->states || !in->n || !in->spline ||
-        !in->k || !out->bounds || !out->n_valid) {
-        h->err = "pqp_bounds: null pointer or non-positive size (batch, n_max > 0, k_max >= 3)";
-        return PQP_E_INVALID;
-    }
+        !in->k || !out->bounds || !out->n_valid)
+        return fail(h->err, PQP_E_INVALID, "pqp_bounds: null pointer or non-positive size (batch, n_max > 0, k_max >= 3)");
     return PQP_OK;
 }
 
@@ -223,30 +213,16 @@ int launch(pqp_bounds_handle *h, const pqp_bounds_in *in, const pqp_bounds_out *
     a.bounds = out->bounds;
     a.n_valid = out->n_valid;
     a.knots = out->knots;
-    PQB_CUDA(h, cudaEventRecord(h->ev0, s));
+    PQP_CUDA(h->err, cudaEventRecord(h->ev0, s));
     init_n_valid_kernel<<<(in->batch + 255) / 256, 256, 0, s>>>(in->n, out->n_valid, in->batch, in->n_max);
     const long long total = (long long)in->batch * in->n_max;
     const long long blocks = (total + 127) / 128;
-    if (blocks > 0x7fffffffLL) {
-        h->err = "pqp_bounds: batch * n_max too large for one launch";
-        return PQP_E_INVALID;
-    }
+    if (blocks > 0x7fffffffLL) return fail(h->err, PQP_E_INVALID, "pqp_bounds: batch * n_max too large for one launch");
     clearance_bounds_kernel<<<dim3((unsigned)blocks, 3), 128, 0, s>>>(a);
-    PQB_CUDA(h, cudaGetLastError());
-    PQB_CUDA(h, cudaEventRecord(h->ev1, s));
+    PQP_CUDA(h->err, cudaGetLastError());
+    PQP_CUDA(h->err, cudaEventRecord(h->ev1, s));
     h->timed = true;
     return PQP_OK;
-}
-
-template <typename T>
-cudaError_t grow(T **p, size_t *cap, size_t need) {
-    if (need <= *cap) return cudaSuccess;
-    if (*p) cudaFree(*p);
-    *p = nullptr;
-    *cap = 0;
-    cudaError_t e = cudaMalloc(reinterpret_cast<void **>(p), need * sizeof(T));
-    if (e == cudaSuccess) *cap = need;
-    return e;
 }
 
 void set_meta(pqp_bounds_handle *h, int rows, int cols, double res, double cx, double cy) {
@@ -271,30 +247,19 @@ int validate_map(pqp_bounds_handle *h, const void *m, int rows, int cols, double
     else if ((size_t)rows * (size_t)cols > h->cap_cells) why = "rows * cols exceeds the cells the handle was created with";
     else if (!(res > 0.0) || !std::isfinite(res)) why = "resolution must be finite and > 0";
     else if (!std::isfinite(cx) || !std::isfinite(cy)) why = "centre must be finite";
-    if (why.empty()) return PQP_OK;
-    h->err = std::string(what) + ": " + why;
-    return PQP_E_INVALID;
+    return why.empty() ? PQP_OK : fail(h->err, PQP_E_INVALID, std::string(what) + ": " + why);
 }
 
 int launch_edt(pqp_bounds_handle *h, const pqp_occupancy_map *occ, const uint8_t *cells, cudaStream_t s) {
     const int rows = occ->rows, cols = occ->cols;
     const size_t smem = (size_t)pqm::kRowSmemPerCol * cols;
     // the dynamic share plus the kernel's static n_env may pass the 48 KB default at any width: always opt in
-    PQB_CUDA(h, cudaFuncSetAttribute(pqm::edt_row_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    PQP_CUDA(h->err, cudaFuncSetAttribute(pqm::edt_row_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     pqm::edt_column_kernel<<<(cols + pqm::kEdtColumnThreads - 1) / pqm::kEdtColumnThreads, pqm::kEdtColumnThreads, 0,
                              s>>>(cells, rows, cols, occ->obstacle_max, reinterpret_cast<int32_t *>(h->d_dist));
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) {
-        h->err = std::string("edt_column_kernel launch: ") + cudaGetErrorString(e);
-        return PQP_E_CUDA;
-    }
+    PQP_CUDA(h->err, cudaGetLastError());
     pqm::edt_row_kernel<<<rows, pqm::kEdtRowThreads, smem, s>>>(h->d_dist, rows, cols, (float)occ->resolution);
-    e = cudaGetLastError();
-    if (e != cudaSuccess) {
-        h->err = std::string("edt_row_kernel launch: ") + cudaGetErrorString(e) + " (" + std::to_string(rows) + " x " +
-                 std::to_string(cols) + ", " + std::to_string(smem) + " B shared)";
-        return PQP_E_CUDA;
-    }
+    PQP_CUDA(h->err, cudaGetLastError());
     return PQP_OK;
 }
 
@@ -303,10 +268,8 @@ int validate_occupancy(pqp_bounds_handle *h, const pqp_occupancy_map *occ, const
                                       occ->cells, what)
                        : validate_map(h, nullptr, 0, 0, 0.0, 0.0, 0.0, nullptr, what);
     if (rc != PQP_OK) return rc;
-    if (occ->rows > pqm::kMaxSide || occ->cols > pqm::kMaxSide) {
-        h->err = std::string(what) + ": rows and cols must be <= 16384 for the distance transform";
-        return PQP_E_INVALID;
-    }
+    if (occ->rows > pqm::kMaxSide || occ->cols > pqm::kMaxSide)
+        return fail(h->err, PQP_E_INVALID, std::string(what) + ": rows and cols must be <= 16384 for the distance transform");
     return PQP_OK;
 }
 
@@ -327,18 +290,15 @@ int pqp_bounds_create(const pqp_bounds_map *map, const pqp_bounds_params *params
                       pqp_bounds_handle **out) {
     if (!out) return PQP_E_INVALID;
     *out = nullptr;
-    if (!map || !map->distance || map->rows < 2 || map->cols < 2 || !(map->resolution > 0.0)) {
-        g_bounds_create_error = "pqp_bounds_create: map needs rows, cols >= 2, resolution > 0 and a distance layer";
-        return PQP_E_INVALID;
-    }
+    if (!map || !map->distance || map->rows < 2 || map->cols < 2 || !(map->resolution > 0.0))
+        return fail(g_bounds_create_error, PQP_E_INVALID,
+                    "pqp_bounds_create: map needs rows, cols >= 2, resolution > 0 and a distance layer");
     int count = 0;
-    if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0 || device < 0 || device >= count) {
-        g_bounds_create_error = "pqp_bounds_create: no CUDA device (there is no CPU fallback)";
-        return PQP_E_NO_DEVICE;
-    }
+    if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0 || device < 0 || device >= count)
+        return fail(g_bounds_create_error, PQP_E_NO_DEVICE, "pqp_bounds_create: no CUDA device (there is no CPU fallback)");
     pqp_bounds_handle *h = new (std::nothrow) pqp_bounds_handle();
     if (!h) return PQP_E_CUDA;
-    h->device = device;
+    h->device = h->res.device = device;
     pqp_bounds_params dflt;
     pqp_bounds_default_params(&dflt);
     const pqp_bounds_params &p = params ? *params : dflt;
@@ -349,17 +309,18 @@ int pqp_bounds_create(const pqp_bounds_map *map, const pqp_bounds_params *params
     h->prm.epsilon = p.epsilon;
     const size_t cells = (size_t)map->rows * map->cols;
     pqp::DeviceGuard guard_(device);
-    cudaError_t e = cudaSuccess;
-    if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void **>(&h->d_dist), cells * sizeof(float));
-    if (e == cudaSuccess) e = cudaMemcpy(h->d_dist, map->distance, cells * sizeof(float), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void **>(&h->d_occ), cells);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaEventCreate(&h->ev0);
-    if (e == cudaSuccess) e = cudaEventCreate(&h->ev1);
-    if (e != cudaSuccess) {
-        g_bounds_create_error = std::string("pqp_bounds_create: ") + cudaGetErrorString(e);
+    const int rc = [&]() -> int {
+        PQP_CUDA(g_bounds_create_error, h->res.alloc(h->d_dist, cells));
+        PQP_CUDA(g_bounds_create_error, cudaMemcpy(h->d_dist, map->distance, cells * sizeof(float), cudaMemcpyHostToDevice));
+        PQP_CUDA(g_bounds_create_error, h->res.alloc(h->d_occ, cells));
+        PQP_CUDA(g_bounds_create_error, h->res.stream(h->stream));
+        PQP_CUDA(g_bounds_create_error, h->res.event(h->ev0));
+        PQP_CUDA(g_bounds_create_error, h->res.event(h->ev1));
+        return PQP_OK;
+    }();
+    if (rc != PQP_OK) {
         pqp_bounds_destroy(h);
-        return PQP_E_CUDA;
+        return rc;
     }
     h->cap_cells = cells;
     set_meta(h, map->rows, map->cols, map->resolution, map->center_x, map->center_y);
@@ -368,23 +329,6 @@ int pqp_bounds_create(const pqp_bounds_map *map, const pqp_bounds_params *params
 }
 
 void pqp_bounds_destroy(pqp_bounds_handle *h) {
-    if (!h) return;
-    pqp::DeviceGuard guard_(h->device);
-    cudaFree(h->d_dist);
-    cudaFree(h->d_occ);
-    cudaFree(h->d_states);
-    cudaFree(h->d_spline);
-    cudaFree(h->d_bounds);
-    cudaFree(h->d_knots);
-    cudaFree(h->d_n);
-    cudaFree(h->d_k);
-    cudaFree(h->d_nvalid);
-    cudaFree(h->d_maxs);
-    cudaFree(h->d_curv);
-    cudaFree(h->d_total);
-    if (h->ev0) cudaEventDestroy(h->ev0);
-    if (h->ev1) cudaEventDestroy(h->ev1);
-    if (h->stream) cudaStreamDestroy(h->stream);
     delete h;
 }
 
@@ -401,19 +345,19 @@ int pqp_bounds_compute(pqp_bounds_handle *h, const pqp_bounds_in *in, const pqp_
     pqp::DeviceGuard guard_(h->device);
     const size_t B = in->batch, ns = B * PQP_STATE_ROWS * in->n_max, nsp = B * PQP_SPLINE_ROWS * in->k_max;
     const size_t nb = B * PQP_BOUND_ROWS * in->n_max, nk = out->knots ? B * PQP_NFIELDS * in->n_max : 0;
-    PQB_CUDA(h, grow(&h->d_states, &h->cap_states, ns));
-    PQB_CUDA(h, grow(&h->d_bounds, &h->cap_bounds, nb));
-    PQB_CUDA(h, grow(&h->d_spline, &h->cap_spline, nsp));
-    if (nk) PQB_CUDA(h, grow(&h->d_knots, &h->cap_knots, nk));
-    PQB_CUDA(h, grow(&h->d_n, &h->cap_n, B));
-    PQB_CUDA(h, grow(&h->d_k, &h->cap_k, B));
-    PQB_CUDA(h, grow(&h->d_nvalid, &h->cap_nvalid, B));
+    PQP_CUDA(h->err, h->res.grow(h->d_states, ns));
+    PQP_CUDA(h->err, h->res.grow(h->d_bounds, nb));
+    PQP_CUDA(h->err, h->res.grow(h->d_spline, nsp));
+    if (nk) PQP_CUDA(h->err, h->res.grow(h->d_knots, nk));
+    PQP_CUDA(h->err, h->res.grow(h->d_n, B));
+    PQP_CUDA(h->err, h->res.grow(h->d_k, B));
+    PQP_CUDA(h->err, h->res.grow(h->d_nvalid, B));
     cudaStream_t s = h->stream;
-    PQB_CUDA(h, cudaMemcpyAsync(h->d_states, in->states, ns * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQB_CUDA(h, cudaMemcpyAsync(h->d_spline, in->spline, nsp * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQB_CUDA(h, cudaMemcpyAsync(h->d_n, in->n, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    PQB_CUDA(h, cudaMemcpyAsync(h->d_k, in->k, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    if (nk) PQB_CUDA(h, cudaMemcpyAsync(h->d_knots, out->knots, nk * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_states, in->states, ns * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_spline, in->spline, nsp * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_n, in->n, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_k, in->k, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    if (nk) PQP_CUDA(h->err, cudaMemcpyAsync(h->d_knots, out->knots, nk * sizeof(double), cudaMemcpyHostToDevice, s));
     pqp_bounds_in din = *in;
     din.states = h->d_states;
     din.spline = h->d_spline;
@@ -425,10 +369,10 @@ int pqp_bounds_compute(pqp_bounds_handle *h, const pqp_bounds_in *in, const pqp_
     dout.knots = nk ? h->d_knots : nullptr;
     rc = launch(h, &din, &dout, s);
     if (rc != PQP_OK) return rc;
-    PQB_CUDA(h, cudaMemcpyAsync(out->bounds, h->d_bounds, nb * sizeof(double), cudaMemcpyDeviceToHost, s));
-    PQB_CUDA(h, cudaMemcpyAsync(out->n_valid, h->d_nvalid, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    if (nk) PQB_CUDA(h, cudaMemcpyAsync(out->knots, h->d_knots, nk * sizeof(double), cudaMemcpyDeviceToHost, s));
-    PQB_CUDA(h, cudaStreamSynchronize(s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(out->bounds, h->d_bounds, nb * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(out->n_valid, h->d_nvalid, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    if (nk) PQP_CUDA(h->err, cudaMemcpyAsync(out->knots, h->d_knots, nk * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaStreamSynchronize(s));
     return PQP_OK;
 }
 
@@ -436,10 +380,9 @@ static int validate_states(pqp_bounds_handle *h, const pqp_states_in *in, const 
     if (!h) return PQP_E_INVALID;
     if (!in || !out || in->batch <= 0 || in->n_max <= 0 || in->k_max < 3 || !in->spline || !in->k || !in->max_s ||
         !out->states || !out->curvature || !out->n || !(in->delta_s_larger > 0.0) || !(in->delta_s_smaller > 0.0) ||
-        in->delta_s_smaller > in->delta_s_larger) {
-        h->err = "pqp_bounds_build_states: null pointer, non-positive size, or 0 < delta_s_smaller <= delta_s_larger violated";
-        return PQP_E_INVALID;
-    }
+        in->delta_s_smaller > in->delta_s_larger)
+        return fail(h->err, PQP_E_INVALID,
+                    "pqp_bounds_build_states: null pointer, non-positive size, or 0 < delta_s_smaller <= delta_s_larger violated");
     return PQP_OK;
 }
 
@@ -459,10 +402,10 @@ static int launch_states(pqp_bounds_handle *h, const pqp_states_in *in, const pq
     a.knots = out->knots;
     a.n = out->n;
     a.total = out->total;
-    PQB_CUDA(h, cudaEventRecord(h->ev0, s));
+    PQP_CUDA(h->err, cudaEventRecord(h->ev0, s));
     reference_states_kernel<<<(in->batch + 63) / 64, 64, 0, s>>>(a);
-    PQB_CUDA(h, cudaGetLastError());
-    PQB_CUDA(h, cudaEventRecord(h->ev1, s));
+    PQP_CUDA(h->err, cudaGetLastError());
+    PQP_CUDA(h->err, cudaEventRecord(h->ev1, s));
     h->timed = true;
     return PQP_OK;
 }
@@ -480,21 +423,21 @@ int pqp_bounds_build_states(pqp_bounds_handle *h, const pqp_states_in *in, const
     pqp::DeviceGuard guard_(h->device);
     const size_t B = in->batch, ns = B * PQP_STATE_ROWS * in->n_max, nsp = B * PQP_SPLINE_ROWS * in->k_max;
     const size_t nc = B * in->n_max, nk = out->knots ? B * PQP_NFIELDS * in->n_max : 0;
-    PQB_CUDA(h, grow(&h->d_states, &h->cap_states, ns));
-    PQB_CUDA(h, grow(&h->d_curv, &h->cap_curv, nc));
-    PQB_CUDA(h, grow(&h->d_spline, &h->cap_spline, nsp));
-    if (nk) PQB_CUDA(h, grow(&h->d_knots, &h->cap_knots, nk));
-    PQB_CUDA(h, grow(&h->d_n, &h->cap_n, B));
-    PQB_CUDA(h, grow(&h->d_k, &h->cap_k, B));
-    PQB_CUDA(h, grow(&h->d_total, &h->cap_total, B));
-    PQB_CUDA(h, grow(&h->d_maxs, &h->cap_maxs, B));
+    PQP_CUDA(h->err, h->res.grow(h->d_states, ns));
+    PQP_CUDA(h->err, h->res.grow(h->d_curv, nc));
+    PQP_CUDA(h->err, h->res.grow(h->d_spline, nsp));
+    if (nk) PQP_CUDA(h->err, h->res.grow(h->d_knots, nk));
+    PQP_CUDA(h->err, h->res.grow(h->d_n, B));
+    PQP_CUDA(h->err, h->res.grow(h->d_k, B));
+    PQP_CUDA(h->err, h->res.grow(h->d_total, B));
+    PQP_CUDA(h->err, h->res.grow(h->d_maxs, B));
     cudaStream_t s = h->stream;
-    PQB_CUDA(h, cudaMemcpyAsync(h->d_spline, in->spline, nsp * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQB_CUDA(h, cudaMemcpyAsync(h->d_k, in->k, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    PQB_CUDA(h, cudaMemcpyAsync(h->d_maxs, in->max_s, B * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQB_CUDA(h, cudaMemsetAsync(h->d_states, 0, ns * sizeof(double), s));
-    PQB_CUDA(h, cudaMemsetAsync(h->d_curv, 0, nc * sizeof(double), s));
-    if (nk) PQB_CUDA(h, cudaMemcpyAsync(h->d_knots, out->knots, nk * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_spline, in->spline, nsp * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_k, in->k, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_maxs, in->max_s, B * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemsetAsync(h->d_states, 0, ns * sizeof(double), s));
+    PQP_CUDA(h->err, cudaMemsetAsync(h->d_curv, 0, nc * sizeof(double), s));
+    if (nk) PQP_CUDA(h->err, cudaMemcpyAsync(h->d_knots, out->knots, nk * sizeof(double), cudaMemcpyHostToDevice, s));
     pqp_states_in din = *in;
     din.spline = h->d_spline;
     din.k = h->d_k;
@@ -507,12 +450,12 @@ int pqp_bounds_build_states(pqp_bounds_handle *h, const pqp_states_in *in, const
     dout.knots = nk ? h->d_knots : nullptr;
     rc = launch_states(h, &din, &dout, s);
     if (rc != PQP_OK) return rc;
-    PQB_CUDA(h, cudaMemcpyAsync(out->states, h->d_states, ns * sizeof(double), cudaMemcpyDeviceToHost, s));
-    PQB_CUDA(h, cudaMemcpyAsync(out->curvature, h->d_curv, nc * sizeof(double), cudaMemcpyDeviceToHost, s));
-    PQB_CUDA(h, cudaMemcpyAsync(out->n, h->d_n, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    if (out->total) PQB_CUDA(h, cudaMemcpyAsync(out->total, h->d_total, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    if (nk) PQB_CUDA(h, cudaMemcpyAsync(out->knots, h->d_knots, nk * sizeof(double), cudaMemcpyDeviceToHost, s));
-    PQB_CUDA(h, cudaStreamSynchronize(s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(out->states, h->d_states, ns * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(out->curvature, h->d_curv, nc * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(out->n, h->d_n, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    if (out->total) PQP_CUDA(h->err, cudaMemcpyAsync(out->total, h->d_total, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    if (nk) PQP_CUDA(h->err, cudaMemcpyAsync(out->knots, h->d_knots, nk * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaStreamSynchronize(s));
     return PQP_OK;
 }
 
@@ -522,8 +465,8 @@ int pqp_bounds_last_kernel_ms(pqp_bounds_handle *h, float *ms) {
         *ms = 0.0f;
         return PQP_OK;
     }
-    PQB_CUDA(h, cudaEventSynchronize(h->ev1));
-    PQB_CUDA(h, cudaEventElapsedTime(ms, h->ev0, h->ev1));
+    PQP_CUDA(h->err, cudaEventSynchronize(h->ev1));
+    PQP_CUDA(h->err, cudaEventElapsedTime(ms, h->ev0, h->ev1));
     return PQP_OK;
 }
 
@@ -536,7 +479,7 @@ int pqp_bounds_set_map_device(pqp_bounds_handle *h, const pqp_bounds_map *map, v
     if (rc != PQP_OK) return rc;
     pqp::DeviceGuard guard_(h->device);
     const size_t cells = (size_t)map->rows * map->cols;
-    PQB_CUDA(h, cudaMemcpyAsync(h->d_dist, map->distance, cells * sizeof(float), cudaMemcpyDefault,
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_dist, map->distance, cells * sizeof(float), cudaMemcpyDefault,
                                 static_cast<cudaStream_t>(stream)));
     set_meta(h, map->rows, map->cols, map->resolution, map->center_x, map->center_y);
     return PQP_OK;
@@ -546,7 +489,7 @@ int pqp_bounds_set_map(pqp_bounds_handle *h, const pqp_bounds_map *map) {
     const int rc = pqp_bounds_set_map_device(h, map, h ? h->stream : nullptr);
     if (rc != PQP_OK) return rc;
     pqp::DeviceGuard guard_(h->device);
-    PQB_CUDA(h, cudaStreamSynchronize(h->stream));
+    PQP_CUDA(h->err, cudaStreamSynchronize(h->stream));
     return PQP_OK;
 }
 
@@ -565,20 +508,17 @@ int pqp_bounds_set_occupancy(pqp_bounds_handle *h, const pqp_occupancy_map *occ)
     if (rc != PQP_OK) return rc;
     pqp::DeviceGuard guard_(h->device);
     const size_t cells = (size_t)occ->rows * occ->cols;
-    PQB_CUDA(h, cudaMemcpyAsync(h->d_occ, occ->cells, cells, cudaMemcpyHostToDevice, h->stream));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_occ, occ->cells, cells, cudaMemcpyHostToDevice, h->stream));
     const int lrc = launch_edt(h, occ, h->d_occ, h->stream);
     if (lrc != PQP_OK) return lrc;
     set_meta(h, occ->rows, occ->cols, occ->resolution, occ->center_x, occ->center_y);
-    PQB_CUDA(h, cudaStreamSynchronize(h->stream));
+    PQP_CUDA(h->err, cudaStreamSynchronize(h->stream));
     return PQP_OK;
 }
 
 int pqp_bounds_get_map(pqp_bounds_handle *h, pqp_bounds_map *meta, float *distance) {
     if (!h) return PQP_E_INVALID;
-    if (!meta) {
-        h->err = "pqp_bounds_get_map: null metadata";
-        return PQP_E_INVALID;
-    }
+    if (!meta) return fail(h->err, PQP_E_INVALID, "pqp_bounds_get_map: null metadata");
     pqp::DeviceGuard guard_(h->device);
     meta->rows = h->map.rows;
     meta->cols = h->map.cols;
@@ -587,8 +527,8 @@ int pqp_bounds_get_map(pqp_bounds_handle *h, pqp_bounds_map *meta, float *distan
     meta->center_y = h->map.cy;
     meta->distance = nullptr;
     if (distance) {
-        PQB_CUDA(h, cudaDeviceSynchronize());
-        PQB_CUDA(h, cudaMemcpy(distance, h->d_dist, (size_t)h->map.rows * h->map.cols * sizeof(float),
+        PQP_CUDA(h->err, cudaDeviceSynchronize());
+        PQP_CUDA(h->err, cudaMemcpy(distance, h->d_dist, (size_t)h->map.rows * h->map.cols * sizeof(float),
                                cudaMemcpyDeviceToHost));
     }
     return PQP_OK;

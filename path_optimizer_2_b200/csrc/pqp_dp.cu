@@ -10,8 +10,8 @@
 
 #include "../../include/pqp_dp.h"
 #include "pqp_bounds_internal.h"
-#include "pqp_device_guard.h"
 #include "pqp_dp_core.cuh"
+#include "pqp_host_handle.h"
 
 namespace {
 
@@ -110,37 +110,24 @@ struct pqp_dp_handle {
     double *d_spline = nullptr, *d_length = nullptr, *d_start = nullptr, *d_layer_s = nullptr, *d_lower = nullptr, *d_upper = nullptr;
     double *d_vehicle_l = nullptr, *d_target_s = nullptr;
     int32_t *d_k = nullptr, *d_status = nullptr, *d_n_layers = nullptr, *d_n_out = nullptr, *d_chosen = nullptr;
-    size_t cap_spline = 0;
     float last_ms = 0.0f;
     std::string err;
+    pqp::Resources res;  // last member: releasing clears the members above
 };
 
 namespace {
 
-#define PQD_CUDA(h, call)                                                      \
-    do {                                                                       \
-        cudaError_t e_ = (call);                                               \
-        if (e_ != cudaSuccess) {                                               \
-            (h)->err = std::string(#call) + ": " + cudaGetErrorString(e_);     \
-            return PQP_E_CUDA;                                                 \
-        }                                                                      \
-    } while (0)
-
-int dfail(pqp_dp_handle *h, int code, const char *msg) {
-    if (h) h->err = msg;
-    else g_dp_create_error = msg;
-    return code;
-}
+using pqp::fail;
 
 int validate(pqp_dp_handle *h, const pqp_dp_in *in, const pqp_dp_out *out) {
     if (!h) return PQP_E_INVALID;
-    if (!in || !out) return dfail(h, PQP_E_INVALID, "null batch");
-    if (!in->spline || !in->k || !in->length || !in->start) return dfail(h, PQP_E_INVALID, "null input buffer");
+    if (!in || !out) return fail(h->err, PQP_E_INVALID, "null batch");
+    if (!in->spline || !in->k || !in->length || !in->start) return fail(h->err, PQP_E_INVALID, "null input buffer");
     if (!out->status || !out->n_layers || !out->n_out || !out->layer_s || !out->lower || !out->upper || !out->chosen ||
         !out->vehicle_l || !out->target_s)
-        return dfail(h, PQP_E_INVALID, "null output buffer");
-    if (in->batch < 1 || in->batch > h->batch_max) return dfail(h, PQP_E_INVALID, "batch out of range");
-    if (in->k_max < 3) return dfail(h, PQP_E_INVALID, "k_max must be >= 3");
+        return fail(h->err, PQP_E_INVALID, "null output buffer");
+    if (in->batch < 1 || in->batch > h->batch_max) return fail(h->err, PQP_E_INVALID, "batch out of range");
+    if (in->k_max < 3) return fail(h->err, PQP_E_INVALID, "k_max must be >= 3");
     return PQP_OK;
 }
 
@@ -170,16 +157,11 @@ int launch(pqp_dp_handle *h, const pqp_dp_in *in, const pqp_dp_out *out, cudaStr
     a.ny = h->d_ny;
     a.dis = h->d_dis;
     a.ref = h->d_ref;
-    PQD_CUDA(h, cudaEventRecord(h->ev0, s));
+    PQP_CUDA(h->err, cudaEventRecord(h->ev0, s));
     dp_search_kernel<<<in->batch, kThreads, 0, s>>>(*pqb::handle_map(h->owner), h->prm, a);
-    PQD_CUDA(h, cudaGetLastError());
-    PQD_CUDA(h, cudaEventRecord(h->ev1, s));
+    PQP_CUDA(h->err, cudaGetLastError());
+    PQP_CUDA(h->err, cudaEventRecord(h->ev1, s));
     return PQP_OK;
-}
-
-template <typename T>
-cudaError_t dalloc(T **p, size_t n) {
-    return cudaMalloc(reinterpret_cast<void **>(p), (n ? n : 1) * sizeof(T));
 }
 
 }  // namespace
@@ -200,17 +182,23 @@ int pqp_dp_create(pqp_bounds_handle *owner, const pqp_dp_params *params, int32_t
                   pqp_dp_handle **out) {
     if (!out) return PQP_E_INVALID;
     *out = nullptr;
-    if (!owner) return dfail(nullptr, PQP_E_INVALID, "pqp_dp_create: a pqp_bounds_handle (the map) is required");
-    if (layers_max < 2 || batch_max < 1) return dfail(nullptr, PQP_E_INVALID, "pqp_dp_create: layers_max >= 2, batch_max >= 1");
+    if (!owner) return fail(g_dp_create_error, PQP_E_INVALID, "pqp_dp_create: a pqp_bounds_handle (the map) is required");
+    if (layers_max < 2 || batch_max < 1) return fail(g_dp_create_error, PQP_E_INVALID, "pqp_dp_create: layers_max >= 2, batch_max >= 1");
     pqp_dp_params dflt;
     pqp_dp_default_params(&dflt);
     const pqp_dp_params &p = params ? *params : dflt;
     if (!(p.lateral_spacing > 0) || !(p.lateral_range > 0) || !(p.longitudinal_spacing > 0))
-        return dfail(nullptr, PQP_E_INVALID, "pqp_dp_create: spacings and range must be positive");
+        return fail(g_dp_create_error, PQP_E_INVALID, "pqp_dp_create: spacings and range must be positive");
+    {
+        double cl = -p.lateral_range;
+        int n = 0;
+        while (cl <= p.lateral_range) { ++n; cl += p.lateral_spacing; }
+        if (n > pqdp::kJMax) return fail(g_dp_create_error, PQP_E_INVALID, "pqp_dp_create: more than 64 lateral samples per layer");
+    }
     pqp_dp_handle *h = new (std::nothrow) pqp_dp_handle;
-    if (!h) return dfail(nullptr, PQP_E_INVALID, "out of host memory");
+    if (!h) return fail(g_dp_create_error, PQP_E_INVALID, "out of host memory");
     h->owner = owner;
-    h->device = pqb::handle_device(owner);
+    h->device = h->res.device = pqb::handle_device(owner);
     h->layers_max = layers_max;
     h->batch_max = batch_max;
     h->prm.lateral_range = p.lateral_range;
@@ -218,43 +206,38 @@ int pqp_dp_create(pqp_bounds_handle *owner, const pqp_dp_params *params, int32_t
     h->prm.lon_spacing = p.longitudinal_spacing;
     h->prm.car_width = p.car_width;
     h->J = pqdp::lateral_count(h->prm);
-    {
-        double cl = -p.lateral_range;
-        int n = 0;
-        while (cl <= p.lateral_range) { ++n; cl += p.lateral_spacing; }
-        if (n > pqdp::kJMax) {
-            delete h;
-            return dfail(nullptr, PQP_E_INVALID, "pqp_dp_create: more than 64 lateral samples per layer");
-        }
-    }
     pqp::DeviceGuard guard_(h->device);
-    const size_t B = batch_max, T = B * layers_max * h->J, Ls = B * layers_max;
-    cudaError_t e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaEventCreate(&h->ev0);
-    if (e == cudaSuccess) e = cudaEventCreate(&h->ev1);
-    if (e == cudaSuccess) e = dalloc(&h->d_nx, T);
-    if (e == cudaSuccess) e = dalloc(&h->d_ny, T);
-    if (e == cudaSuccess) e = dalloc(&h->d_dis, T);
-    if (e == cudaSuccess) e = dalloc(&h->d_cost, T);
-    if (e == cudaSuccess) e = dalloc(&h->d_parent, T);
-    if (e == cudaSuccess) e = dalloc(&h->d_feasible, T);
-    if (e == cudaSuccess) e = dalloc(&h->d_ref, Ls * 4);
-    if (e == cudaSuccess) e = dalloc(&h->d_length, B);
-    if (e == cudaSuccess) e = dalloc(&h->d_start, B * 3);
-    if (e == cudaSuccess) e = dalloc(&h->d_k, B);
-    if (e == cudaSuccess) e = dalloc(&h->d_status, B);
-    if (e == cudaSuccess) e = dalloc(&h->d_n_layers, B);
-    if (e == cudaSuccess) e = dalloc(&h->d_n_out, B);
-    if (e == cudaSuccess) e = dalloc(&h->d_vehicle_l, B);
-    if (e == cudaSuccess) e = dalloc(&h->d_target_s, B);
-    if (e == cudaSuccess) e = dalloc(&h->d_layer_s, Ls);
-    if (e == cudaSuccess) e = dalloc(&h->d_lower, Ls);
-    if (e == cudaSuccess) e = dalloc(&h->d_upper, Ls);
-    if (e == cudaSuccess) e = dalloc(&h->d_chosen, Ls);
-    if (e != cudaSuccess) {
-        g_dp_create_error = std::string("pqp_dp_create: ") + cudaGetErrorString(e);
+    const int rc = [&]() -> int {
+        std::string &err = g_dp_create_error;
+        pqp::Resources &r = h->res;
+        const size_t B = batch_max, T = B * layers_max * h->J, Ls = B * layers_max;
+        PQP_CUDA(err, r.stream(h->stream));
+        PQP_CUDA(err, r.event(h->ev0));
+        PQP_CUDA(err, r.event(h->ev1));
+        PQP_CUDA(err, r.alloc(h->d_nx, T));
+        PQP_CUDA(err, r.alloc(h->d_ny, T));
+        PQP_CUDA(err, r.alloc(h->d_dis, T));
+        PQP_CUDA(err, r.alloc(h->d_cost, T));
+        PQP_CUDA(err, r.alloc(h->d_parent, T));
+        PQP_CUDA(err, r.alloc(h->d_feasible, T));
+        PQP_CUDA(err, r.alloc(h->d_ref, Ls * 4));
+        PQP_CUDA(err, r.alloc(h->d_length, B));
+        PQP_CUDA(err, r.alloc(h->d_start, B * 3));
+        PQP_CUDA(err, r.alloc(h->d_k, B));
+        PQP_CUDA(err, r.alloc(h->d_status, B));
+        PQP_CUDA(err, r.alloc(h->d_n_layers, B));
+        PQP_CUDA(err, r.alloc(h->d_n_out, B));
+        PQP_CUDA(err, r.alloc(h->d_vehicle_l, B));
+        PQP_CUDA(err, r.alloc(h->d_target_s, B));
+        PQP_CUDA(err, r.alloc(h->d_layer_s, Ls));
+        PQP_CUDA(err, r.alloc(h->d_lower, Ls));
+        PQP_CUDA(err, r.alloc(h->d_upper, Ls));
+        PQP_CUDA(err, r.alloc(h->d_chosen, Ls));
+        return PQP_OK;
+    }();
+    if (rc != PQP_OK) {
         pqp_dp_destroy(h);
-        return PQP_E_CUDA;
+        return rc;
     }
     *out = h;
     return PQP_OK;
@@ -264,13 +247,6 @@ void pqp_dp_destroy(pqp_dp_handle *h) {
     if (!h) return;
     pqp::DeviceGuard guard_(h->device);
     if (h->stream) cudaStreamSynchronize(h->stream);
-    cudaFree(h->d_nx); cudaFree(h->d_ny); cudaFree(h->d_dis); cudaFree(h->d_ref); cudaFree(h->d_cost);
-    cudaFree(h->d_parent); cudaFree(h->d_feasible); cudaFree(h->d_spline); cudaFree(h->d_length); cudaFree(h->d_start);
-    cudaFree(h->d_layer_s); cudaFree(h->d_lower); cudaFree(h->d_upper); cudaFree(h->d_vehicle_l); cudaFree(h->d_target_s);
-    cudaFree(h->d_k); cudaFree(h->d_status); cudaFree(h->d_n_layers); cudaFree(h->d_n_out); cudaFree(h->d_chosen);
-    if (h->ev0) cudaEventDestroy(h->ev0);
-    if (h->ev1) cudaEventDestroy(h->ev1);
-    if (h->stream) cudaStreamDestroy(h->stream);
     delete h;
 }
 
@@ -288,40 +264,35 @@ int pqp_dp_search(pqp_dp_handle *h, const pqp_dp_in *in, const pqp_dp_out *out) 
     if (rc != PQP_OK) return rc;
     pqp::DeviceGuard guard_(h->device);
     const size_t B = in->batch, nsp = B * PQP_SPLINE_ROWS * in->k_max, Ls = B * h->layers_max, T = Ls * h->J;
-    if (nsp > h->cap_spline) {
-        cudaFree(h->d_spline);
-        h->d_spline = nullptr;
-        PQD_CUDA(h, dalloc(&h->d_spline, nsp));
-        h->cap_spline = nsp;
-    }
+    PQP_CUDA(h->err, h->res.grow(h->d_spline, nsp));
     cudaStream_t s = h->stream;
-    PQD_CUDA(h, cudaMemcpyAsync(h->d_spline, in->spline, nsp * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQD_CUDA(h, cudaMemcpyAsync(h->d_k, in->k, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    PQD_CUDA(h, cudaMemcpyAsync(h->d_length, in->length, B * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQD_CUDA(h, cudaMemcpyAsync(h->d_start, in->start, B * 3 * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQD_CUDA(h, cudaMemsetAsync(h->d_chosen, 0, Ls * sizeof(int32_t), s));
-    PQD_CUDA(h, cudaMemsetAsync(h->d_layer_s, 0, Ls * sizeof(double), s));
-    PQD_CUDA(h, cudaMemsetAsync(h->d_lower, 0, Ls * sizeof(double), s));
-    PQD_CUDA(h, cudaMemsetAsync(h->d_upper, 0, Ls * sizeof(double), s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_spline, in->spline, nsp * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_k, in->k, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_length, in->length, B * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_start, in->start, B * 3 * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemsetAsync(h->d_chosen, 0, Ls * sizeof(int32_t), s));
+    PQP_CUDA(h->err, cudaMemsetAsync(h->d_layer_s, 0, Ls * sizeof(double), s));
+    PQP_CUDA(h->err, cudaMemsetAsync(h->d_lower, 0, Ls * sizeof(double), s));
+    PQP_CUDA(h->err, cudaMemsetAsync(h->d_upper, 0, Ls * sizeof(double), s));
     pqp_dp_in din = {in->batch, in->k_max, h->d_spline, h->d_k, h->d_length, h->d_start};
     pqp_dp_out dout = {h->d_status, h->d_n_layers, h->d_n_out, h->d_layer_s, h->d_lower, h->d_upper, h->d_chosen,
                        h->d_vehicle_l, h->d_target_s, nullptr, nullptr, nullptr};
     rc = launch(h, &din, &dout, s);
     if (rc != PQP_OK) return rc;
-    PQD_CUDA(h, cudaMemcpyAsync(out->status, h->d_status, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    PQD_CUDA(h, cudaMemcpyAsync(out->n_layers, h->d_n_layers, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    PQD_CUDA(h, cudaMemcpyAsync(out->n_out, h->d_n_out, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    PQD_CUDA(h, cudaMemcpyAsync(out->vehicle_l, h->d_vehicle_l, B * sizeof(double), cudaMemcpyDeviceToHost, s));
-    PQD_CUDA(h, cudaMemcpyAsync(out->target_s, h->d_target_s, B * sizeof(double), cudaMemcpyDeviceToHost, s));
-    PQD_CUDA(h, cudaMemcpyAsync(out->layer_s, h->d_layer_s, Ls * sizeof(double), cudaMemcpyDeviceToHost, s));
-    PQD_CUDA(h, cudaMemcpyAsync(out->lower, h->d_lower, Ls * sizeof(double), cudaMemcpyDeviceToHost, s));
-    PQD_CUDA(h, cudaMemcpyAsync(out->upper, h->d_upper, Ls * sizeof(double), cudaMemcpyDeviceToHost, s));
-    PQD_CUDA(h, cudaMemcpyAsync(out->chosen, h->d_chosen, Ls * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    if (out->cost) PQD_CUDA(h, cudaMemcpyAsync(out->cost, h->d_cost, T * sizeof(double), cudaMemcpyDeviceToHost, s));
-    if (out->parent) PQD_CUDA(h, cudaMemcpyAsync(out->parent, h->d_parent, T * sizeof(int8_t), cudaMemcpyDeviceToHost, s));
-    if (out->feasible) PQD_CUDA(h, cudaMemcpyAsync(out->feasible, h->d_feasible, T * sizeof(uint8_t), cudaMemcpyDeviceToHost, s));
-    PQD_CUDA(h, cudaStreamSynchronize(s));
-    PQD_CUDA(h, cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1));
+    PQP_CUDA(h->err, cudaMemcpyAsync(out->status, h->d_status, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(out->n_layers, h->d_n_layers, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(out->n_out, h->d_n_out, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(out->vehicle_l, h->d_vehicle_l, B * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(out->target_s, h->d_target_s, B * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(out->layer_s, h->d_layer_s, Ls * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(out->lower, h->d_lower, Ls * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(out->upper, h->d_upper, Ls * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(out->chosen, h->d_chosen, Ls * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    if (out->cost) PQP_CUDA(h->err, cudaMemcpyAsync(out->cost, h->d_cost, T * sizeof(double), cudaMemcpyDeviceToHost, s));
+    if (out->parent) PQP_CUDA(h->err, cudaMemcpyAsync(out->parent, h->d_parent, T * sizeof(int8_t), cudaMemcpyDeviceToHost, s));
+    if (out->feasible) PQP_CUDA(h->err, cudaMemcpyAsync(out->feasible, h->d_feasible, T * sizeof(uint8_t), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaStreamSynchronize(s));
+    PQP_CUDA(h->err, cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1));
     return PQP_OK;
 }
 

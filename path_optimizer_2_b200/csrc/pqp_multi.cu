@@ -13,7 +13,7 @@
 #include <vector>
 
 #include "../../include/pqp_multi.h"
-#include "pqp_device_guard.h"
+#include "pqp_host_handle.h"
 
 namespace {
 
@@ -70,31 +70,28 @@ struct pqp_multi {
     int last_batch = 0, last_per = 0;
     float gather_ms = 0.0f;
     std::string err;
+    std::vector<pqp::Resources> res;  // one per device; last member: releasing clears the members above
 };
 
 namespace {
 
-int mfail(pqp_multi *m, int code, const std::string &msg) {
-    if (m) m->err = msg;
-    else g_multi_create_error = msg;
-    return code;
-}
+using pqp::fail;
 
 int run(pqp_multi *m, const pqp_batch_in *in, const pqp_batch_out *out, bool warm) {
     if (!m) return PQP_E_INVALID;
-    if (!out || !out->sol) return mfail(m, PQP_E_INVALID, "null output");
+    if (!out || !out->sol) return fail(m->err, PQP_E_INVALID, "null output");
     int B;
     if (in) {
-        if (!in->knots || !in->inst || !in->n) return mfail(m, PQP_E_INVALID, "null buffer");
-        if (in->batch < 1 || in->batch > m->batch_max) return mfail(m, PQP_E_INVALID, "batch out of range");
-        if (in->n_max != m->n_max) return mfail(m, PQP_E_INVALID, "n_max differs from the handle's");
+        if (!in->knots || !in->inst || !in->n) return fail(m->err, PQP_E_INVALID, "null buffer");
+        if (in->batch < 1 || in->batch > m->batch_max) return fail(m->err, PQP_E_INVALID, "batch out of range");
+        if (in->n_max != m->n_max) return fail(m->err, PQP_E_INVALID, "n_max differs from the handle's");
         B = in->batch;
     } else {
-        if (!warm) return mfail(m, PQP_E_INVALID, "null batch");
+        if (!warm) return fail(m->err, PQP_E_INVALID, "null batch");
         B = m->last_batch;
-        if (B < 1) return mfail(m, PQP_E_STATE, "resolve(NULL) needs a previous solve");
+        if (B < 1) return fail(m->err, PQP_E_STATE, "resolve(NULL) needs a previous solve");
     }
-    if (warm && B != m->last_batch) return mfail(m, PQP_E_STATE, "resolve needs a previous solve of the same batch");
+    if (warm && B != m->last_batch) return fail(m->err, PQP_E_STATE, "resolve needs a previous solve of the same batch");
     const int G = m->n_dev, nmax = m->n_max;
     const int per = (B + G - 1) / G;
     const size_t nvm = 6 * (size_t)nmax - 1, mm = 6 * (size_t)nmax + 2;
@@ -128,7 +125,7 @@ int run(pqp_multi *m, const pqp_batch_in *in, const pqp_batch_out *out, bool war
     work(0);
     for (auto &t : workers) t.join();
     for (int d = 0; d < G; ++d)
-        if (rc[d] != PQP_OK) return mfail(m, rc[d], std::string("device ") + std::to_string(m->dev[d]) + ": " + pqp_last_error(m->h[d]));
+        if (rc[d] != PQP_OK) return fail(m->err, rc[d], std::string("device ") + std::to_string(m->dev[d]) + ": " + pqp_last_error(m->h[d]));
     m->last_batch = B;
     m->last_per = per;
     // pack on every device, then one all-gather of per * 16 bytes per device
@@ -142,7 +139,7 @@ int run(pqp_multi *m, const pqp_batch_in *in, const pqp_batch_out *out, bool war
             const int32_t *status, *iters;
             int r = pqp_resident_results(m->h[d], nullptr, &cost, &status, &iters);
             if (r == PQP_OK) r = pqp_pack_results_device(m->h[d], hi - lo, cost, status, iters, m->d_send[d], m->stream[d]);
-            if (r != PQP_OK) return mfail(m, r, pqp_last_error(m->h[d]));
+            if (r != PQP_OK) return fail(m->err, r, pqp_last_error(m->h[d]));
         }
     }
     if (G == 1) {
@@ -155,14 +152,13 @@ int run(pqp_multi *m, const pqp_batch_in *in, const pqp_batch_out *out, bool war
             e = N.AllGather(m->d_send[d], m->d_table[d], (size_t)per * sizeof(pqp_result_rec), /*ncclInt8*/ 0, m->comm[d], m->stream[d]);
         const int e2 = N.GroupEnd();
         if (e == 0) e = e2;
-        if (e != 0) return mfail(m, PQP_E_CUDA, std::string("ncclAllGather: ") + N.GetErrorString(e));
+        if (e != 0) return fail(m->err, PQP_E_CUDA, std::string("ncclAllGather: ") + N.GetErrorString(e));
     }
     float worst = 0.0f;
     for (int d = 0; d < G; ++d) {
         pqp::DeviceGuard g(m->dev[d]);
         cudaEventRecord(m->ev1[d], m->stream[d]);
-        const cudaError_t ce = cudaStreamSynchronize(m->stream[d]);
-        if (ce != cudaSuccess) return mfail(m, PQP_E_CUDA, std::string("gather: ") + cudaGetErrorString(ce));
+        PQP_CUDA(m->err, cudaStreamSynchronize(m->stream[d]));
         float ms = 0.0f;
         cudaEventElapsedTime(&ms, m->ev0[d], m->ev1[d]);
         worst = std::max(worst, ms);
@@ -179,15 +175,16 @@ const char *pqp_multi_last_error(const pqp_multi *m) { return m ? m->err.c_str()
 
 int pqp_multi_create(const pqp_params *params, int32_t n_max, int32_t batch_max, int32_t n_devices,
                      const int32_t *devices, pqp_multi **out) {
-    if (!out) return mfail(nullptr, PQP_E_INVALID, "out is null");
+    std::string &err = g_multi_create_error;
+    if (!out) return fail(err, PQP_E_INVALID, "out is null");
     *out = nullptr;
-    if (!params || n_devices < 1 || batch_max < 1) return mfail(nullptr, PQP_E_INVALID, "invalid arguments");
+    if (!params || n_devices < 1 || batch_max < 1) return fail(err, PQP_E_INVALID, "invalid arguments");
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < n_devices)
-        return mfail(nullptr, PQP_E_NO_DEVICE, "fewer CUDA devices than n_devices (there is no CPU fallback)");
+        return fail(err, PQP_E_NO_DEVICE, "fewer CUDA devices than n_devices (there is no CPU fallback)");
     if (n_devices > 1 && !nccl().load(&g_multi_create_error)) return PQP_E_NO_DEVICE;
     pqp_multi *m = new (std::nothrow) pqp_multi;
-    if (!m) return mfail(nullptr, PQP_E_INVALID, "out of host memory");
+    if (!m) return fail(err, PQP_E_INVALID, "out of host memory");
     m->n_dev = n_devices;
     m->n_max = n_max;
     m->batch_max = batch_max;
@@ -201,34 +198,32 @@ int pqp_multi_create(const pqp_params *params, int32_t n_max, int32_t batch_max,
     m->d_send.assign(G, nullptr);
     m->d_table.assign(G, nullptr);
     m->comm.assign(G, nullptr);
-    for (int d = 0; d < n_devices; ++d) m->dev[d] = devices ? devices[d] : d;
-    for (int d = 0; d < n_devices; ++d) {
-        int rc = pqp_create(params, n_max, m->per_max, m->dev[d], &m->h[d]);
-        if (rc != PQP_OK) {
-            g_multi_create_error = pqp_last_error(nullptr);
-            pqp_multi_destroy(m);
-            return rc;
+    m->res = std::vector<pqp::Resources>(G);
+    for (int d = 0; d < n_devices; ++d) m->dev[d] = m->res[d].device = devices ? devices[d] : d;
+    const int rc = [&]() -> int {
+        for (int d = 0; d < n_devices; ++d) {
+            const int hrc = pqp_create(params, n_max, m->per_max, m->dev[d], &m->h[d]);
+            if (hrc != PQP_OK) return fail(err, hrc, pqp_last_error(nullptr));
+            pqp::DeviceGuard g(m->dev[d]);
+            pqp::Resources &r = m->res[d];
+            PQP_CUDA(err, r.stream(m->stream[d]));
+            PQP_CUDA(err, r.event(m->ev0[d]));
+            PQP_CUDA(err, r.event(m->ev1[d]));
+            PQP_CUDA(err, r.alloc(m->d_send[d], (size_t)m->per_max));
+            PQP_CUDA(err, r.alloc(m->d_table[d], G * m->per_max));
         }
-        pqp::DeviceGuard g(m->dev[d]);
-        cudaError_t e = cudaStreamCreateWithFlags(&m->stream[d], cudaStreamNonBlocking);
-        if (e == cudaSuccess) e = cudaEventCreate(&m->ev0[d]);
-        if (e == cudaSuccess) e = cudaEventCreate(&m->ev1[d]);
-        if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void **>(&m->d_send[d]), (size_t)m->per_max * sizeof(pqp_result_rec));
-        if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void **>(&m->d_table[d]), G * m->per_max * sizeof(pqp_result_rec));
-        if (e != cudaSuccess) {
-            g_multi_create_error = std::string("pqp_multi_create: ") + cudaGetErrorString(e);
-            pqp_multi_destroy(m);
-            return PQP_E_CUDA;
+        if (n_devices > 1) {
+            const int e = nccl().CommInitAll(m->comm.data(), n_devices, m->dev.data());
+            if (e != 0) {
+                for (auto &c : m->comm) c = nullptr;
+                return fail(err, PQP_E_CUDA, std::string("ncclCommInitAll: ") + nccl().GetErrorString(e));
+            }
         }
-    }
-    if (n_devices > 1) {
-        const int e = nccl().CommInitAll(m->comm.data(), n_devices, m->dev.data());
-        if (e != 0) {
-            g_multi_create_error = std::string("ncclCommInitAll: ") + nccl().GetErrorString(e);
-            for (auto &c : m->comm) c = nullptr;
-            pqp_multi_destroy(m);
-            return PQP_E_CUDA;
-        }
+        return PQP_OK;
+    }();
+    if (rc != PQP_OK) {
+        pqp_multi_destroy(m);
+        return rc;
     }
     *out = m;
     return PQP_OK;
@@ -241,11 +236,6 @@ int pqp_multi_destroy(pqp_multi *m) {
         if (m->stream[d]) cudaStreamSynchronize(m->stream[d]);
         if (m->comm[d]) nccl().CommDestroy(m->comm[d]);
         if (m->h[d]) pqp_destroy(m->h[d]);
-        cudaFree(m->d_send[d]);
-        cudaFree(m->d_table[d]);
-        if (m->ev0[d]) cudaEventDestroy(m->ev0[d]);
-        if (m->ev1[d]) cudaEventDestroy(m->ev1[d]);
-        if (m->stream[d]) cudaStreamDestroy(m->stream[d]);
     }
     delete m;
     return PQP_OK;
@@ -253,7 +243,7 @@ int pqp_multi_destroy(pqp_multi *m) {
 
 int pqp_multi_solve(pqp_multi *m, const pqp_batch_in *in, const pqp_batch_out *out) {
     if (!m) return PQP_E_INVALID;
-    if (!in) return mfail(m, PQP_E_INVALID, "null batch");
+    if (!in) return fail(m->err, PQP_E_INVALID, "null batch");
     return run(m, in, out, false);
 }
 
@@ -261,7 +251,7 @@ int pqp_multi_resolve(pqp_multi *m, const pqp_batch_in *in, const pqp_batch_out 
 
 int pqp_multi_gathered(pqp_multi *m, int32_t i, const pqp_result_rec **table, int32_t *per) {
     if (!m || i < 0 || i >= m->n_dev) return PQP_E_INVALID;
-    if (m->last_batch < 1) return mfail(m, PQP_E_STATE, "nothing solved yet");
+    if (m->last_batch < 1) return fail(m->err, PQP_E_STATE, "nothing solved yet");
     if (table) *table = m->d_table[i];
     if (per) *per = m->last_per;
     return PQP_OK;

@@ -14,7 +14,7 @@
 
 #include "../../include/pqp_plan.h"
 #include "pqp_bounds_internal.h"
-#include "pqp_device_guard.h"
+#include "pqp_host_handle.h"
 #include "pqp_plan_core.cuh"
 #include "pqp_smoother_internal.h"
 
@@ -341,11 +341,6 @@ __global__ void final_kernel(const FinalArgs a) {
     }
 }
 
-template <typename T>
-cudaError_t dalloc(T **p, size_t n) {
-    return cudaMalloc(reinterpret_cast<void **>(p), (n ? n : 1) * sizeof(T));
-}
-
 }  // namespace
 
 struct pqp_plan_handle {
@@ -385,59 +380,54 @@ struct pqp_plan_handle {
     double *full[6] = {};  // x, y, z of the first solve, then of the second: written only when traced
     int32_t *status1 = nullptr, *iters1 = nullptr, *status2 = nullptr, *iters2 = nullptr;
     std::string err;
+    pqp::Resources res;  // last member: releasing clears the members above
 };
 
 namespace {
 
-int pfail(pqp_plan_handle *h, int code, const std::string &msg) {
-    if (h) h->err = msg;
-    else g_plan_create_error = msg;
-    return code;
-}
+using pqp::fail;
 
-#define PQL_CUDA(h, call)                                                  \
-    do {                                                                   \
-        cudaError_t e_ = (call);                                           \
-        if (e_ != cudaSuccess) {                                           \
-            (h)->err = std::string(#call) + ": " + cudaGetErrorString(e_); \
-            return PQP_E_CUDA;                                             \
-        }                                                                  \
+#define PQL_SUB(h, call, errfn, sub)                                                              \
+    do {                                                                                          \
+        const int rc_ = (call);                                                                   \
+        if (rc_ != PQP_OK) return fail((h)->err, rc_, std::string(#call) + ": " + errfn(sub));   \
     } while (0)
 
-#define PQL_SUB(h, call, errfn, sub)                                                          \
-    do {                                                                                      \
-        const int rc_ = (call);                                                               \
-        if (rc_ != PQP_OK) return pfail((h), rc_, std::string(#call) + ": " + errfn(sub));   \
+// a stage handle's create inside pqp_plan_create: its error is the plan's create error
+#define PQL_SUB_CREATE(call, errfn)                                                                \
+    do {                                                                                           \
+        const int rc_ = (call);                                                                    \
+        if (rc_ != PQP_OK) return fail(g_plan_create_error, rc_, std::string("pqp_plan_create: ") + errfn(nullptr)); \
     } while (0)
 
 #define PQL_LAUNCH(h)                              \
     do {                                           \
-        PQL_CUDA(h, cudaGetLastError());           \
+        PQP_CUDA((h)->err, cudaGetLastError());    \
         (h)->launches++;                           \
     } while (0)
 
 int validate(pqp_plan_handle *h, const pqp_plan_in *in, const pqp_plan_out *out) {
     if (!h) return PQP_E_INVALID;
-    if (!in || !out) return pfail(h, PQP_E_INVALID, "null batch");
-    if (!in->raw_x || !in->raw_y || !in->r || !in->start || !in->target) return pfail(h, PQP_E_INVALID, "null input buffer");
-    if (!out->status || !out->n || !out->path || !out->cost || !out->iters) return pfail(h, PQP_E_INVALID, "null output buffer");
-    if (in->batch < 1 || in->batch > h->batch_max) return pfail(h, PQP_E_INVALID, "batch out of range");
-    if (in->r_max < 3 || in->r_max > h->R) return pfail(h, PQP_E_INVALID, "r_max must be in [3, the handle's r_max]");
+    if (!in || !out) return fail(h->err, PQP_E_INVALID, "null batch");
+    if (!in->raw_x || !in->raw_y || !in->r || !in->start || !in->target) return fail(h->err, PQP_E_INVALID, "null input buffer");
+    if (!out->status || !out->n || !out->path || !out->cost || !out->iters) return fail(h->err, PQP_E_INVALID, "null output buffer");
+    if (in->batch < 1 || in->batch > h->batch_max) return fail(h->err, PQP_E_INVALID, "batch out of range");
+    if (in->r_max < 3 || in->r_max > h->R) return fail(h->err, PQP_E_INVALID, "r_max must be in [3, the handle's r_max]");
     return PQP_OK;
 }
 
 int validate_points(pqp_plan_handle *h, const pqp_plan_points_in *in, const pqp_plan_out *out) {
     if (!h) return PQP_E_INVALID;
-    if (!in || !out) return pfail(h, PQP_E_INVALID, "null batch");
-    if (!in->ref_x || !in->ref_y || !in->m || !in->start || !in->target) return pfail(h, PQP_E_INVALID, "null input buffer");
-    if (!out->status || !out->n || !out->path || !out->cost || !out->iters) return pfail(h, PQP_E_INVALID, "null output buffer");
-    if (in->batch < 1 || in->batch > h->batch_max) return pfail(h, PQP_E_INVALID, "batch out of range");
-    if (in->m_max < 1 || in->m_max > h->R) return pfail(h, PQP_E_INVALID, "m_max must be in [1, the handle's r_max]");
+    if (!in || !out) return fail(h->err, PQP_E_INVALID, "null batch");
+    if (!in->ref_x || !in->ref_y || !in->m || !in->start || !in->target) return fail(h->err, PQP_E_INVALID, "null input buffer");
+    if (!out->status || !out->n || !out->path || !out->cost || !out->iters) return fail(h->err, PQP_E_INVALID, "null output buffer");
+    if (in->batch < 1 || in->batch > h->batch_max) return fail(h->err, PQP_E_INVALID, "batch out of range");
+    if (in->m_max < 1 || in->m_max > h->R) return fail(h->err, PQP_E_INVALID, "m_max must be in [1, the handle's r_max]");
     return PQP_OK;
 }
 
 int copy_out(pqp_plan_handle *h, void *dst, const void *src, size_t bytes, cudaStream_t s) {
-    if (dst) PQL_CUDA(h, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, s));
+    if (dst) PQP_CUDA(h->err, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, s));
     return PQP_OK;
 }
 
@@ -503,12 +493,12 @@ int copy_trace(pqp_plan_handle *h, const pqp_plan_trace *t, int B, bool points, 
 // the host calls' outputs from the handle's staging buffers; waits for the call to finish
 int copy_results(pqp_plan_handle *h, const pqp_plan_out *out, int batch, cudaStream_t s) {
     const size_t B = batch, N = h->N;
-    PQL_CUDA(h, cudaMemcpyAsync(out->status, h->o_status, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    PQL_CUDA(h, cudaMemcpyAsync(out->n, h->o_n, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    PQL_CUDA(h, cudaMemcpyAsync(out->iters, h->o_iters, B * 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    PQL_CUDA(h, cudaMemcpyAsync(out->cost, h->o_cost, B * sizeof(double), cudaMemcpyDeviceToHost, s));
-    PQL_CUDA(h, cudaMemcpyAsync(out->path, h->o_path, B * PQP_PLAN_PATH_ROWS * N * sizeof(double), cudaMemcpyDeviceToHost, s));
-    PQL_CUDA(h, cudaStreamSynchronize(s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(out->status, h->o_status, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(out->n, h->o_n, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(out->iters, h->o_iters, B * 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(out->cost, h->o_cost, B * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(out->path, h->o_path, B * PQP_PLAN_PATH_ROWS * N * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaStreamSynchronize(s));
     return PQP_OK;
 }
 
@@ -520,7 +510,7 @@ int run(pqp_plan_handle *h, const pqp_plan_in *in, const pqp_plan_out *out, cuda
     const Dims d{B, h->R, h->P, h->L, h->N, in->r_max};
     const pqp_plan_trace *tr = out->trace;
     h->timed = true;
-    PQL_CUDA(h, cudaEventRecord(h->ev[0], s));
+    PQP_CUDA(h->err, cudaEventRecord(h->ev[0], s));
     // ---- reference path smoothing (ReferencePathSmoother::solve) ----
     if (pts) {
         bspline_prep_kernel<<<blocks_for(B), kThreads, 0, s>>>(d, pts->m_max, pts->ref_x, pts->ref_y, pts->m, h->bs_t,
@@ -574,7 +564,7 @@ int run(pqp_plan_handle *h, const pqp_plan_in *in, const pqp_plan_out *out, cuda
     PQL_LAUNCH(h);
     fit_kernel<<<blocks_for(2LL * B), kThreads, 0, s>>>(B, h->L, h->r_rows, h->rk);
     PQL_LAUNCH(h);
-    PQL_CUDA(h, cudaEventRecord(h->ev[1], s));
+    PQP_CUDA(h->err, cudaEventRecord(h->ev[1], s));
     // ---- processReferencePath ----
     process_kernel<<<blocks_for(B), kThreads, 0, s>>>(d, h->prm.bounds.epsilon, h->r_rows, h->rk, h->r_len, in->start,
                                                        in->target, h->status, h->max_s, h->inst);
@@ -614,10 +604,10 @@ int run(pqp_plan_handle *h, const pqp_plan_in *in, const pqp_plan_out *out, cuda
         inst_kernel<<<blocks_for(B), kThreads, 0, s>>>(a);
         PQL_LAUNCH(h);
     }
-    PQL_CUDA(h, cudaEventRecord(h->ev[2], s));
+    PQP_CUDA(h->err, cudaEventRecord(h->ev[2], s));
     // ---- optimizePath: solve, updateProblemFormulationAndSolve, getOptimizedPath ----
     const size_t kb = (size_t)B * PQP_NFIELDS * h->N * sizeof(double);
-    PQL_CUDA(h, cudaMemcpyAsync(h->knots2, h->knots, kb, cudaMemcpyDeviceToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->knots2, h->knots, kb, cudaMemcpyDeviceToDevice, s));
     {
         pqp_batch_in bi = {B, h->N, h->knots, h->inst, h->n1, h->p};
         pqp_batch_out bo = {h->sol1, h->cost1, h->status1, h->iters1, (tr && tr->x_full1) ? h->full[0] : nullptr,
@@ -657,7 +647,7 @@ int run(pqp_plan_handle *h, const pqp_plan_in *in, const pqp_plan_out *out, cuda
         final_kernel<<<blocks_for((long long)B * h->N), kThreads, 0, s>>>(a);
         PQL_LAUNCH(h);
     }
-    PQL_CUDA(h, cudaEventRecord(h->ev[3], s));
+    PQP_CUDA(h->err, cudaEventRecord(h->ev[3], s));
     h->launches += kStageLaunches;
     return copy_trace(h, tr, B, pts != nullptr, s);
 }
@@ -693,145 +683,127 @@ int pqp_plan_create(const pqp_bounds_map *map, const pqp_plan_params *params, in
                     int32_t layers_max, int32_t n_max, int32_t batch_max, int32_t device, pqp_plan_handle **out) {
     if (!out) return PQP_E_INVALID;
     *out = nullptr;
-    if (!map) return pfail(nullptr, PQP_E_INVALID, "pqp_plan_create: a map is required");
+    if (!map) return fail(g_plan_create_error, PQP_E_INVALID, "pqp_plan_create: a map is required");
     if (r_max < 3 || p_max < 4 || layers_max < 4 || n_max < 2 || n_max > 511 || batch_max < 1)
-        return pfail(nullptr, PQP_E_INVALID,
-                     "pqp_plan_create: r_max >= 3, p_max >= 4, layers_max >= 4, 2 <= n_max <= 511, batch_max >= 1");
+        return fail(g_plan_create_error, PQP_E_INVALID,
+                    "pqp_plan_create: r_max >= 3, p_max >= 4, layers_max >= 4, 2 <= n_max <= 511, batch_max >= 1");
     pqp_plan_params dflt;
     pqp_plan_default_params(&dflt);
+    const pqp_plan_params &prm = params ? *params : dflt;
+    if (!(prm.output_spacing > 0))
+        return fail(g_plan_create_error, PQP_E_INVALID, "pqp_plan_create: output_spacing must be positive");
+    if (prm.smoothing_method != PQP_PLAN_SMOOTH_TENSION2 && prm.smoothing_method != PQP_PLAN_SMOOTH_TENSION)
+        return fail(g_plan_create_error, PQP_E_INVALID,
+                    "pqp_plan_create: smoothing_method must be PQP_PLAN_SMOOTH_TENSION2 (0) or PQP_PLAN_SMOOTH_TENSION (1)");
     pqp_plan_handle *h = new (std::nothrow) pqp_plan_handle;
-    if (!h) return pfail(nullptr, PQP_E_INVALID, "out of host memory");
-    h->prm = params ? *params : dflt;
-    if (!(h->prm.output_spacing > 0)) {
-        delete h;
-        return pfail(nullptr, PQP_E_INVALID, "pqp_plan_create: output_spacing must be positive");
-    }
-    if (h->prm.smoothing_method != PQP_PLAN_SMOOTH_TENSION2 && h->prm.smoothing_method != PQP_PLAN_SMOOTH_TENSION) {
-        delete h;
-        return pfail(nullptr, PQP_E_INVALID,
-                     "pqp_plan_create: smoothing_method must be PQP_PLAN_SMOOTH_TENSION2 (0) or PQP_PLAN_SMOOTH_TENSION (1)");
-    }
-    h->device = device;
+    if (!h) return fail(g_plan_create_error, PQP_E_INVALID, "out of host memory");
+    h->prm = prm;
+    h->device = h->res.device = device;
     h->R = r_max;
     h->P = p_max;
     h->L = layers_max;
     h->N = n_max;
     h->batch_max = batch_max;
-    int rc = pqp_bounds_create(map, &h->prm.bounds, device, &h->bounds);
-    if (rc == PQP_OK) {
-        rc = pqp_dp_create(h->bounds, &h->prm.dp, layers_max, batch_max, &h->dp);
-        if (rc != PQP_OK) g_plan_create_error = std::string("pqp_plan_create: ") + pqp_dp_last_error(nullptr);
-    } else {
-        g_plan_create_error = std::string("pqp_plan_create: ") + pqp_bounds_last_error(nullptr);
-    }
-    if (rc == PQP_OK) {
-        rc = pqp_smoother_create(&h->prm.smoother, p_max, batch_max, device, &h->tension);
-        if (rc == PQP_OK) rc = pqp_smoother_create(&h->prm.smoother, layers_max, batch_max, device, &h->post);
-        if (rc != PQP_OK) g_plan_create_error = std::string("pqp_plan_create: ") + pqp_smoother_last_error(nullptr);
-    }
-    if (rc == PQP_OK && h->prm.smoothing_method == PQP_PLAN_SMOOTH_TENSION) {
-        if (const char *why = pqs::cartesian_unavailable(h->tension)) {
-            rc = PQP_E_INVALID;
-            g_plan_create_error = std::string("pqp_plan_create: smoothing_method TENSION: ") + why;
-        }
-    }
-    if (rc == PQP_OK) {
-        rc = pqp_create(&h->prm.solver, n_max, batch_max, device, &h->solver);
-        if (rc != PQP_OK) g_plan_create_error = std::string("pqp_plan_create: ") + pqp_last_error(nullptr);
-    }
-    if (rc != PQP_OK) {
-        const std::string msg = g_plan_create_error;
-        pqp_plan_destroy(h);
-        g_plan_create_error = msg;
-        return rc;
-    }
+    std::string &err = g_plan_create_error;
     pqp::DeviceGuard guard_(device);
-    const size_t B = batch_max, R = r_max, P = p_max, L = layers_max, N = n_max, S = PQP_SPLINE_ROWS;
-    cudaError_t e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking);
-    for (int i = 0; i < 4 && e == cudaSuccess; ++i) e = cudaEventCreate(&h->ev[i]);
-    if (e == cudaSuccess) e = dalloc(&h->in_x, B * R);
-    if (e == cudaSuccess) e = dalloc(&h->in_y, B * R);
-    if (e == cudaSuccess) e = dalloc(&h->in_start, B * 4);
-    if (e == cudaSuccess) e = dalloc(&h->in_target, B * 3);
-    if (e == cudaSuccess) e = dalloc(&h->in_r, B);
-    if (e == cudaSuccess) e = dalloc(&h->o_status, B);
-    if (e == cudaSuccess) e = dalloc(&h->o_n, B);
-    if (e == cudaSuccess) e = dalloc(&h->o_iters, B * 2);
-    if (e == cudaSuccess) e = dalloc(&h->o_path, B * PQP_PLAN_PATH_ROWS * N);
-    if (e == cudaSuccess) e = dalloc(&h->o_cost, B);
-    if (e == cudaSuccess) e = dalloc(&h->status, B);
-    if (e == cudaSuccess) e = dalloc(&h->raw_k, B);
-    if (e == cudaSuccess) e = dalloc(&h->seg_p, B);
-    if (e == cudaSuccess) e = dalloc(&h->t_status, B);
-    if (e == cudaSuccess) e = dalloc(&h->t_iters, B);
-    if (e == cudaSuccess) e = dalloc(&h->tk, B);
-    if (e == cudaSuccess) e = dalloc(&h->start3, B * 3);
-    if (e == cudaSuccess) e = dalloc(&h->raw_rows, B * S * R);
-    for (int i = 0; i < 5 && e == cudaSuccess; ++i) e = dalloc(&h->seg[i], B * P);
-    if (e == cudaSuccess) e = dalloc(&h->t_x, B * P);
-    if (e == cudaSuccess) e = dalloc(&h->t_y, B * P);
-    if (e == cudaSuccess) e = dalloc(&h->t_s, B * P);
-    if (e == cudaSuccess) e = dalloc(&h->t_rows, B * S * P);
-    if (e == cudaSuccess) e = dalloc(&h->t_len, B);
-    if (e == cudaSuccess) e = dalloc(&h->dp_status, B);
-    if (e == cudaSuccess) e = dalloc(&h->dp_nl, B);
-    if (e == cudaSuccess) e = dalloc(&h->dp_nout, B);
-    if (e == cudaSuccess) e = dalloc(&h->dp_chosen, B * L);
-    if (e == cudaSuccess) e = dalloc(&h->dp_ls, B * L);
-    if (e == cudaSuccess) e = dalloc(&h->dp_lo, B * L);
-    if (e == cudaSuccess) e = dalloc(&h->dp_up, B * L);
-    if (e == cudaSuccess) e = dalloc(&h->dp_vl, B);
-    if (e == cudaSuccess) e = dalloc(&h->dp_ts, B);
-    if (e == cudaSuccess) e = dalloc(&h->post_p, B);
-    if (e == cudaSuccess) e = dalloc(&h->post_status, B);
-    if (e == cudaSuccess) e = dalloc(&h->post_iters, B);
-    if (e == cudaSuccess) e = dalloc(&h->rk, B);
-    if (e == cudaSuccess) e = dalloc(&h->post_off, B * L);
-    if (e == cudaSuccess) e = dalloc(&h->r_rows, B * S * L);
-    if (e == cudaSuccess) e = dalloc(&h->r_len, B);
-    if (e == cudaSuccess) e = dalloc(&h->max_s, B);
-    if (e == cudaSuccess) e = dalloc(&h->states, B * PQP_STATE_ROWS * N);
-    if (e == cudaSuccess) e = dalloc(&h->curv, B * N);
-    if (e == cudaSuccess) e = dalloc(&h->bnd, B * PQP_BOUND_ROWS * N);
-    if (e == cudaSuccess) e = dalloc(&h->knots, B * PQP_NFIELDS * N);
-    if (e == cudaSuccess) e = dalloc(&h->knots2, B * PQP_NFIELDS * N);
-    if (e == cudaSuccess) e = dalloc(&h->inst, B * PQP_NINST);
-    if (e == cudaSuccess) e = dalloc(&h->ref_xyh, B * 3 * N);
-    if (e == cudaSuccess) e = dalloc(&h->xyh, B * 3 * N);
-    if (e == cudaSuccess) e = dalloc(&h->n_states, B);
-    if (e == cudaSuccess) e = dalloc(&h->total, B);
-    if (e == cudaSuccess) e = dalloc(&h->n_valid, B);
-    if (e == cudaSuccess) e = dalloc(&h->n1, B);
-    if (e == cudaSuccess) e = dalloc(&h->n2, B);
-    if (e == cudaSuccess) e = dalloc(&h->p, B);
-    if (e == cudaSuccess) e = dalloc(&h->sol1, B * 4 * N);
-    if (e == cudaSuccess) e = dalloc(&h->sol2, B * 4 * N);
-    if (e == cudaSuccess) e = dalloc(&h->cost1, B);
-    if (e == cudaSuccess) e = dalloc(&h->cost2, B);
-    if (e == cudaSuccess) e = dalloc(&h->status1, B);
-    if (e == cudaSuccess) e = dalloc(&h->iters1, B);
-    if (e == cudaSuccess) e = dalloc(&h->status2, B);
-    if (e == cudaSuccess) e = dalloc(&h->iters2, B);
-    for (int i = 0; i < 6 && e == cudaSuccess; ++i) e = dalloc(&h->full[i], B * (i % 3 == 0 ? 6 * N - 1 : 6 * N + 2));
-    if (e == cudaSuccess && h->prm.smoothing_method == PQP_PLAN_SMOOTH_TENSION) e = dalloc(&h->t_clear, B * P);
-    if (e == cudaSuccess) e = dalloc(&h->pt_x, B * R);
-    if (e == cudaSuccess) e = dalloc(&h->pt_y, B * R);
-    if (e == cudaSuccess) e = dalloc(&h->pt_m, B);
-    if (e == cudaSuccess) e = dalloc(&h->bs_t, B * R);
-    if (e == cudaSuccess) e = dalloc(&h->raw_r, B);
-    if (e == cudaSuccess) e = dalloc(&h->bs_deg, B);
-    // spline rows are zero beyond each path's k, so every row read past the end of a fit is defined
-    if (e == cudaSuccess) e = cudaMemset(h->raw_rows, 0, B * S * R * sizeof(double));
-    if (e == cudaSuccess) e = cudaMemset(h->t_rows, 0, B * S * P * sizeof(double));
-    if (e == cudaSuccess) e = cudaMemset(h->r_rows, 0, B * S * L * sizeof(double));
-    if (e == cudaSuccess) e = cudaMemset(h->knots, 0, B * PQP_NFIELDS * N * sizeof(double));
-    if (e == cudaSuccess) e = cudaMemset(h->ref_xyh, 0, B * 3 * N * sizeof(double));
-    if (e == cudaSuccess) e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) {
-        const std::string msg = std::string("pqp_plan_create: ") + cudaGetErrorString(e);
+    const int rc = [&]() -> int {
+        PQL_SUB_CREATE(pqp_bounds_create(map, &h->prm.bounds, device, &h->bounds), pqp_bounds_last_error);
+        PQL_SUB_CREATE(pqp_dp_create(h->bounds, &h->prm.dp, layers_max, batch_max, &h->dp), pqp_dp_last_error);
+        PQL_SUB_CREATE(pqp_smoother_create(&h->prm.smoother, p_max, batch_max, device, &h->tension), pqp_smoother_last_error);
+        PQL_SUB_CREATE(pqp_smoother_create(&h->prm.smoother, layers_max, batch_max, device, &h->post), pqp_smoother_last_error);
+        if (h->prm.smoothing_method == PQP_PLAN_SMOOTH_TENSION)
+            if (const char *why = pqs::cartesian_unavailable(h->tension))
+                return fail(err, PQP_E_INVALID, std::string("pqp_plan_create: smoothing_method TENSION: ") + why);
+        PQL_SUB_CREATE(pqp_create(&h->prm.solver, n_max, batch_max, device, &h->solver), pqp_last_error);
+        pqp::Resources &r = h->res;
+        const size_t B = batch_max, R = r_max, P = p_max, L = layers_max, N = n_max, S = PQP_SPLINE_ROWS;
+        PQP_CUDA(err, r.stream(h->stream));
+        for (int i = 0; i < 4; ++i) PQP_CUDA(err, r.event(h->ev[i]));
+        PQP_CUDA(err, r.alloc(h->in_x, B * R));
+        PQP_CUDA(err, r.alloc(h->in_y, B * R));
+        PQP_CUDA(err, r.alloc(h->in_start, B * 4));
+        PQP_CUDA(err, r.alloc(h->in_target, B * 3));
+        PQP_CUDA(err, r.alloc(h->in_r, B));
+        PQP_CUDA(err, r.alloc(h->o_status, B));
+        PQP_CUDA(err, r.alloc(h->o_n, B));
+        PQP_CUDA(err, r.alloc(h->o_iters, B * 2));
+        PQP_CUDA(err, r.alloc(h->o_path, B * PQP_PLAN_PATH_ROWS * N));
+        PQP_CUDA(err, r.alloc(h->o_cost, B));
+        PQP_CUDA(err, r.alloc(h->status, B));
+        PQP_CUDA(err, r.alloc(h->raw_k, B));
+        PQP_CUDA(err, r.alloc(h->seg_p, B));
+        PQP_CUDA(err, r.alloc(h->t_status, B));
+        PQP_CUDA(err, r.alloc(h->t_iters, B));
+        PQP_CUDA(err, r.alloc(h->tk, B));
+        PQP_CUDA(err, r.alloc(h->start3, B * 3));
+        PQP_CUDA(err, r.alloc(h->raw_rows, B * S * R));
+        for (int i = 0; i < 5; ++i) PQP_CUDA(err, r.alloc(h->seg[i], B * P));
+        PQP_CUDA(err, r.alloc(h->t_x, B * P));
+        PQP_CUDA(err, r.alloc(h->t_y, B * P));
+        PQP_CUDA(err, r.alloc(h->t_s, B * P));
+        PQP_CUDA(err, r.alloc(h->t_rows, B * S * P));
+        PQP_CUDA(err, r.alloc(h->t_len, B));
+        PQP_CUDA(err, r.alloc(h->dp_status, B));
+        PQP_CUDA(err, r.alloc(h->dp_nl, B));
+        PQP_CUDA(err, r.alloc(h->dp_nout, B));
+        PQP_CUDA(err, r.alloc(h->dp_chosen, B * L));
+        PQP_CUDA(err, r.alloc(h->dp_ls, B * L));
+        PQP_CUDA(err, r.alloc(h->dp_lo, B * L));
+        PQP_CUDA(err, r.alloc(h->dp_up, B * L));
+        PQP_CUDA(err, r.alloc(h->dp_vl, B));
+        PQP_CUDA(err, r.alloc(h->dp_ts, B));
+        PQP_CUDA(err, r.alloc(h->post_p, B));
+        PQP_CUDA(err, r.alloc(h->post_status, B));
+        PQP_CUDA(err, r.alloc(h->post_iters, B));
+        PQP_CUDA(err, r.alloc(h->rk, B));
+        PQP_CUDA(err, r.alloc(h->post_off, B * L));
+        PQP_CUDA(err, r.alloc(h->r_rows, B * S * L));
+        PQP_CUDA(err, r.alloc(h->r_len, B));
+        PQP_CUDA(err, r.alloc(h->max_s, B));
+        PQP_CUDA(err, r.alloc(h->states, B * PQP_STATE_ROWS * N));
+        PQP_CUDA(err, r.alloc(h->curv, B * N));
+        PQP_CUDA(err, r.alloc(h->bnd, B * PQP_BOUND_ROWS * N));
+        PQP_CUDA(err, r.alloc(h->knots, B * PQP_NFIELDS * N));
+        PQP_CUDA(err, r.alloc(h->knots2, B * PQP_NFIELDS * N));
+        PQP_CUDA(err, r.alloc(h->inst, B * PQP_NINST));
+        PQP_CUDA(err, r.alloc(h->ref_xyh, B * 3 * N));
+        PQP_CUDA(err, r.alloc(h->xyh, B * 3 * N));
+        PQP_CUDA(err, r.alloc(h->n_states, B));
+        PQP_CUDA(err, r.alloc(h->total, B));
+        PQP_CUDA(err, r.alloc(h->n_valid, B));
+        PQP_CUDA(err, r.alloc(h->n1, B));
+        PQP_CUDA(err, r.alloc(h->n2, B));
+        PQP_CUDA(err, r.alloc(h->p, B));
+        PQP_CUDA(err, r.alloc(h->sol1, B * 4 * N));
+        PQP_CUDA(err, r.alloc(h->sol2, B * 4 * N));
+        PQP_CUDA(err, r.alloc(h->cost1, B));
+        PQP_CUDA(err, r.alloc(h->cost2, B));
+        PQP_CUDA(err, r.alloc(h->status1, B));
+        PQP_CUDA(err, r.alloc(h->iters1, B));
+        PQP_CUDA(err, r.alloc(h->status2, B));
+        PQP_CUDA(err, r.alloc(h->iters2, B));
+        for (int i = 0; i < 6; ++i) PQP_CUDA(err, r.alloc(h->full[i], B * (i % 3 == 0 ? 6 * N - 1 : 6 * N + 2)));
+        if (h->prm.smoothing_method == PQP_PLAN_SMOOTH_TENSION) PQP_CUDA(err, r.alloc(h->t_clear, B * P));
+        PQP_CUDA(err, r.alloc(h->pt_x, B * R));
+        PQP_CUDA(err, r.alloc(h->pt_y, B * R));
+        PQP_CUDA(err, r.alloc(h->pt_m, B));
+        PQP_CUDA(err, r.alloc(h->bs_t, B * R));
+        PQP_CUDA(err, r.alloc(h->raw_r, B));
+        PQP_CUDA(err, r.alloc(h->bs_deg, B));
+        // spline rows are zero beyond each path's k, so every row read past the end of a fit is defined
+        PQP_CUDA(err, cudaMemset(h->raw_rows, 0, B * S * R * sizeof(double)));
+        PQP_CUDA(err, cudaMemset(h->t_rows, 0, B * S * P * sizeof(double)));
+        PQP_CUDA(err, cudaMemset(h->r_rows, 0, B * S * L * sizeof(double)));
+        PQP_CUDA(err, cudaMemset(h->knots, 0, B * PQP_NFIELDS * N * sizeof(double)));
+        PQP_CUDA(err, cudaMemset(h->ref_xyh, 0, B * 3 * N * sizeof(double)));
+        PQP_CUDA(err, cudaDeviceSynchronize());
+        return PQP_OK;
+    }();
+    if (rc != PQP_OK) {
+        const std::string msg = err;
         pqp_plan_destroy(h);
-        g_plan_create_error = msg;
-        return PQP_E_CUDA;
+        err = msg;
+        return rc;
     }
     *out = h;
     return PQP_OK;
@@ -839,23 +811,8 @@ int pqp_plan_create(const pqp_bounds_map *map, const pqp_plan_params *params, in
 
 void pqp_plan_destroy(pqp_plan_handle *h) {
     if (!h) return;
-    {
-        pqp::DeviceGuard guard_(h->device);
-        if (h->stream) cudaStreamSynchronize(h->stream);
-        void *bufs[] = {h->in_x, h->in_y, h->in_start, h->in_target, h->in_r, h->o_status, h->o_n, h->o_iters, h->o_path,
-                        h->o_cost, h->status, h->raw_k, h->seg_p, h->t_status, h->t_iters, h->tk, h->start3, h->raw_rows,
-                        h->seg[0], h->seg[1], h->seg[2], h->seg[3], h->seg[4], h->t_x, h->t_y, h->t_s, h->t_rows, h->t_len,
-                        h->dp_status, h->dp_nl, h->dp_nout, h->dp_chosen, h->dp_ls, h->dp_lo, h->dp_up, h->dp_vl, h->dp_ts,
-                        h->post_p, h->post_status, h->post_iters, h->rk, h->post_off, h->r_rows, h->r_len, h->max_s,
-                        h->states, h->curv, h->bnd, h->knots, h->knots2, h->inst, h->ref_xyh, h->xyh, h->n_states,
-                        h->total, h->n_valid, h->n1, h->n2, h->p, h->sol1, h->sol2, h->cost1, h->cost2, h->status1,
-                        h->iters1, h->status2, h->iters2, h->full[0], h->full[1], h->full[2], h->full[3], h->full[4],
-                        h->full[5], h->t_clear, h->pt_x, h->pt_y, h->pt_m, h->bs_t, h->raw_r, h->bs_deg};
-        for (void *p : bufs) cudaFree(p);
-        for (cudaEvent_t ev : h->ev)
-            if (ev) cudaEventDestroy(ev);
-        if (h->stream) cudaStreamDestroy(h->stream);
-    }
+    pqp::DeviceGuard guard_(h->device);
+    if (h->stream) cudaStreamSynchronize(h->stream);
     if (h->solver) pqp_destroy(h->solver);
     if (h->post) pqp_smoother_destroy(h->post);
     if (h->tension) pqp_smoother_destroy(h->tension);
@@ -877,11 +834,11 @@ int pqp_plan(pqp_plan_handle *h, const pqp_plan_in *in, const pqp_plan_out *out)
     pqp::DeviceGuard guard_(h->device);
     cudaStream_t s = h->stream;
     const size_t B = in->batch, R = in->r_max;
-    PQL_CUDA(h, cudaMemcpyAsync(h->in_x, in->raw_x, B * R * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQL_CUDA(h, cudaMemcpyAsync(h->in_y, in->raw_y, B * R * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQL_CUDA(h, cudaMemcpyAsync(h->in_r, in->r, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    PQL_CUDA(h, cudaMemcpyAsync(h->in_start, in->start, B * 4 * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQL_CUDA(h, cudaMemcpyAsync(h->in_target, in->target, B * 3 * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_x, in->raw_x, B * R * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_y, in->raw_y, B * R * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_r, in->r, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_start, in->start, B * 4 * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_target, in->target, B * 3 * sizeof(double), cudaMemcpyHostToDevice, s));
     const pqp_plan_in din = {in->batch, in->r_max, h->in_x, h->in_y, h->in_r, h->in_start, h->in_target};
     const pqp_plan_out dout = {h->o_status, h->o_n, h->o_path, h->o_cost, h->o_iters, out->trace};
     rc = run(h, &din, &dout, s);
@@ -902,11 +859,11 @@ int pqp_plan_points(pqp_plan_handle *h, const pqp_plan_points_in *in, const pqp_
     pqp::DeviceGuard guard_(h->device);
     cudaStream_t s = h->stream;
     const size_t B = in->batch, M = in->m_max;
-    PQL_CUDA(h, cudaMemcpyAsync(h->pt_x, in->ref_x, B * M * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQL_CUDA(h, cudaMemcpyAsync(h->pt_y, in->ref_y, B * M * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQL_CUDA(h, cudaMemcpyAsync(h->pt_m, in->m, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    PQL_CUDA(h, cudaMemcpyAsync(h->in_start, in->start, B * 4 * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQL_CUDA(h, cudaMemcpyAsync(h->in_target, in->target, B * 3 * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->pt_x, in->ref_x, B * M * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->pt_y, in->ref_y, B * M * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->pt_m, in->m, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_start, in->start, B * 4 * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_target, in->target, B * 3 * sizeof(double), cudaMemcpyHostToDevice, s));
     const pqp_plan_points_in din = {in->batch, in->m_max, h->pt_x, h->pt_y, h->pt_m, h->in_start, h->in_target};
     const pqp_plan_out dout = {h->o_status, h->o_n, h->o_path, h->o_cost, h->o_iters, out->trace};
     rc = run_points(h, &din, &dout, s);
@@ -924,7 +881,7 @@ int pqp_plan_set_map(pqp_plan_handle *h, const pqp_bounds_map *map) {
     if (!h) return PQP_E_INVALID;
     PQL_SUB(h, pqp_plan_set_map_device(h, map, h->stream), pqp_plan_last_error, h);
     pqp::DeviceGuard guard_(h->device);
-    PQL_CUDA(h, cudaStreamSynchronize(h->stream));
+    PQP_CUDA(h->err, cudaStreamSynchronize(h->stream));
     return PQP_OK;
 }
 
@@ -950,13 +907,13 @@ int pqp_plan_get_map(pqp_plan_handle *h, pqp_bounds_map *meta, float *distance) 
 
 int pqp_plan_last_stage_ms(pqp_plan_handle *h, float *ms) {
     if (!h || !ms) return PQP_E_INVALID;
-    if (!h->timed) return pfail(h, PQP_E_STATE, "no plan has run yet");
+    if (!h->timed) return fail(h->err, PQP_E_STATE, "no plan has run yet");
     pqp::DeviceGuard guard_(h->device);
-    PQL_CUDA(h, cudaEventSynchronize(h->ev[3]));
-    PQL_CUDA(h, cudaEventElapsedTime(&ms[PQP_PLAN_STAGE_SMOOTHING], h->ev[0], h->ev[1]));
-    PQL_CUDA(h, cudaEventElapsedTime(&ms[PQP_PLAN_STAGE_SEGMENTATION], h->ev[1], h->ev[2]));
-    PQL_CUDA(h, cudaEventElapsedTime(&ms[PQP_PLAN_STAGE_OPTIMISATION], h->ev[2], h->ev[3]));
-    PQL_CUDA(h, cudaEventElapsedTime(&ms[PQP_PLAN_STAGE_TOTAL], h->ev[0], h->ev[3]));
+    PQP_CUDA(h->err, cudaEventSynchronize(h->ev[3]));
+    PQP_CUDA(h->err, cudaEventElapsedTime(&ms[PQP_PLAN_STAGE_SMOOTHING], h->ev[0], h->ev[1]));
+    PQP_CUDA(h->err, cudaEventElapsedTime(&ms[PQP_PLAN_STAGE_SEGMENTATION], h->ev[1], h->ev[2]));
+    PQP_CUDA(h->err, cudaEventElapsedTime(&ms[PQP_PLAN_STAGE_OPTIMISATION], h->ev[2], h->ev[3]));
+    PQP_CUDA(h->err, cudaEventElapsedTime(&ms[PQP_PLAN_STAGE_TOTAL], h->ev[0], h->ev[3]));
     return PQP_OK;
 }
 
@@ -964,7 +921,7 @@ int pqp_plan_launch_count(pqp_plan_handle *h, int64_t *count) {
     if (!h || !count) return PQP_E_INVALID;
     int64_t solver = 0;
     const int rc = pqp_launch_count(h->solver, &solver);
-    if (rc != PQP_OK) return pfail(h, rc, pqp_last_error(h->solver));
+    if (rc != PQP_OK) return fail(h->err, rc, pqp_last_error(h->solver));
     *count = h->launches + solver;
     return PQP_OK;
 }

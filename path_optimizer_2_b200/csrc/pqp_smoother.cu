@@ -9,7 +9,7 @@
 #include <string>
 
 #include "../../include/pqp_smoother.h"
-#include "pqp_device_guard.h"
+#include "pqp_host_handle.h"
 #include "pqp_smoother_core.cuh"
 #include "pqp_smoother_internal.h"
 
@@ -136,24 +136,12 @@ struct pqp_smoother_handle {
     int32_t *d_p = nullptr, *d_status = nullptr, *d_iters = nullptr;
     float last_ms = 0.0f;
     std::string err;
+    pqp::Resources res;  // last member: releasing clears the members above
 };
 
 namespace {
 
-#define PQS_CUDA(h, call)                                                      \
-    do {                                                                       \
-        cudaError_t e_ = (call);                                               \
-        if (e_ != cudaSuccess) {                                               \
-            (h)->err = std::string(#call) + ": " + cudaGetErrorString(e_);     \
-            return PQP_E_CUDA;                                                 \
-        }                                                                      \
-    } while (0)
-
-int sfail(pqp_smoother_handle *h, int code, const char *msg) {
-    if (h) h->err = msg;
-    else g_smoother_create_error = msg;
-    return code;
-}
+using pqp::fail;
 
 pqs::Settings settings_of(const pqp_smoother_params &p) {
     pqs::Settings s;
@@ -162,6 +150,17 @@ pqs::Settings settings_of(const pqp_smoother_params &p) {
     s.max_iter = p.max_iter; s.check_termination = p.check_termination; s.scaling = p.scaling;
     s.adaptive_rho = p.adaptive_rho; s.adaptive_rho_interval = p.adaptive_rho_interval;
     return s;
+}
+
+// resident one-warp CTAs of `kernel` at `smem` bytes of band: 1 to 16 per SM, at most batch_max in all
+template <typename Kernel>
+cudaError_t resident_grid(Kernel *kernel, size_t smem, int sm_count, int batch_max, int *grid) {
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    int per_sm = 1;
+    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, 32, smem);
+    per_sm = per_sm < 1 ? 1 : (per_sm > 16 ? 16 : per_sm);
+    *grid = sm_count * per_sm < batch_max ? sm_count * per_sm : batch_max;
+    return e;
 }
 
 int launch(pqp_smoother_handle *h, KArgs &a, cudaStream_t s) {
@@ -174,11 +173,11 @@ int launch(pqp_smoother_handle *h, KArgs &a, cudaStream_t s) {
     const int grid = a.batch < h->grid_max ? a.batch : h->grid_max;
     // the dynamic shared-memory limit is an attribute of the kernel, not of the handle: a handle created later with a
     // smaller p_max lowers it, so each launch sets this handle's own
-    PQS_CUDA(h, cudaFuncSetAttribute(smoother_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem));
-    PQS_CUDA(h, cudaEventRecord(h->ev0, s));
+    PQP_CUDA(h->err, cudaFuncSetAttribute(smoother_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem));
+    PQP_CUDA(h->err, cudaEventRecord(h->ev0, s));
     smoother_kernel<<<grid, 32, h->smem, s>>>(a);
-    PQS_CUDA(h, cudaGetLastError());
-    PQS_CUDA(h, cudaEventRecord(h->ev1, s));
+    PQP_CUDA(h->err, cudaGetLastError());
+    PQP_CUDA(h->err, cudaEventRecord(h->ev1, s));
     return PQP_OK;
 }
 
@@ -189,27 +188,80 @@ int launch_cartesian(pqp_smoother_handle *h, CArgs &a, cudaStream_t s) {
     a.scratch = h->d_scratch;
     a.scratch_stride = h->cart_stride;
     const int grid = a.batch < h->cart_grid_max ? a.batch : h->cart_grid_max;
-    PQS_CUDA(h, cudaFuncSetAttribute(cartesian_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->cart_smem));
-    PQS_CUDA(h, cudaEventRecord(h->ev0, s));
+    PQP_CUDA(h->err, cudaFuncSetAttribute(cartesian_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->cart_smem));
+    PQP_CUDA(h->err, cudaEventRecord(h->ev0, s));
     cartesian_kernel<<<grid, 32, h->cart_smem, s>>>(a);
-    PQS_CUDA(h, cudaGetLastError());
-    PQS_CUDA(h, cudaEventRecord(h->ev1, s));
+    PQP_CUDA(h->err, cudaGetLastError());
+    PQP_CUDA(h->err, cudaEventRecord(h->ev1, s));
     return PQP_OK;
 }
 
-int check_cartesian(pqp_smoother_handle *h, const pqp_cartesian_tension_in *in, const pqp_tension_out *out) {
+// the argument checks of each call, shared by its host-pointer and device-pointer forms
+int check_size(pqp_smoother_handle *h, int batch, int p_max) {
+    if (batch < 1 || batch > h->batch_max || p_max != h->p_max) return fail(h->err, PQP_E_INVALID, "batch / p_max do not fit the handle");
+    return PQP_OK;
+}
+int check(pqp_smoother_handle *h, const pqp_tension_in *in, const pqp_tension_out *out) {
     if (!h) return PQP_E_INVALID;
-    if (!h->cart_err.empty()) return sfail(h, PQP_E_INVALID, h->cart_err.c_str());
+    if (!in || !out || !in->p || !in->x || !in->y || !in->angle || !in->k || !in->s || !out->x || !out->y || !out->s ||
+        !out->status || !out->iters)
+        return fail(h->err, PQP_E_INVALID, "null buffer");
+    return check_size(h, in->batch, in->p_max);
+}
+int check(pqp_smoother_handle *h, const pqp_post_in *in, const pqp_post_out *out) {
+    if (!h) return PQP_E_INVALID;
+    if (!in || !out || !in->p || !in->layer_s || !in->lower || !in->upper || !in->vehicle_l || !out->offsets || !out->status || !out->iters)
+        return fail(h->err, PQP_E_INVALID, "null buffer");
+    return check_size(h, in->batch, in->p_max);
+}
+int check(pqp_smoother_handle *h, const pqp_cartesian_tension_in *in, const pqp_tension_out *out) {
+    if (!h) return PQP_E_INVALID;
+    if (!h->cart_err.empty()) return fail(h->err, PQP_E_INVALID, h->cart_err);
     if (!in || !out || !in->p || !in->x || !in->y || !in->angle || !in->clearance || !out->x || !out->y || !out->s ||
         !out->status || !out->iters)
-        return sfail(h, PQP_E_INVALID, "null buffer");
-    if (in->batch < 1 || in->batch > h->batch_max || in->p_max != h->p_max) return sfail(h, PQP_E_INVALID, "batch / p_max do not fit the handle");
-    return PQP_OK;
+        return fail(h->err, PQP_E_INVALID, "null buffer");
+    return check_size(h, in->batch, in->p_max);
 }
 
-template <typename T>
-cudaError_t dalloc(T **p, size_t n) {
-    return cudaMalloc(reinterpret_cast<void **>(p), (n ? n : 1) * sizeof(T));
+// A host-pointer call: its input lists (and post's vehicle_l) and p are staged into d_in / d_vl / d_p, its outputs
+// cleared, the device form `run` is launched on the handle's stream with the staging buffers, and the outputs are
+// copied back. `p_min` is the smallest p[b] the call accepts; `full_rows` the rows of one QP's x_full.
+struct HostCall {
+    int batch;
+    const int32_t *p;
+    int p_min;
+    const double *const *in;
+    int n_in;
+    const double *vehicle_l;
+    double *const *out;
+    int n_out;
+    int32_t *status, *iters;
+    double *x_full;
+    int full_rows;
+};
+
+template <typename Run>
+int run_host(pqp_smoother_handle *h, const HostCall &c, Run run) {
+    for (int b = 0; b < c.batch; ++b)
+        if (c.p[b] < c.p_min || c.p[b] > h->p_max)
+            return fail(h->err, PQP_E_INVALID, c.p_min == 2 ? "p[b] must be in [2, p_max]" : "p[b] must be in [3, p_max]");
+    pqp::DeviceGuard guard_(h->device);
+    cudaStream_t s = h->stream;
+    const size_t B = c.batch, Ls = B * h->p_max, nf = Ls * c.full_rows;
+    for (int i = 0; i < c.n_in; ++i) PQP_CUDA(h->err, cudaMemcpyAsync(h->d_in[i], c.in[i], Ls * sizeof(double), cudaMemcpyHostToDevice, s));
+    if (c.vehicle_l) PQP_CUDA(h->err, cudaMemcpyAsync(h->d_vl, c.vehicle_l, B * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_p, c.p, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    for (int i = 0; i < c.n_out; ++i) PQP_CUDA(h->err, cudaMemsetAsync(h->d_out[i], 0, Ls * sizeof(double), s));
+    if (c.x_full) PQP_CUDA(h->err, cudaMemsetAsync(h->d_xfull, 0, nf * sizeof(double), s));
+    const int rc = run(s, c.x_full ? h->d_xfull : nullptr);
+    if (rc != PQP_OK) return rc;
+    for (int i = 0; i < c.n_out; ++i) PQP_CUDA(h->err, cudaMemcpyAsync(c.out[i], h->d_out[i], Ls * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(c.status, h->d_status, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(c.iters, h->d_iters, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    if (c.x_full) PQP_CUDA(h->err, cudaMemcpyAsync(c.x_full, h->d_xfull, nf * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaStreamSynchronize(s));
+    PQP_CUDA(h->err, cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1));
+    return PQP_OK;
 }
 
 }  // namespace
@@ -251,78 +303,67 @@ const char *pqp_smoother_last_error(const pqp_smoother_handle *h) { return h ? h
 
 int pqp_smoother_create(const pqp_smoother_params *params, int32_t p_max, int32_t batch_max, int32_t device,
                         pqp_smoother_handle **out) {
+    std::string &err = g_smoother_create_error;
     if (!out) return PQP_E_INVALID;
     *out = nullptr;
-    if (p_max < 4 || p_max > 2000 || batch_max < 1) return sfail(nullptr, PQP_E_INVALID, "pqp_smoother_create: 4 <= p_max <= 2000, batch_max >= 1");
+    if (p_max < 4 || p_max > 2000 || batch_max < 1) return fail(err, PQP_E_INVALID, "pqp_smoother_create: 4 <= p_max <= 2000, batch_max >= 1");
     int count = 0;
     if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0 || device < 0 || device >= count)
-        return sfail(nullptr, PQP_E_NO_DEVICE, "pqp_smoother_create: no CUDA device (there is no CPU fallback)");
+        return fail(err, PQP_E_NO_DEVICE, "pqp_smoother_create: no CUDA device (there is no CPU fallback)");
+    pqp_smoother_params prm;
+    if (params) prm = *params;
+    else pqp_smoother_default_params(&prm);
+    if (!(prm.rho > 0) || !(prm.sigma > 0) || !(prm.alpha > 0 && prm.alpha < 2) || prm.max_iter < 1)
+        return fail(err, PQP_E_INVALID, "pqp_smoother_create: invalid OSQP settings");
+    cudaDeviceProp prop;
+    PQP_CUDA(err, cudaGetDeviceProperties(&prop, device));
+    const size_t smem_limit = prop.sharedMemPerBlockOptin;
+    if (pqs::band_doubles(p_max) * sizeof(double) > smem_limit)
+        return fail(err, PQP_E_INVALID, "pqp_smoother_create: p_max too large for the shared-memory band");
     pqp_smoother_handle *h = new (std::nothrow) pqp_smoother_handle;
-    if (!h) return sfail(nullptr, PQP_E_INVALID, "out of host memory");
-    if (params) h->prm = *params;
-    else pqp_smoother_default_params(&h->prm);
-    if (!(h->prm.rho > 0) || !(h->prm.sigma > 0) || !(h->prm.alpha > 0 && h->prm.alpha < 2) || h->prm.max_iter < 1) {
-        delete h;
-        return sfail(nullptr, PQP_E_INVALID, "pqp_smoother_create: invalid OSQP settings");
-    }
-    h->device = device;
+    if (!h) return fail(err, PQP_E_INVALID, "out of host memory");
+    h->prm = prm;
+    h->device = h->res.device = device;
     h->p_max = p_max;
     h->batch_max = batch_max;
     h->scratch_stride = pqs::scratch_bytes(p_max);
     h->smem = pqs::band_doubles(p_max) * sizeof(double);
-    pqp::DeviceGuard guard_(device);
-    cudaDeviceProp prop;
-    cudaError_t e = cudaGetDeviceProperties(&prop, device);
-    if (e == cudaSuccess && h->smem > (size_t)prop.sharedMemPerBlockOptin) {
-        delete h;
-        return sfail(nullptr, PQP_E_INVALID, "pqp_smoother_create: p_max too large for the shared-memory band");
-    }
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(smoother_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem);
-    int per_sm = 1;
-    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, smoother_kernel, 32, h->smem);
-    if (per_sm < 1) per_sm = 1;
-    if (per_sm > 16) per_sm = 16;
-    h->grid_max = prop.multiProcessorCount * per_sm;
-    if (h->grid_max > batch_max) h->grid_max = batch_max;
     // the Cartesian QP's band is wider: beyond its limit only the Cartesian calls are refused
     h->cart_stride = pqs::cartesian_scratch_bytes(p_max);
     h->cart_smem = pqs::cartesian_band_doubles(p_max) * sizeof(double);
-    if (e == cudaSuccess && h->cart_smem > (size_t)prop.sharedMemPerBlockOptin) {
+    if (h->cart_smem > smem_limit)
         h->cart_err = "pqp_cartesian_tension_smooth: p_max = " + std::to_string(p_max) +
                       " too large for the Cartesian QP's shared-memory band ((3 p_max + 9) * 11 doubles = " +
-                      std::to_string(h->cart_smem) + " bytes, the device allows " +
-                      std::to_string((size_t)prop.sharedMemPerBlockOptin) + " per block)";
-    } else if (e == cudaSuccess) {
-        e = cudaFuncSetAttribute(cartesian_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->cart_smem);
-        int cart_per_sm = 1;
-        if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cart_per_sm, cartesian_kernel, 32, h->cart_smem);
-        if (cart_per_sm < 1) cart_per_sm = 1;
-        if (cart_per_sm > 16) cart_per_sm = 16;
-        h->cart_grid_max = prop.multiProcessorCount * cart_per_sm;
-        if (h->cart_grid_max > batch_max) h->cart_grid_max = batch_max;
-    }
-    // one scratch block serves both working-set shapes: the Cartesian grid is capped by how many of its (larger)
-    // working sets fit, and the block holds at least one
-    h->scratch_total = (size_t)h->grid_max * h->scratch_stride;
-    if (h->cart_err.empty() && h->scratch_total < h->cart_stride) h->scratch_total = h->cart_stride;
-    if (h->cart_err.empty() && (size_t)h->cart_grid_max > h->scratch_total / h->cart_stride)
-        h->cart_grid_max = (int)(h->scratch_total / h->cart_stride);
-    const size_t B = batch_max, Ls = B * p_max;
-    if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void **>(&h->d_scratch), h->scratch_total);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaEventCreate(&h->ev0);
-    if (e == cudaSuccess) e = cudaEventCreate(&h->ev1);
-    for (int i = 0; i < 5 && e == cudaSuccess; ++i) e = dalloc(&h->d_in[i], Ls);
-    for (int i = 0; i < 3 && e == cudaSuccess; ++i) e = dalloc(&h->d_out[i], Ls);
-    if (e == cudaSuccess) e = dalloc(&h->d_xfull, Ls * 4);
-    if (e == cudaSuccess) e = dalloc(&h->d_vl, B);
-    if (e == cudaSuccess) e = dalloc(&h->d_p, B);
-    if (e == cudaSuccess) e = dalloc(&h->d_status, B);
-    if (e == cudaSuccess) e = dalloc(&h->d_iters, B);
-    if (e != cudaSuccess) {
-        g_smoother_create_error = std::string("pqp_smoother_create: ") + cudaGetErrorString(e);
+                      std::to_string(h->cart_smem) + " bytes, the device allows " + std::to_string(smem_limit) + " per block)";
+    pqp::DeviceGuard guard_(device);
+    const int rc = [&]() -> int {
+        PQP_CUDA(err, resident_grid(smoother_kernel, h->smem, prop.multiProcessorCount, batch_max, &h->grid_max));
+        if (h->cart_err.empty())
+            PQP_CUDA(err, resident_grid(cartesian_kernel, h->cart_smem, prop.multiProcessorCount, batch_max, &h->cart_grid_max));
+        // one scratch block serves both working-set shapes: the Cartesian grid is capped by how many of its (larger)
+        // working sets fit, and the block holds at least one
+        h->scratch_total = (size_t)h->grid_max * h->scratch_stride;
+        if (h->cart_err.empty() && h->scratch_total < h->cart_stride) h->scratch_total = h->cart_stride;
+        if (h->cart_err.empty() && (size_t)h->cart_grid_max > h->scratch_total / h->cart_stride)
+            h->cart_grid_max = (int)(h->scratch_total / h->cart_stride);
+        pqp::Resources &r = h->res;
+        const size_t B = batch_max, Ls = B * p_max;
+        PQP_CUDA(err, r.alloc(h->d_scratch, h->scratch_total));
+        PQP_CUDA(err, r.stream(h->stream));
+        PQP_CUDA(err, r.event(h->ev0));
+        PQP_CUDA(err, r.event(h->ev1));
+        for (int i = 0; i < 5; ++i) PQP_CUDA(err, r.alloc(h->d_in[i], Ls));
+        for (int i = 0; i < 3; ++i) PQP_CUDA(err, r.alloc(h->d_out[i], Ls));
+        PQP_CUDA(err, r.alloc(h->d_xfull, Ls * 4));
+        PQP_CUDA(err, r.alloc(h->d_vl, B));
+        PQP_CUDA(err, r.alloc(h->d_p, B));
+        PQP_CUDA(err, r.alloc(h->d_status, B));
+        PQP_CUDA(err, r.alloc(h->d_iters, B));
+        return PQP_OK;
+    }();
+    if (rc != PQP_OK) {
         pqp_smoother_destroy(h);
-        return PQP_E_CUDA;
+        return rc;
     }
     *out = h;
     return PQP_OK;
@@ -332,22 +373,12 @@ void pqp_smoother_destroy(pqp_smoother_handle *h) {
     if (!h) return;
     pqp::DeviceGuard guard_(h->device);
     if (h->stream) cudaStreamSynchronize(h->stream);
-    cudaFree(h->d_scratch);
-    for (int i = 0; i < 5; ++i) cudaFree(h->d_in[i]);
-    for (int i = 0; i < 3; ++i) cudaFree(h->d_out[i]);
-    cudaFree(h->d_xfull); cudaFree(h->d_vl); cudaFree(h->d_p); cudaFree(h->d_status); cudaFree(h->d_iters);
-    if (h->ev0) cudaEventDestroy(h->ev0);
-    if (h->ev1) cudaEventDestroy(h->ev1);
-    if (h->stream) cudaStreamDestroy(h->stream);
     delete h;
 }
 
 int pqp_tension_smooth_device(pqp_smoother_handle *h, const pqp_tension_in *in, const pqp_tension_out *out, void *stream) {
-    if (!h) return PQP_E_INVALID;
-    if (!in || !out || !in->p || !in->x || !in->y || !in->angle || !in->k || !in->s || !out->x || !out->y || !out->s ||
-        !out->status || !out->iters)
-        return sfail(h, PQP_E_INVALID, "null buffer");
-    if (in->batch < 1 || in->batch > h->batch_max || in->p_max != h->p_max) return sfail(h, PQP_E_INVALID, "batch / p_max do not fit the handle");
+    const int rc = check(h, in, out);
+    if (rc != PQP_OK) return rc;
     pqp::DeviceGuard guard_(h->device);
     KArgs a{};
     a.batch = in->batch;
@@ -362,10 +393,8 @@ int pqp_tension_smooth_device(pqp_smoother_handle *h, const pqp_tension_in *in, 
 }
 
 int pqp_post_smooth_device(pqp_smoother_handle *h, const pqp_post_in *in, const pqp_post_out *out, void *stream) {
-    if (!h) return PQP_E_INVALID;
-    if (!in || !out || !in->p || !in->layer_s || !in->lower || !in->upper || !in->vehicle_l || !out->offsets || !out->status || !out->iters)
-        return sfail(h, PQP_E_INVALID, "null buffer");
-    if (in->batch < 1 || in->batch > h->batch_max || in->p_max != h->p_max) return sfail(h, PQP_E_INVALID, "batch / p_max do not fit the handle");
+    const int rc = check(h, in, out);
+    if (rc != PQP_OK) return rc;
     pqp::DeviceGuard guard_(h->device);
     KArgs a{};
     a.batch = in->batch;
@@ -381,7 +410,7 @@ int pqp_post_smooth_device(pqp_smoother_handle *h, const pqp_post_in *in, const 
 
 int pqp_cartesian_tension_smooth_device(pqp_smoother_handle *h, const pqp_cartesian_tension_in *in,
                                         const pqp_tension_out *out, void *stream) {
-    const int rc = check_cartesian(h, in, out);
+    const int rc = check(h, in, out);
     if (rc != PQP_OK) return rc;
     pqp::DeviceGuard guard_(h->device);
     CArgs a{};
@@ -396,89 +425,42 @@ int pqp_cartesian_tension_smooth_device(pqp_smoother_handle *h, const pqp_cartes
 }
 
 int pqp_cartesian_tension_smooth(pqp_smoother_handle *h, const pqp_cartesian_tension_in *in, const pqp_tension_out *out) {
-    int rc = check_cartesian(h, in, out);
+    const int rc = check(h, in, out);
     if (rc != PQP_OK) return rc;
-    for (int b = 0; b < in->batch; ++b)
-        if (in->p[b] < 3 || in->p[b] > in->p_max) return sfail(h, PQP_E_INVALID, "p[b] must be in [3, p_max]");
-    pqp::DeviceGuard guard_(h->device);
-    cudaStream_t s = h->stream;
-    const size_t B = in->batch, Ls = B * h->p_max;
-    const double *src[4] = {in->x, in->y, in->angle, in->clearance};
-    for (int i = 0; i < 4; ++i) PQS_CUDA(h, cudaMemcpyAsync(h->d_in[i], src[i], Ls * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQS_CUDA(h, cudaMemcpyAsync(h->d_p, in->p, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    for (int i = 0; i < 3; ++i) PQS_CUDA(h, cudaMemsetAsync(h->d_out[i], 0, Ls * sizeof(double), s));
-    if (out->x_full) PQS_CUDA(h, cudaMemsetAsync(h->d_xfull, 0, Ls * 3 * sizeof(double), s));
-    pqp_cartesian_tension_in din = {in->batch, in->p_max, h->d_p, h->d_in[0], h->d_in[1], h->d_in[2], h->d_in[3]};
-    pqp_tension_out dout = {h->d_out[0], h->d_out[1], h->d_out[2], h->d_status, h->d_iters, out->x_full ? h->d_xfull : nullptr};
-    rc = pqp_cartesian_tension_smooth_device(h, &din, &dout, s);
-    if (rc != PQP_OK) return rc;
-    double *dst[3] = {out->x, out->y, out->s};
-    for (int i = 0; i < 3; ++i) PQS_CUDA(h, cudaMemcpyAsync(dst[i], h->d_out[i], Ls * sizeof(double), cudaMemcpyDeviceToHost, s));
-    PQS_CUDA(h, cudaMemcpyAsync(out->status, h->d_status, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    PQS_CUDA(h, cudaMemcpyAsync(out->iters, h->d_iters, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    if (out->x_full) PQS_CUDA(h, cudaMemcpyAsync(out->x_full, h->d_xfull, Ls * 3 * sizeof(double), cudaMemcpyDeviceToHost, s));
-    PQS_CUDA(h, cudaStreamSynchronize(s));
-    PQS_CUDA(h, cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1));
-    return PQP_OK;
+    const double *src[] = {in->x, in->y, in->angle, in->clearance};
+    double *dst[] = {out->x, out->y, out->s};
+    return run_host(h, {in->batch, in->p, 3, src, 4, nullptr, dst, 3, out->status, out->iters, out->x_full, 3},
+                    [&](cudaStream_t s, double *x_full) {
+                        const pqp_cartesian_tension_in din = {in->batch, in->p_max, h->d_p, h->d_in[0], h->d_in[1], h->d_in[2], h->d_in[3]};
+                        const pqp_tension_out dout = {h->d_out[0], h->d_out[1], h->d_out[2], h->d_status, h->d_iters, x_full};
+                        return pqp_cartesian_tension_smooth_device(h, &din, &dout, s);
+                    });
 }
 
 int pqp_tension_smooth(pqp_smoother_handle *h, const pqp_tension_in *in, const pqp_tension_out *out) {
-    if (!h) return PQP_E_INVALID;
-    if (!in || !out || !in->p || !in->x || !in->y || !in->angle || !in->k || !in->s || !out->x || !out->y || !out->s ||
-        !out->status || !out->iters)
-        return sfail(h, PQP_E_INVALID, "null buffer");
-    if (in->batch < 1 || in->batch > h->batch_max || in->p_max != h->p_max) return sfail(h, PQP_E_INVALID, "batch / p_max do not fit the handle");
-    for (int b = 0; b < in->batch; ++b)
-        if (in->p[b] < 3 || in->p[b] > in->p_max) return sfail(h, PQP_E_INVALID, "p[b] must be in [3, p_max]");
-    pqp::DeviceGuard guard_(h->device);
-    cudaStream_t s = h->stream;
-    const size_t B = in->batch, Ls = B * h->p_max;
-    const double *src[5] = {in->x, in->y, in->angle, in->k, in->s};
-    for (int i = 0; i < 5; ++i) PQS_CUDA(h, cudaMemcpyAsync(h->d_in[i], src[i], Ls * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQS_CUDA(h, cudaMemcpyAsync(h->d_p, in->p, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    for (int i = 0; i < 3; ++i) PQS_CUDA(h, cudaMemsetAsync(h->d_out[i], 0, Ls * sizeof(double), s));
-    if (out->x_full) PQS_CUDA(h, cudaMemsetAsync(h->d_xfull, 0, Ls * 4 * sizeof(double), s));
-    pqp_tension_in din = {in->batch, in->p_max, h->d_p, h->d_in[0], h->d_in[1], h->d_in[2], h->d_in[3], h->d_in[4]};
-    pqp_tension_out dout = {h->d_out[0], h->d_out[1], h->d_out[2], h->d_status, h->d_iters, out->x_full ? h->d_xfull : nullptr};
-    int rc = pqp_tension_smooth_device(h, &din, &dout, s);
+    const int rc = check(h, in, out);
     if (rc != PQP_OK) return rc;
-    double *dst[3] = {out->x, out->y, out->s};
-    for (int i = 0; i < 3; ++i) PQS_CUDA(h, cudaMemcpyAsync(dst[i], h->d_out[i], Ls * sizeof(double), cudaMemcpyDeviceToHost, s));
-    PQS_CUDA(h, cudaMemcpyAsync(out->status, h->d_status, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    PQS_CUDA(h, cudaMemcpyAsync(out->iters, h->d_iters, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    if (out->x_full) PQS_CUDA(h, cudaMemcpyAsync(out->x_full, h->d_xfull, Ls * 4 * sizeof(double), cudaMemcpyDeviceToHost, s));
-    PQS_CUDA(h, cudaStreamSynchronize(s));
-    PQS_CUDA(h, cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1));
-    return PQP_OK;
+    const double *src[] = {in->x, in->y, in->angle, in->k, in->s};
+    double *dst[] = {out->x, out->y, out->s};
+    return run_host(h, {in->batch, in->p, 3, src, 5, nullptr, dst, 3, out->status, out->iters, out->x_full, 4},
+                    [&](cudaStream_t s, double *x_full) {
+                        const pqp_tension_in din = {in->batch, in->p_max, h->d_p, h->d_in[0], h->d_in[1], h->d_in[2], h->d_in[3], h->d_in[4]};
+                        const pqp_tension_out dout = {h->d_out[0], h->d_out[1], h->d_out[2], h->d_status, h->d_iters, x_full};
+                        return pqp_tension_smooth_device(h, &din, &dout, s);
+                    });
 }
 
 int pqp_post_smooth(pqp_smoother_handle *h, const pqp_post_in *in, const pqp_post_out *out) {
-    if (!h) return PQP_E_INVALID;
-    if (!in || !out || !in->p || !in->layer_s || !in->lower || !in->upper || !in->vehicle_l || !out->offsets || !out->status || !out->iters)
-        return sfail(h, PQP_E_INVALID, "null buffer");
-    if (in->batch < 1 || in->batch > h->batch_max || in->p_max != h->p_max) return sfail(h, PQP_E_INVALID, "batch / p_max do not fit the handle");
-    for (int b = 0; b < in->batch; ++b)
-        if (in->p[b] < 2 || in->p[b] > in->p_max) return sfail(h, PQP_E_INVALID, "p[b] must be in [2, p_max]");
-    pqp::DeviceGuard guard_(h->device);
-    cudaStream_t s = h->stream;
-    const size_t B = in->batch, Ls = B * h->p_max;
-    const double *src[3] = {in->layer_s, in->lower, in->upper};
-    for (int i = 0; i < 3; ++i) PQS_CUDA(h, cudaMemcpyAsync(h->d_in[i], src[i], Ls * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQS_CUDA(h, cudaMemcpyAsync(h->d_vl, in->vehicle_l, B * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQS_CUDA(h, cudaMemcpyAsync(h->d_p, in->p, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    PQS_CUDA(h, cudaMemsetAsync(h->d_out[0], 0, Ls * sizeof(double), s));
-    if (out->x_full) PQS_CUDA(h, cudaMemsetAsync(h->d_xfull, 0, Ls * 3 * sizeof(double), s));
-    pqp_post_in din = {in->batch, in->p_max, h->d_p, h->d_in[0], h->d_in[1], h->d_in[2], h->d_vl};
-    pqp_post_out dout = {h->d_out[0], h->d_status, h->d_iters, out->x_full ? h->d_xfull : nullptr};
-    int rc = pqp_post_smooth_device(h, &din, &dout, s);
+    const int rc = check(h, in, out);
     if (rc != PQP_OK) return rc;
-    PQS_CUDA(h, cudaMemcpyAsync(out->offsets, h->d_out[0], Ls * sizeof(double), cudaMemcpyDeviceToHost, s));
-    PQS_CUDA(h, cudaMemcpyAsync(out->status, h->d_status, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    PQS_CUDA(h, cudaMemcpyAsync(out->iters, h->d_iters, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    if (out->x_full) PQS_CUDA(h, cudaMemcpyAsync(out->x_full, h->d_xfull, Ls * 3 * sizeof(double), cudaMemcpyDeviceToHost, s));
-    PQS_CUDA(h, cudaStreamSynchronize(s));
-    PQS_CUDA(h, cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1));
-    return PQP_OK;
+    const double *src[] = {in->layer_s, in->lower, in->upper};
+    double *dst[] = {out->offsets};
+    return run_host(h, {in->batch, in->p, 2, src, 3, in->vehicle_l, dst, 1, out->status, out->iters, out->x_full, 3},
+                    [&](cudaStream_t s, double *x_full) {
+                        const pqp_post_in din = {in->batch, in->p_max, h->d_p, h->d_in[0], h->d_in[1], h->d_in[2], h->d_vl};
+                        const pqp_post_out dout = {h->d_out[0], h->d_status, h->d_iters, x_full};
+                        return pqp_post_smooth_device(h, &din, &dout, s);
+                    });
 }
 
 int pqp_smoother_last_kernel_ms(pqp_smoother_handle *h, float *ms) {

@@ -35,7 +35,7 @@ def build_library(force=False, verbose=False):
     """nvcc-compile the CUDA library in-tree for sm_90a (no GPU needed to compile)."""
     root = os.path.dirname(_PKG)
     cu = [os.path.join(_CSRC, f) for f in ("pqp_api.cu", "pqp_bounds.cu", "pqp_multi.cu", "pqp_smoother.cu")]
-    deps = cu + [os.path.join(_CSRC, f) for f in ("pqp_kernel.cuh", "pqp_host_common.h", "pqp_bounds_core.cuh", "pqp_device_guard.h",
+    deps = cu + [os.path.join(_CSRC, f) for f in ("pqp_kernel.cuh", "pqp_host_common.h", "pqp_bounds_core.cuh", "pqp_host_handle.h",
                                                   "pqp_dp.cu", "pqp_dp_core.cuh", "pqp_bounds_internal.h", "pqp_smoother_core.cuh",
                                                   "pqp_plan.cu", "pqp_plan_core.cuh", "pqp_smoother_internal.h",
                                                   "pqp_map_core.cuh")]
