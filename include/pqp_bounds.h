@@ -1,6 +1,6 @@
 /* pqp_bounds.h — C ABI of the clearance-bounds front end (SURVEY.md §8 row f-1, "next").
  *
- * Replaces, for a batch of reference paths over ONE obstacle map:
+ * Replaces, for a batch of reference paths over one obstacle map (or one map per path, pqp_bounds_create_maps):
  *   ReferencePathImpl::updateBoundsImproved        src/data_struct/reference_path_impl.cpp:177-230
  *   ReferencePathImpl::getClearanceWithDirectionStrict                             ...:232-312
  *   getDirectionalProjectionByNewton               src/tools/tools.cpp:156-189
@@ -148,6 +148,54 @@ int pqp_bounds_set_map_device(pqp_bounds_handle *h, const pqp_bounds_map *map, v
 int pqp_bounds_set_occupancy(pqp_bounds_handle *h, const pqp_occupancy_map *occ);
 int pqp_bounds_set_occupancy_device(pqp_bounds_handle *h, const pqp_occupancy_map *occ, void *stream);
 int pqp_bounds_get_map(pqp_bounds_handle *h, pqp_bounds_map *meta, float *distance);
+
+/* Per-path maps: a handle holds n_maps map slots (1 <= n_maps <= PQP_MAX_MAP_SLOTS), each with the capacity of the
+ * largest of the maps it was created with; the *_mapped calls plan path b on slot map_index[b]. A handle made by
+ * pqp_bounds_create has one slot, and every call above acts on slot 0. Memory: 5 bytes per cell per slot (the float
+ * layer and the 1-byte occupancy staging), allocated at create; a failed allocation returns PQP_E_CUDA.
+ *
+ * The map-reading kernels index a device table of the slots' metadata. Slot updates write their entries with a
+ * kernel launch on the update's stream, so they keep the ordering of the calls above: work enqueued before an update
+ * sees the old slot, work enqueued after the new one, and no update waits for the host. Launches per update:
+ *   set_map_slot(_device), and pqp_bounds_set_map(_device):        1 (the table entry; the layer is a copy)
+ *   pqp_bounds_set_occupancy(_device):                             2 (the entry is written by the column pass)
+ *   set_occupancy_slots(_device):   2 + ceil(count / PQP_MAP_TABLE_CHUNK) (column pass, row pass, table entries)
+ *
+ * A slot update is refused (PQP_E_INVALID, every slot untouched) for a slot outside [0, n_maps) or anything
+ * pqp_bounds_set_map / pqp_bounds_set_occupancy refuse. */
+#define PQP_MAX_MAP_SLOTS 65535
+#define PQP_MAP_TABLE_CHUNK 1024 /* table entries one table-write launch carries in its parameters */
+
+/* count occupancy images of one size, [count][rows][cols] uint8 (host pointer for set_occupancy_slots, device
+ * pointer for set_occupancy_slots_device), each with its own centre; resolution and obstacle_max are shared. */
+typedef struct pqp_occupancy_stack {
+    int32_t count, rows, cols;
+    double resolution;
+    const double *center_x;   /* [count], host */
+    const double *center_y;   /* [count], host */
+    const uint8_t *cells;     /* [count][rows][cols] */
+    int32_t obstacle_max;
+} pqp_occupancy_stack;
+
+int pqp_bounds_create_maps(const pqp_bounds_map *maps, int32_t n_maps, const pqp_bounds_params *params,
+                           int32_t device, pqp_bounds_handle **out);
+int pqp_bounds_set_map_slot(pqp_bounds_handle *h, int32_t slot, const pqp_bounds_map *map);
+int pqp_bounds_set_map_slot_device(pqp_bounds_handle *h, int32_t slot, const pqp_bounds_map *map, void *stream);
+/* The images go into slots first_slot .. first_slot + count - 1: the exact distance transform of each, as
+ * pqp_bounds_set_occupancy computes it for one image. The column pass runs on grid (ceil(cols / 128), count), the row
+ * pass on grid (rows, count). The host call copies the stack into the slots' staging and returns when done. */
+int pqp_bounds_set_occupancy_slots(pqp_bounds_handle *h, int32_t first_slot, const pqp_occupancy_stack *stack);
+int pqp_bounds_set_occupancy_slots_device(pqp_bounds_handle *h, int32_t first_slot, const pqp_occupancy_stack *stack,
+                                          void *stream);
+/* As pqp_bounds_get_map for one slot. */
+int pqp_bounds_get_map_slot(pqp_bounds_handle *h, int32_t slot, pqp_bounds_map *meta, float *distance);
+int32_t pqp_bounds_map_count(const pqp_bounds_handle *h);
+/* As pqp_bounds_compute(_device), path b on slot map_index[b] (map_index [batch] in the memory space of the other
+ * buffers). A path whose index is outside [0, n_maps) reads no map and gets n_valid = 0. */
+int pqp_bounds_compute_mapped(pqp_bounds_handle *h, const pqp_bounds_in *in, const int32_t *map_index,
+                              const pqp_bounds_out *out);
+int pqp_bounds_compute_mapped_device(pqp_bounds_handle *h, const pqp_bounds_in *in, const int32_t *map_index,
+                                     const pqp_bounds_out *out, void *stream);
 
 #ifdef __cplusplus
 }

@@ -38,7 +38,9 @@ typedef struct pqp_dp_params {
 enum {
     PQP_DP_OK = 1,              /* graphSearchDp returned true */
     PQP_DP_VEHICLE_FAR = 0,     /* |vehicle offset| > lateral range: the reference returns false (:167-170) */
-    PQP_DP_TOO_MANY_LAYERS = -1 /* more layers than the handle's layers_max: nothing searched */
+    PQP_DP_TOO_MANY_LAYERS = -1, /* more layers than the handle's layers_max: nothing searched */
+    PQP_DP_MAP_INDEX = -2        /* pqp_dp_search_mapped*: map index outside [0, n_maps); no map read, n_layers =
+                                    n_out = 0 and the other outputs of the path unspecified */
 };
 
 typedef struct pqp_dp_in {
@@ -78,6 +80,11 @@ int pqp_dp_search(pqp_dp_handle *h, const pqp_dp_in *in, const pqp_dp_out *out);
 /* Device buffers; asynchronous on `stream` (a cudaStream_t passed as void*). Optional tables that are NULL are
  * kept in the handle's own scratch. */
 int pqp_dp_search_device(pqp_dp_handle *h, const pqp_dp_in *in, const pqp_dp_out *out, void *stream);
+/* As pqp_dp_search(_device), path b on map slot map_index[b] of the map owner (pqp_bounds_create_maps);
+ * map_index [batch] in the memory space of the other buffers. */
+int pqp_dp_search_mapped(pqp_dp_handle *h, const pqp_dp_in *in, const int32_t *map_index, const pqp_dp_out *out);
+int pqp_dp_search_mapped_device(pqp_dp_handle *h, const pqp_dp_in *in, const int32_t *map_index, const pqp_dp_out *out,
+                                void *stream);
 int pqp_dp_last_kernel_ms(pqp_dp_handle *h, float *ms);
 const char *pqp_dp_last_error(const pqp_dp_handle *h); /* h may be NULL: last create error */
 

@@ -53,8 +53,10 @@ enum {
     PQP_PLAN_SOLVE_FAILED = 12,     /* re-solve not PQP_SOLVED (:153-157) */
     PQP_PLAN_POINT_COUNT = 13,      /* pqp_plan_points: fewer than 4 reference points (reference_path_smoother.cpp:33-36),
                                        or more than the row stride m_max */
-    PQP_PLAN_BSPLINE_DEGREE = 14    /* pqp_plan_points: B-spline degree >= the number of points (tinyspline's
+    PQP_PLAN_BSPLINE_DEGREE = 14,   /* pqp_plan_points: B-spline degree >= the number of points (tinyspline's
                                        TS_DEG_GE_NCTRLP, an exception in the reference) */
+    PQP_PLAN_MAP_INDEX = 15         /* the mapped calls: map index outside [0, n_maps). Takes precedence over every
+                                       other status; the path reads no map, n = 0 and its path rows are 0 */
 };
 
 #define PQP_PLAN_PATH_ROWS 7 /* x, y, heading, k, d_k, l, d_heading: the SlState fields getOptimizedPath sets */
@@ -193,6 +195,32 @@ int pqp_plan_set_map_device(pqp_plan_handle *h, const pqp_bounds_map *map, void 
 int pqp_plan_set_occupancy(pqp_plan_handle *h, const pqp_occupancy_map *occ);
 int pqp_plan_set_occupancy_device(pqp_plan_handle *h, const pqp_occupancy_map *occ, void *stream);
 int pqp_plan_get_map(pqp_plan_handle *h, pqp_bounds_map *meta, float *distance);
+
+/* Per-path maps (pqp_bounds.h, "Per-path maps"). pqp_plan_create_maps: n_maps slots of the capacity of the largest
+ * map given, otherwise as pqp_plan_create (which makes one slot; the calls above act on slot 0). The mapped calls plan
+ * path b on slot map_index[b]; map_index [batch] is in the memory space of the call's other buffers. The index is
+ * checked in the chain's first glue kernel, so a mapped call takes the launches of the unmapped one (23 / 24 / 25 /
+ * 26); a path with an index outside [0, n_maps) gets PQP_PLAN_MAP_INDEX and no other path changes. Slot updates
+ * are ordered like pqp_plan_set_map_device and counted by pqp_plan_launch_count: set_map(_device) and
+ * set_map_slot(_device) 1 launch, set_occupancy(_device) 2, set_occupancy_slots(_device)
+ * 2 + ceil(count / PQP_MAP_TABLE_CHUNK). */
+int pqp_plan_create_maps(const pqp_bounds_map *maps, int32_t n_maps, const pqp_plan_params *params, int32_t r_max,
+                         int32_t p_max, int32_t layers_max, int32_t n_max, int32_t batch_max, int32_t device,
+                         pqp_plan_handle **out);
+int pqp_plan_mapped(pqp_plan_handle *h, const pqp_plan_in *in, const int32_t *map_index, const pqp_plan_out *out);
+int pqp_plan_mapped_device(pqp_plan_handle *h, const pqp_plan_in *in, const int32_t *map_index, const pqp_plan_out *out,
+                           void *stream);
+int pqp_plan_points_mapped(pqp_plan_handle *h, const pqp_plan_points_in *in, const int32_t *map_index,
+                           const pqp_plan_out *out);
+int pqp_plan_points_mapped_device(pqp_plan_handle *h, const pqp_plan_points_in *in, const int32_t *map_index,
+                                  const pqp_plan_out *out, void *stream);
+int pqp_plan_set_map_slot(pqp_plan_handle *h, int32_t slot, const pqp_bounds_map *map);
+int pqp_plan_set_map_slot_device(pqp_plan_handle *h, int32_t slot, const pqp_bounds_map *map, void *stream);
+int pqp_plan_set_occupancy_slots(pqp_plan_handle *h, int32_t first_slot, const pqp_occupancy_stack *stack);
+int pqp_plan_set_occupancy_slots_device(pqp_plan_handle *h, int32_t first_slot, const pqp_occupancy_stack *stack,
+                                        void *stream);
+int pqp_plan_get_map_slot(pqp_plan_handle *h, int32_t slot, pqp_bounds_map *meta, float *distance);
+int32_t pqp_plan_map_count(const pqp_plan_handle *h);
 /* ms[PQP_PLAN_NSTAGES] of the last call (CUDA events; waits for that call to finish). */
 int pqp_plan_last_stage_ms(pqp_plan_handle *h, float *ms);
 /* Kernel launches issued by the handle so far: the glue kernels plus those of every stage handle it owns. */

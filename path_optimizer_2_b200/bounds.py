@@ -20,7 +20,12 @@ EXPORTED_SYMBOLS = [
     "pqp_bounds_compute_device", "pqp_bounds_build_states", "pqp_bounds_build_states_device",
     "pqp_bounds_last_kernel_ms", "pqp_bounds_last_error", "pqp_bounds_set_map", "pqp_bounds_set_map_device",
     "pqp_bounds_set_occupancy", "pqp_bounds_set_occupancy_device", "pqp_bounds_get_map",
+    "pqp_bounds_create_maps", "pqp_bounds_set_map_slot", "pqp_bounds_set_map_slot_device",
+    "pqp_bounds_set_occupancy_slots", "pqp_bounds_set_occupancy_slots_device", "pqp_bounds_get_map_slot",
+    "pqp_bounds_map_count", "pqp_bounds_compute_mapped", "pqp_bounds_compute_mapped_device",
 ]
+MAX_MAP_SLOTS = 65535
+MAP_TABLE_CHUNK = 1024  # table entries per table-write launch of a slot update
 
 
 class BoundsMap(C.Structure):
@@ -33,6 +38,40 @@ class OccupancyMap(C.Structure):
     _fields_ = [("rows", C.c_int32), ("cols", C.c_int32), ("resolution", C.c_double),
                 ("center_x", C.c_double), ("center_y", C.c_double), ("cells", C.c_void_p),
                 ("obstacle_max", C.c_int32)]
+
+
+class OccupancyStack(C.Structure):
+    """pqp_occupancy_stack: `count` uint8 images [count, rows, cols] with one centre each (host arrays)."""
+    _fields_ = [("count", C.c_int32), ("rows", C.c_int32), ("cols", C.c_int32), ("resolution", C.c_double),
+                ("center_x", C.c_void_p), ("center_y", C.c_void_p), ("cells", C.c_void_p), ("obstacle_max", C.c_int32)]
+
+
+def occupancy_stack(cells_ptr, shape, resolution, centers, obstacle_max):
+    """(OccupancyStack, the float64 centre arrays it points at) for an image stack of `shape` (count, rows, cols) at
+    `cells_ptr`; `centers` is [count, 2] (None: all at the origin)."""
+    count, rows, cols = (int(v) for v in shape)
+    c = np.zeros((count, 2)) if centers is None else np.asarray(centers, dtype=np.float64).reshape(count, 2)
+    cx, cy = np.ascontiguousarray(c[:, 0]), np.ascontiguousarray(c[:, 1])
+    return OccupancyStack(count, rows, cols, float(resolution), cx.ctypes.data, cy.ctypes.data, cells_ptr,
+                          int(obstacle_max)), (cx, cy)
+
+
+def map_list(dists, resolutions, centers):
+    """(BoundsMap array, the float32 layers it points at) for per-slot layers; `resolutions` is one value or one per
+    map, `centers` None or [(x, y)] per map."""
+    dists = [np.ascontiguousarray(d, dtype=np.float32) for d in dists]
+    n = len(dists)
+    res = np.broadcast_to(np.asarray(resolutions, dtype=np.float64), (n,))
+    cen = np.zeros((n, 2)) if centers is None else np.asarray(centers, dtype=np.float64).reshape(n, 2)
+    arr = (BoundsMap * n)(*(BoundsMap(d.shape[0], d.shape[1], float(r), float(c[0]), float(c[1]), d.ctypes.data)
+                            for d, r, c in zip(dists, res, cen)))
+    return arr, dists
+
+
+def index_array(map_index, batch):
+    idx = np.ascontiguousarray(map_index, dtype=np.int32)
+    assert idx.shape == (batch,)
+    return idx
 
 
 def distance_map(dist, resolution, center):
@@ -51,8 +90,11 @@ def occupancy_map(img, resolution, center, obstacle_max):
                         img.ctypes.data, int(obstacle_max)), img
 
 
-def get_map(fn, h, check):
-    """`fn`(h, meta, layer) read-back -> (float32 layer [rows, cols], resolution, (center_x, center_y))."""
+def get_map(fn, h, check, slot_fn=None, slot=0):
+    """`fn`(h, meta, layer) read-back -> (float32 layer [rows, cols], resolution, (center_x, center_y)); a slot other
+    than 0 is read with `slot_fn`(h, slot, meta, layer)."""
+    if slot:
+        fn = lambda h_, m_, d_: slot_fn(h_, int(slot), m_, d_)  # noqa: E731
     meta = BoundsMap()
     check(fn(h, C.byref(meta), None))
     dist = np.empty((meta.rows, meta.cols), dtype=np.float32)
@@ -113,6 +155,17 @@ def _declare(L):
     L.pqp_bounds_set_occupancy.argtypes = [vp, C.POINTER(OccupancyMap)]
     L.pqp_bounds_set_occupancy_device.argtypes = [vp, C.POINTER(OccupancyMap), vp]
     L.pqp_bounds_get_map.argtypes = [vp, C.POINTER(BoundsMap), vp]
+    L.pqp_bounds_create_maps.argtypes = [C.POINTER(BoundsMap), C.c_int32, C.POINTER(BoundsParams), C.c_int32,
+                                         C.POINTER(vp)]
+    L.pqp_bounds_set_map_slot.argtypes = [vp, C.c_int32, C.POINTER(BoundsMap)]
+    L.pqp_bounds_set_map_slot_device.argtypes = [vp, C.c_int32, C.POINTER(BoundsMap), vp]
+    L.pqp_bounds_set_occupancy_slots.argtypes = [vp, C.c_int32, C.POINTER(OccupancyStack)]
+    L.pqp_bounds_set_occupancy_slots_device.argtypes = [vp, C.c_int32, C.POINTER(OccupancyStack), vp]
+    L.pqp_bounds_get_map_slot.argtypes = [vp, C.c_int32, C.POINTER(BoundsMap), vp]
+    L.pqp_bounds_map_count.argtypes = [vp]
+    L.pqp_bounds_map_count.restype = C.c_int32
+    L.pqp_bounds_compute_mapped.argtypes = [vp, C.POINTER(BoundsIn), vp, C.POINTER(BoundsOut)]
+    L.pqp_bounds_compute_mapped_device.argtypes = [vp, C.POINTER(BoundsIn), vp, C.POINTER(BoundsOut), vp]
     L._pqp_bounds_declared = True
     return L
 
@@ -132,6 +185,26 @@ class PathBounds:
             raise PqpError(rc, (self.L.pqp_bounds_last_error(None) or b"").decode())
         self.h = h
 
+    @classmethod
+    def from_maps(cls, dists, resolutions, *, centers=None, params=None, device=0):
+        """One handle with a map slot per float32 layer in `dists` (each slot as large as the largest layer);
+        `resolutions` is one value or one per map, `centers` [(x, y)] per map (default: the origin)."""
+        self = cls.__new__(cls)
+        self.L = _declare(load_library())
+        arr, self._layers = map_list(dists, resolutions, centers)
+        self.dist = self._layers[0]
+        self.params = params if params is not None else default_params()
+        h = C.c_void_p()
+        rc = self.L.pqp_bounds_create_maps(arr, len(self._layers), C.byref(self.params), int(device), C.byref(h))
+        if rc:
+            raise PqpError(rc, (self.L.pqp_bounds_last_error(None) or b"").decode())
+        self.h = h
+        return self
+
+    @property
+    def n_maps(self):
+        return int(self.L.pqp_bounds_map_count(self.h))
+
     def close(self):
         if getattr(self, "h", None):
             self.L.pqp_bounds_destroy(self.h)
@@ -143,9 +216,10 @@ class PathBounds:
         if rc:
             raise PqpError(rc, (self.L.pqp_bounds_last_error(self.h) or b"").decode())
 
-    def compute(self, states, n, spline, k, *, knots=None):
+    def compute(self, states, n, spline, k, *, knots=None, map_index=None):
         """Host buffers: states[b][4][n_max], n[b], spline[b][9][k_max], k[b] ->
-        (bounds[b][6][n_max], n_valid[b]); `knots` (solver block [b][9][n_max]) is filled in place."""
+        (bounds[b][6][n_max], n_valid[b]); `knots` (solver block [b][9][n_max]) is filled in place. `map_index` [b]:
+        path b on map slot map_index[b] (out of range: n_valid 0)."""
         states = np.ascontiguousarray(states, dtype=np.float64)
         spline = np.ascontiguousarray(spline, dtype=np.float64)
         n = np.ascontiguousarray(n, dtype=np.int32)
@@ -157,7 +231,11 @@ class PathBounds:
             assert knots.flags.c_contiguous and knots.dtype == np.float64 and knots.shape == (B, abi.NFIELDS, n_max)
         bi = BoundsIn(B, n_max, spline.shape[2], states.ctypes.data, n.ctypes.data, spline.ctypes.data, k.ctypes.data)
         bo = BoundsOut(bounds.ctypes.data, n_valid.ctypes.data, knots.ctypes.data if knots is not None else None)
-        self._check(self.L.pqp_bounds_compute(self.h, C.byref(bi), C.byref(bo)))
+        if map_index is None:
+            self._check(self.L.pqp_bounds_compute(self.h, C.byref(bi), C.byref(bo)))
+        else:
+            idx = index_array(map_index, B)
+            self._check(self.L.pqp_bounds_compute_mapped(self.h, C.byref(bi), idx.ctypes.data, C.byref(bo)))
         return bounds, n_valid
 
     def compute_device(self, bin_struct: BoundsIn, bout_struct: BoundsOut, stream=0):
@@ -193,17 +271,42 @@ class PathBounds:
         self._check(self.L.pqp_bounds_last_kernel_ms(self.h, C.byref(ms)))
         return ms.value
 
-    def set_map(self, dist, resolution, center=(0.0, 0.0)):
-        """Replace the map with a float32 distance layer [rows, cols] (rows * cols <= the cells at construction)."""
+    def set_map(self, dist, resolution, center=(0.0, 0.0), slot=0):
+        """Replace the map (of `slot`) with a float32 distance layer [rows, cols] (rows * cols <= the cells at
+        construction)."""
         m, _keep = distance_map(dist, resolution, center)
-        self._check(self.L.pqp_bounds_set_map(self.h, C.byref(m)))
+        if slot:
+            self._check(self.L.pqp_bounds_set_map_slot(self.h, int(slot), C.byref(m)))
+        else:
+            self._check(self.L.pqp_bounds_set_map(self.h, C.byref(m)))
 
-    def set_occupancy(self, img, resolution, center=(0.0, 0.0), obstacle_max=0):
-        """Replace the map with the exact Euclidean distance transform of a uint8 image [rows, cols], computed on the
-        GPU: cells <= obstacle_max are obstacles (0: the demo's zero pixels)."""
+    def set_occupancy(self, img, resolution, center=(0.0, 0.0), obstacle_max=0, slot=0):
+        """Replace the map (of `slot`) with the exact Euclidean distance transform of a uint8 image [rows, cols],
+        computed on the GPU: cells <= obstacle_max are obstacles (0: the demo's zero pixels)."""
+        if slot:
+            img = np.ascontiguousarray(img, dtype=np.uint8)
+            self.set_occupancy_slots(img[None], resolution, [center], obstacle_max, first_slot=slot)
+            return
         m, _keep = occupancy_map(img, resolution, center, obstacle_max)
         self._check(self.L.pqp_bounds_set_occupancy(self.h, C.byref(m)))
 
-    def get_map(self):
-        """-> (float32 distance layer [rows, cols], resolution, (center_x, center_y)) of the current map."""
-        return get_map(self.L.pqp_bounds_get_map, self.h, self._check)
+    def set_occupancy_slots(self, imgs, resolution, centers=None, obstacle_max=0, *, first_slot=0):
+        """The distance transforms of a uint8 stack [count, rows, cols] into slots first_slot .. + count - 1 (host,
+        synchronous); `centers` [count, 2]."""
+        imgs = np.ascontiguousarray(imgs, dtype=np.uint8)
+        assert imgs.ndim == 3
+        st, _keep = occupancy_stack(imgs.ctypes.data, imgs.shape, resolution, centers, obstacle_max)
+        self._check(self.L.pqp_bounds_set_occupancy_slots(self.h, int(first_slot), C.byref(st)))
+
+    def set_occupancy_slots_device(self, imgs, resolution, centers=None, obstacle_max=0, *, first_slot=0, stream=0):
+        """As `set_occupancy_slots` from a torch uint8 CUDA tensor [count, rows, cols], asynchronous on `stream` (a raw
+        cudaStream_t; the tensor must live until the stream has run the transform)."""
+        import torch
+        assert imgs.is_cuda and imgs.is_contiguous() and imgs.dtype == torch.uint8 and imgs.dim() == 3
+        st, _keep = occupancy_stack(imgs.data_ptr(), imgs.shape, resolution, centers, obstacle_max)
+        self._check(self.L.pqp_bounds_set_occupancy_slots_device(self.h, int(first_slot), C.byref(st),
+                                                                 C.c_void_p(stream)))
+
+    def get_map(self, slot=0):
+        """-> (float32 distance layer [rows, cols], resolution, (center_x, center_y)) of the current map (of `slot`)."""
+        return get_map(self.L.pqp_bounds_get_map, self.h, self._check, self.L.pqp_bounds_get_map_slot, slot)

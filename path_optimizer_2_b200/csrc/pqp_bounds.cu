@@ -10,8 +10,10 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <new>
 #include <string>
+#include <vector>
 
 #include "../../include/pqp_bounds.h"
 #include "pqp_bounds_core.cuh"
@@ -22,7 +24,10 @@
 namespace {
 
 struct BoundsArgs {
-    pqb::MapView map;
+    pqb::MapView map;             // the shared map, when map_index is NULL
+    const pqb::MapView *table;    // per-path maps: path b reads table[map_index[b]]
+    const int32_t *map_index;
+    int n_maps;
     pqb::Params prm;
     int batch, n_max, k_max;
     const double *states;
@@ -34,10 +39,13 @@ struct BoundsArgs {
     double *knots;
 };
 
-__global__ void init_n_valid_kernel(const int32_t *__restrict__ n, int32_t *__restrict__ n_valid, int batch, int n_max) {
+// a path whose map index is out of range gets n_valid = 0 here and is skipped by the clearance kernel
+__global__ void init_n_valid_kernel(const int32_t *__restrict__ n, int32_t *__restrict__ n_valid, int batch, int n_max,
+                                    const int32_t *__restrict__ map_index, int n_maps) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b < batch) {
         int v = n[b];
+        if (map_index && !(map_index[b] >= 0 && map_index[b] < n_maps)) v = 0;
         n_valid[b] = v < 0 ? 0 : (v > n_max ? n_max : v);
     }
 }
@@ -64,7 +72,13 @@ __global__ void __launch_bounds__(128) clearance_bounds_kernel(const BoundsArgs 
     sp.ya = sb + 5 * (size_t)a.k_max; sp.yb = sb + 6 * (size_t)a.k_max; sp.yc = sb + 7 * (size_t)a.k_max; sp.yy = sb + 8 * (size_t)a.k_max;
     sp.k = a.k[b] > a.k_max ? a.k_max : a.k[b];
     double lb, ub;
-    pqb::anchor_bounds(a.map, a.prm, sp, s, x, y, heading, anchor, lb, ub);
+    if (a.map_index) {
+        const pqb::MapView *map = pqb::slot_view(a.table, a.n_maps, a.map_index, b);
+        if (!map) return;
+        pqb::anchor_bounds(*map, a.prm, sp, s, x, y, heading, anchor, lb, ub);
+    } else {
+        pqb::anchor_bounds(a.map, a.prm, sp, s, x, y, heading, anchor, lb, ub);
+    }
     double *ob = a.bounds + (size_t)b * PQP_BOUND_ROWS * a.n_max;
     ob[(size_t)(2 * anchor) * a.n_max + i] = lb;
     ob[(size_t)(2 * anchor + 1) * a.n_max + i] = ub;
@@ -129,22 +143,50 @@ namespace pqm {
 constexpr int kEdtColumnThreads = 128;
 constexpr int kEdtRowThreads = 64;
 
-// one thread per column: consecutive threads read consecutive bytes of a row
-__global__ void __launch_bounds__(kEdtColumnThreads) edt_column_kernel(const uint8_t *__restrict__ img, int rows, int cols,
-                                                                        int obstacle_max, int32_t *__restrict__ g) {
-    const int j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j < cols) pqm::column_pass(img, rows, cols, j, obstacle_max, g);
+// Table entries first .. first + n - 1 of a slot update: `meta` with slot first + i's layer and centre i. Passed by
+// value, so the entries a launch writes are fixed when it is enqueued (PQP_MAP_TABLE_CHUNK * 16 B of parameters).
+struct TableWrite {
+    pqb::MapView *table;
+    pqb::MapView meta;  // dist: the layer of slot `first`
+    size_t slot_cells;
+    int first, n;
+    double cx[PQP_MAP_TABLE_CHUNK], cy[PQP_MAP_TABLE_CHUNK];
+};
+
+__global__ void map_table_kernel(const TableWrite w) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= w.n) return;
+    pqb::MapView m = w.meta;
+    m.dist += (size_t)i * w.slot_cells;
+    m.cx = w.cx[i];
+    m.cy = w.cy[i];
+    w.table[w.first + i] = m;
 }
 
-// one block per row: the block loads the row's g, thread 0 builds the lower envelope, the block fills d2 per
-// envelope parabola and converts it to the layer's floats
-__global__ void __launch_bounds__(kEdtRowThreads) edt_row_kernel(void *layer, int rows, int cols, float res) {
+// one thread per column of image blockIdx.y: consecutive threads read consecutive bytes of a row. Images are
+// rows * cols bytes apart, their g slot_cells int32 apart (in the layers of consecutive slots). A one-image update
+// also writes its slot's table entry (`entry_dst`, NULL for none) here, so it costs no launch of its own.
+__global__ void __launch_bounds__(kEdtColumnThreads) edt_column_kernel(const uint8_t *__restrict__ img, int rows, int cols,
+                                                                        int obstacle_max, int32_t *__restrict__ g,
+                                                                        size_t slot_cells, pqb::MapView *entry_dst,
+                                                                        const pqb::MapView entry) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    const size_t y = blockIdx.y;
+    if (entry_dst && j == 0 && y == 0) *entry_dst = entry;
+    if (j < cols) pqm::column_pass(img + y * rows * cols, rows, cols, j, obstacle_max, g + y * slot_cells);
+}
+
+// one block per row of image blockIdx.y: the block loads the row's g, thread 0 builds the lower envelope, the block
+// fills d2 per envelope parabola and converts it to the layer's floats
+__global__ void __launch_bounds__(kEdtRowThreads) edt_row_kernel(void *layers, size_t slot_cells, int rows, int cols,
+                                                                 float res) {
     extern __shared__ int4 edt_smem[];
     int32_t *g = reinterpret_cast<int32_t *>(edt_smem);
     int32_t *h = g + cols;
     int16_t *s = reinterpret_cast<int16_t *>(h + cols);
     int16_t *t = s + cols;
     __shared__ int n_env;
+    void *layer = static_cast<int32_t *>(layers) + blockIdx.y * slot_cells;
     const size_t row = (size_t)blockIdx.x * cols;
     const int32_t *gin = static_cast<const int32_t *>(layer) + row;
     for (int u = threadIdx.x; u < cols; u += blockDim.x) g[u] = gin[u];
@@ -163,16 +205,19 @@ __global__ void __launch_bounds__(kEdtRowThreads) edt_row_kernel(void *layer, in
 
 struct pqp_bounds_handle {
     int device = 0;
-    pqb::MapView map{};
+    int n_maps = 1;
+    std::vector<pqb::MapView> maps;  // the slots' metadata as the host calls left them (slot 0: the unmapped calls' map)
     pqb::Params prm{};
-    float *d_dist = nullptr;
-    size_t cap_cells = 0;        // cells of the map the handle was created with: the most any later map may have
-    uint8_t *d_occ = nullptr;    // [cap_cells] staging of pqp_bounds_set_occupancy's host image
+    float *d_dist = nullptr;          // [n_maps][cap_cells] distance layers
+    size_t cap_cells = 0;             // cells per slot: the largest map the handle was created with
+    uint8_t *d_occ = nullptr;         // [n_maps][cap_cells] staging of the host set_occupancy calls' images
+    pqb::MapView *d_table = nullptr;  // [n_maps] the slots' metadata as the mapped kernels read it, in stream order
+    std::unique_ptr<pqm::TableWrite> tw{new (std::nothrow) pqm::TableWrite};  // parameters of map_table_kernel
     cudaStream_t stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     // staging for the host-pointer call (grown on demand)
     double *d_states = nullptr, *d_spline = nullptr, *d_bounds = nullptr, *d_knots = nullptr;
-    int32_t *d_n = nullptr, *d_k = nullptr, *d_nvalid = nullptr;
+    int32_t *d_n = nullptr, *d_k = nullptr, *d_nvalid = nullptr, *d_map_index = nullptr;
     double *d_maxs = nullptr, *d_curv = nullptr;
     int32_t *d_total = nullptr;
     bool timed = false;
@@ -181,8 +226,10 @@ struct pqp_bounds_handle {
 };
 
 namespace pqb {
-const MapView *handle_map(const pqp_bounds_handle *h) { return h ? &h->map : nullptr; }
+const MapView *handle_map(const pqp_bounds_handle *h) { return h ? &h->maps[0] : nullptr; }
 int handle_device(const pqp_bounds_handle *h) { return h ? h->device : -1; }
+const MapView *handle_table(const pqp_bounds_handle *h) { return h ? h->d_table : nullptr; }
+int handle_map_count(const pqp_bounds_handle *h) { return h ? h->n_maps : 0; }
 }  // namespace pqb
 
 namespace {
@@ -199,9 +246,14 @@ int validate(pqp_bounds_handle *h, const pqp_bounds_in *in, const pqp_bounds_out
     return PQP_OK;
 }
 
-int launch(pqp_bounds_handle *h, const pqp_bounds_in *in, const pqp_bounds_out *out, cudaStream_t s) {
+// map_index: NULL for the shared map (slot 0 as the host last set it), else [batch] slot per path on the device
+int launch(pqp_bounds_handle *h, const pqp_bounds_in *in, const int32_t *map_index, const pqp_bounds_out *out,
+           cudaStream_t s) {
     BoundsArgs a;
-    a.map = h->map;
+    a.map = h->maps[0];
+    a.table = h->d_table;
+    a.map_index = map_index;
+    a.n_maps = h->n_maps;
     a.prm = h->prm;
     a.batch = in->batch;
     a.n_max = in->n_max;
@@ -214,7 +266,8 @@ int launch(pqp_bounds_handle *h, const pqp_bounds_in *in, const pqp_bounds_out *
     a.n_valid = out->n_valid;
     a.knots = out->knots;
     PQP_CUDA(h->err, cudaEventRecord(h->ev0, s));
-    init_n_valid_kernel<<<(in->batch + 255) / 256, 256, 0, s>>>(in->n, out->n_valid, in->batch, in->n_max);
+    init_n_valid_kernel<<<(in->batch + 255) / 256, 256, 0, s>>>(in->n, out->n_valid, in->batch, in->n_max, map_index,
+                                                                 h->n_maps);
     const long long total = (long long)in->batch * in->n_max;
     const long long blocks = (total + 127) / 128;
     if (blocks > 0x7fffffffLL) return fail(h->err, PQP_E_INVALID, "pqp_bounds: batch * n_max too large for one launch");
@@ -225,19 +278,46 @@ int launch(pqp_bounds_handle *h, const pqp_bounds_in *in, const pqp_bounds_out *
     return PQP_OK;
 }
 
-void set_meta(pqp_bounds_handle *h, int rows, int cols, double res, double cx, double cy) {
-    h->map.dist = h->d_dist;
-    h->map.rows = rows;
-    h->map.cols = cols;
-    h->map.res = res;
-    h->map.inv_res = 1.0 / res;
-    h->map.half_lx = 0.5 * rows * res;
-    h->map.half_ly = 0.5 * cols * res;
-    h->map.cx = cx;
-    h->map.cy = cy;
+pqb::MapView make_view(const float *dist, int rows, int cols, double res, double cx, double cy) {
+    pqb::MapView m;
+    m.dist = dist;
+    m.rows = rows;
+    m.cols = cols;
+    m.res = res;
+    m.inv_res = 1.0 / res;
+    m.half_lx = 0.5 * rows * res;
+    m.half_ly = 0.5 * cols * res;
+    m.cx = cx;
+    m.cy = cy;
+    return m;
 }
 
-// what pqp_bounds_set_map* and pqp_bounds_set_occupancy* accept; a refused map leaves the handle's map untouched
+float *slot_layer(pqp_bounds_handle *h, int slot) { return h->d_dist + (size_t)slot * h->cap_cells; }
+
+// table entries first .. first + count - 1: `meta` (dist: slot first's layer) with centre i = (cx[i], cy[i]), in
+// launches of PQP_MAP_TABLE_CHUNK entries
+int write_table(pqp_bounds_handle *h, int first, int count, const pqb::MapView &meta, const double *cx, const double *cy,
+                cudaStream_t s) {
+    pqm::TableWrite &w = *h->tw;
+    for (int done = 0; done < count; done += PQP_MAP_TABLE_CHUNK) {
+        const int n = count - done < PQP_MAP_TABLE_CHUNK ? count - done : PQP_MAP_TABLE_CHUNK;
+        w.table = h->d_table;
+        w.meta = meta;
+        w.meta.dist = meta.dist + (size_t)done * h->cap_cells;
+        w.slot_cells = h->cap_cells;
+        w.first = first + done;
+        w.n = n;
+        for (int i = 0; i < n; ++i) {
+            w.cx[i] = cx[done + i];
+            w.cy[i] = cy[done + i];
+        }
+        pqm::map_table_kernel<<<(n + 127) / 128, 128, 0, s>>>(w);
+        PQP_CUDA(h->err, cudaGetLastError());
+    }
+    return PQP_OK;
+}
+
+// what pqp_bounds_set_map* and pqp_bounds_set_occupancy* accept; a refused map leaves the handle's maps untouched
 int validate_map(pqp_bounds_handle *h, const void *m, int rows, int cols, double res, double cx, double cy,
                  const void *data, const char *what) {
     if (!h) return PQP_E_INVALID;
@@ -250,15 +330,29 @@ int validate_map(pqp_bounds_handle *h, const void *m, int rows, int cols, double
     return why.empty() ? PQP_OK : fail(h->err, PQP_E_INVALID, std::string(what) + ": " + why);
 }
 
-int launch_edt(pqp_bounds_handle *h, const pqp_occupancy_map *occ, const uint8_t *cells, cudaStream_t s) {
-    const int rows = occ->rows, cols = occ->cols;
+int validate_slots(pqp_bounds_handle *h, long long first, long long count, const char *what) {
+    if (first < 0 || count < 1 || first + count > h->n_maps)
+        return fail(h->err, PQP_E_INVALID, std::string(what) + ": slots " + std::to_string(first) + " .. " +
+                                               std::to_string(first + count - 1) + " outside [0, " +
+                                               std::to_string(h->n_maps) + ")");
+    return PQP_OK;
+}
+
+// the two passes over `count` images of rows x cols (consecutive in `cells`) into slots first .. first + count - 1;
+// entry_dst (one image only): the table entry the column pass writes
+int launch_edt(pqp_bounds_handle *h, int rows, int cols, double resolution, int obstacle_max, const uint8_t *cells,
+               int count, int first, pqb::MapView *entry_dst, const pqb::MapView &entry, cudaStream_t s) {
     const size_t smem = (size_t)pqm::kRowSmemPerCol * cols;
     // the dynamic share plus the kernel's static n_env may pass the 48 KB default at any width: always opt in
     PQP_CUDA(h->err, cudaFuncSetAttribute(pqm::edt_row_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    pqm::edt_column_kernel<<<(cols + pqm::kEdtColumnThreads - 1) / pqm::kEdtColumnThreads, pqm::kEdtColumnThreads, 0,
-                             s>>>(cells, rows, cols, occ->obstacle_max, reinterpret_cast<int32_t *>(h->d_dist));
+    float *layer = slot_layer(h, first);
+    pqm::edt_column_kernel<<<dim3((cols + pqm::kEdtColumnThreads - 1) / pqm::kEdtColumnThreads, count),
+                             pqm::kEdtColumnThreads, 0, s>>>(cells, rows, cols, obstacle_max,
+                                                             reinterpret_cast<int32_t *>(layer), h->cap_cells, entry_dst,
+                                                             entry);
     PQP_CUDA(h->err, cudaGetLastError());
-    pqm::edt_row_kernel<<<rows, pqm::kEdtRowThreads, smem, s>>>(h->d_dist, rows, cols, (float)occ->resolution);
+    pqm::edt_row_kernel<<<dim3(rows, count), pqm::kEdtRowThreads, smem, s>>>(layer, h->cap_cells, rows, cols,
+                                                                             (float)resolution);
     PQP_CUDA(h->err, cudaGetLastError());
     return PQP_OK;
 }
@@ -270,6 +364,185 @@ int validate_occupancy(pqp_bounds_handle *h, const pqp_occupancy_map *occ, const
     if (rc != PQP_OK) return rc;
     if (occ->rows > pqm::kMaxSide || occ->cols > pqm::kMaxSide)
         return fail(h->err, PQP_E_INVALID, std::string(what) + ": rows and cols must be <= 16384 for the distance transform");
+    return PQP_OK;
+}
+
+// one image into slot 0, the table entry written by the column pass (no launch of its own)
+int set_occupancy0(pqp_bounds_handle *h, const pqp_occupancy_map *occ, const uint8_t *cells, cudaStream_t s) {
+    const pqb::MapView m = make_view(slot_layer(h, 0), occ->rows, occ->cols, occ->resolution, occ->center_x, occ->center_y);
+    const int rc = launch_edt(h, occ->rows, occ->cols, occ->resolution, occ->obstacle_max, cells, 1, 0, h->d_table, m, s);
+    if (rc != PQP_OK) return rc;
+    h->maps[0] = m;
+    return PQP_OK;
+}
+
+int validate_stack(pqp_bounds_handle *h, int first, const pqp_occupancy_stack *st, const char *what) {
+    if (!h) return PQP_E_INVALID;
+    if (!st || !st->cells || !st->center_x || !st->center_y)
+        return fail(h->err, PQP_E_INVALID, std::string(what) + ": null stack, image or centres");
+    int rc = validate_slots(h, first, st->count, what);
+    if (rc != PQP_OK) return rc;
+    for (int i = 0; i < st->count; ++i) {
+        rc = validate_map(h, st, st->rows, st->cols, st->resolution, st->center_x[i], st->center_y[i], st->cells, what);
+        if (rc != PQP_OK) return rc;
+    }
+    if (st->rows > pqm::kMaxSide || st->cols > pqm::kMaxSide)
+        return fail(h->err, PQP_E_INVALID, std::string(what) + ": rows and cols must be <= 16384 for the distance transform");
+    return PQP_OK;
+}
+
+int set_occupancy_slots(pqp_bounds_handle *h, int first, const pqp_occupancy_stack *st, const uint8_t *cells,
+                        cudaStream_t s) {
+    const pqb::MapView meta = make_view(slot_layer(h, first), st->rows, st->cols, st->resolution, 0.0, 0.0);
+    int rc = launch_edt(h, st->rows, st->cols, st->resolution, st->obstacle_max, cells, st->count, first, nullptr, meta, s);
+    if (rc != PQP_OK) return rc;
+    rc = write_table(h, first, st->count, meta, st->center_x, st->center_y, s);
+    if (rc != PQP_OK) return rc;
+    for (int i = 0; i < st->count; ++i)
+        h->maps[first + i] = make_view(slot_layer(h, first + i), st->rows, st->cols, st->resolution, st->center_x[i],
+                                       st->center_y[i]);
+    return PQP_OK;
+}
+
+int create(const pqp_bounds_map *maps, int n_maps, const pqp_bounds_params *params, int32_t device,
+           pqp_bounds_handle **out, const char *what) {
+    if (!out) return PQP_E_INVALID;
+    *out = nullptr;
+    if (n_maps < 1 || n_maps > PQP_MAX_MAP_SLOTS)
+        return fail(g_bounds_create_error, PQP_E_INVALID, std::string(what) + ": 1 <= n_maps <= 65535 required");
+    size_t cap = 0;
+    for (int i = 0; i < n_maps; ++i) {
+        if (!maps || !maps[i].distance || maps[i].rows < 2 || maps[i].cols < 2 || !(maps[i].resolution > 0.0))
+            return fail(g_bounds_create_error, PQP_E_INVALID,
+                        std::string(what) + ": map needs rows, cols >= 2, resolution > 0 and a distance layer");
+        const size_t cells = (size_t)maps[i].rows * maps[i].cols;
+        cap = cells > cap ? cells : cap;
+    }
+    int count = 0;
+    if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0 || device < 0 || device >= count)
+        return fail(g_bounds_create_error, PQP_E_NO_DEVICE, std::string(what) + ": no CUDA device (there is no CPU fallback)");
+    pqp_bounds_handle *h = new (std::nothrow) pqp_bounds_handle();
+    if (!h || !h->tw) {
+        delete h;
+        return fail(g_bounds_create_error, PQP_E_CUDA, std::string(what) + ": out of host memory");
+    }
+    h->device = h->res.device = device;
+    pqp_bounds_params dflt;
+    pqp_bounds_default_params(&dflt);
+    const pqp_bounds_params &p = params ? *params : dflt;
+    h->prm.front_length = p.front_length;
+    h->prm.rear_length = p.rear_length;
+    h->prm.car_width = p.car_width;
+    h->prm.safety_margin = p.safety_margin;
+    h->prm.epsilon = p.epsilon;
+    h->n_maps = n_maps;
+    h->cap_cells = cap;
+    pqp::DeviceGuard guard_(device);
+    const int rc = [&]() -> int {
+        std::string &err = g_bounds_create_error;
+        const size_t total = (size_t)n_maps * cap;
+        const cudaError_t e = h->res.alloc(h->d_dist, total);
+        if (e != cudaSuccess)
+            return fail(err, PQP_E_CUDA, std::string(what) + ": cannot allocate " + std::to_string(n_maps) + " slots of " +
+                                             std::to_string(cap) + " cells (" + std::to_string(total * sizeof(float)) +
+                                             " bytes of layers): " + cudaGetErrorString(e));
+        PQP_CUDA(err, h->res.alloc(h->d_occ, total));
+        PQP_CUDA(err, h->res.alloc(h->d_table, (size_t)n_maps));
+        h->maps.resize(n_maps);
+        for (int i = 0; i < n_maps; ++i) {
+            const pqp_bounds_map &m = maps[i];
+            h->maps[i] = make_view(slot_layer(h, i), m.rows, m.cols, m.resolution, m.center_x, m.center_y);
+            PQP_CUDA(err, cudaMemcpy(slot_layer(h, i), m.distance, (size_t)m.rows * m.cols * sizeof(float),
+                                     cudaMemcpyHostToDevice));
+        }
+        PQP_CUDA(err, cudaMemcpy(h->d_table, h->maps.data(), n_maps * sizeof(pqb::MapView), cudaMemcpyHostToDevice));
+        PQP_CUDA(err, h->res.stream(h->stream));
+        PQP_CUDA(err, h->res.event(h->ev0));
+        PQP_CUDA(err, h->res.event(h->ev1));
+        return PQP_OK;
+    }();
+    if (rc != PQP_OK) {
+        pqp_bounds_destroy(h);
+        return rc;
+    }
+    *out = h;
+    return PQP_OK;
+}
+
+int set_map_slot(pqp_bounds_handle *h, int slot, const pqp_bounds_map *map, cudaStream_t s, const char *what) {
+    if (!h) return PQP_E_INVALID;
+    int rc = validate_slots(h, slot, 1, what);
+    if (rc != PQP_OK) return rc;
+    rc = map ? validate_map(h, map, map->rows, map->cols, map->resolution, map->center_x, map->center_y, map->distance,
+                            what)
+             : validate_map(h, nullptr, 0, 0, 0.0, 0.0, 0.0, nullptr, what);
+    if (rc != PQP_OK) return rc;
+    pqp::DeviceGuard guard_(h->device);
+    const size_t cells = (size_t)map->rows * map->cols;
+    PQP_CUDA(h->err, cudaMemcpyAsync(slot_layer(h, slot), map->distance, cells * sizeof(float), cudaMemcpyDefault, s));
+    const pqb::MapView m = make_view(slot_layer(h, slot), map->rows, map->cols, map->resolution, map->center_x,
+                                     map->center_y);
+    rc = write_table(h, slot, 1, m, &map->center_x, &map->center_y, s);
+    if (rc != PQP_OK) return rc;
+    h->maps[slot] = m;
+    return PQP_OK;
+}
+
+int get_map_slot(pqp_bounds_handle *h, int slot, pqp_bounds_map *meta, float *distance, const char *what) {
+    if (!h) return PQP_E_INVALID;
+    if (!meta) return fail(h->err, PQP_E_INVALID, std::string(what) + ": null metadata");
+    const int rc = validate_slots(h, slot, 1, what);
+    if (rc != PQP_OK) return rc;
+    pqp::DeviceGuard guard_(h->device);
+    const pqb::MapView &m = h->maps[slot];
+    meta->rows = m.rows;
+    meta->cols = m.cols;
+    meta->resolution = m.res;
+    meta->center_x = m.cx;
+    meta->center_y = m.cy;
+    meta->distance = nullptr;
+    if (distance) {
+        PQP_CUDA(h->err, cudaDeviceSynchronize());
+        PQP_CUDA(h->err, cudaMemcpy(distance, m.dist, (size_t)m.rows * m.cols * sizeof(float), cudaMemcpyDeviceToHost));
+    }
+    return PQP_OK;
+}
+
+int compute_host(pqp_bounds_handle *h, const pqp_bounds_in *in, const int32_t *map_index, const pqp_bounds_out *out) {
+    pqp::DeviceGuard guard_(h->device);
+    const size_t B = in->batch, ns = B * PQP_STATE_ROWS * in->n_max, nsp = B * PQP_SPLINE_ROWS * in->k_max;
+    const size_t nb = B * PQP_BOUND_ROWS * in->n_max, nk = out->knots ? B * PQP_NFIELDS * in->n_max : 0;
+    PQP_CUDA(h->err, h->res.grow(h->d_states, ns));
+    PQP_CUDA(h->err, h->res.grow(h->d_bounds, nb));
+    PQP_CUDA(h->err, h->res.grow(h->d_spline, nsp));
+    if (nk) PQP_CUDA(h->err, h->res.grow(h->d_knots, nk));
+    PQP_CUDA(h->err, h->res.grow(h->d_n, B));
+    PQP_CUDA(h->err, h->res.grow(h->d_k, B));
+    PQP_CUDA(h->err, h->res.grow(h->d_nvalid, B));
+    if (map_index) PQP_CUDA(h->err, h->res.grow(h->d_map_index, B));
+    cudaStream_t s = h->stream;
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_states, in->states, ns * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_spline, in->spline, nsp * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_n, in->n, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_k, in->k, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    if (nk) PQP_CUDA(h->err, cudaMemcpyAsync(h->d_knots, out->knots, nk * sizeof(double), cudaMemcpyHostToDevice, s));
+    if (map_index)
+        PQP_CUDA(h->err, cudaMemcpyAsync(h->d_map_index, map_index, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    pqp_bounds_in din = *in;
+    din.states = h->d_states;
+    din.spline = h->d_spline;
+    din.n = h->d_n;
+    din.k = h->d_k;
+    pqp_bounds_out dout;
+    dout.bounds = h->d_bounds;
+    dout.n_valid = h->d_nvalid;
+    dout.knots = nk ? h->d_knots : nullptr;
+    const int rc = launch(h, &din, map_index ? h->d_map_index : nullptr, &dout, s);
+    if (rc != PQP_OK) return rc;
+    PQP_CUDA(h->err, cudaMemcpyAsync(out->bounds, h->d_bounds, nb * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(out->n_valid, h->d_nvalid, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    if (nk) PQP_CUDA(h->err, cudaMemcpyAsync(out->knots, h->d_knots, nk * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaStreamSynchronize(s));
     return PQP_OK;
 }
 
@@ -288,92 +561,48 @@ void pqp_bounds_default_params(pqp_bounds_params *p) {
 
 int pqp_bounds_create(const pqp_bounds_map *map, const pqp_bounds_params *params, int32_t device,
                       pqp_bounds_handle **out) {
-    if (!out) return PQP_E_INVALID;
-    *out = nullptr;
-    if (!map || !map->distance || map->rows < 2 || map->cols < 2 || !(map->resolution > 0.0))
-        return fail(g_bounds_create_error, PQP_E_INVALID,
-                    "pqp_bounds_create: map needs rows, cols >= 2, resolution > 0 and a distance layer");
-    int count = 0;
-    if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0 || device < 0 || device >= count)
-        return fail(g_bounds_create_error, PQP_E_NO_DEVICE, "pqp_bounds_create: no CUDA device (there is no CPU fallback)");
-    pqp_bounds_handle *h = new (std::nothrow) pqp_bounds_handle();
-    if (!h) return PQP_E_CUDA;
-    h->device = h->res.device = device;
-    pqp_bounds_params dflt;
-    pqp_bounds_default_params(&dflt);
-    const pqp_bounds_params &p = params ? *params : dflt;
-    h->prm.front_length = p.front_length;
-    h->prm.rear_length = p.rear_length;
-    h->prm.car_width = p.car_width;
-    h->prm.safety_margin = p.safety_margin;
-    h->prm.epsilon = p.epsilon;
-    const size_t cells = (size_t)map->rows * map->cols;
-    pqp::DeviceGuard guard_(device);
-    const int rc = [&]() -> int {
-        PQP_CUDA(g_bounds_create_error, h->res.alloc(h->d_dist, cells));
-        PQP_CUDA(g_bounds_create_error, cudaMemcpy(h->d_dist, map->distance, cells * sizeof(float), cudaMemcpyHostToDevice));
-        PQP_CUDA(g_bounds_create_error, h->res.alloc(h->d_occ, cells));
-        PQP_CUDA(g_bounds_create_error, h->res.stream(h->stream));
-        PQP_CUDA(g_bounds_create_error, h->res.event(h->ev0));
-        PQP_CUDA(g_bounds_create_error, h->res.event(h->ev1));
-        return PQP_OK;
-    }();
-    if (rc != PQP_OK) {
-        pqp_bounds_destroy(h);
-        return rc;
-    }
-    h->cap_cells = cells;
-    set_meta(h, map->rows, map->cols, map->resolution, map->center_x, map->center_y);
-    *out = h;
-    return PQP_OK;
+    return create(map, 1, params, device, out, "pqp_bounds_create");
+}
+
+int pqp_bounds_create_maps(const pqp_bounds_map *maps, int32_t n_maps, const pqp_bounds_params *params,
+                           int32_t device, pqp_bounds_handle **out) {
+    return create(maps, n_maps, params, device, out, "pqp_bounds_create_maps");
 }
 
 void pqp_bounds_destroy(pqp_bounds_handle *h) {
     delete h;
 }
 
+int32_t pqp_bounds_map_count(const pqp_bounds_handle *h) { return h ? h->n_maps : 0; }
+
 int pqp_bounds_compute_device(pqp_bounds_handle *h, const pqp_bounds_in *in, const pqp_bounds_out *out, void *stream) {
     int rc = validate(h, in, out);
     if (rc != PQP_OK) return rc;
     pqp::DeviceGuard guard_(h->device);
-    return launch(h, in, out, static_cast<cudaStream_t>(stream));
+    return launch(h, in, nullptr, out, static_cast<cudaStream_t>(stream));
 }
 
 int pqp_bounds_compute(pqp_bounds_handle *h, const pqp_bounds_in *in, const pqp_bounds_out *out) {
+    const int rc = validate(h, in, out);
+    if (rc != PQP_OK) return rc;
+    return compute_host(h, in, nullptr, out);
+}
+
+int pqp_bounds_compute_mapped_device(pqp_bounds_handle *h, const pqp_bounds_in *in, const int32_t *map_index,
+                                     const pqp_bounds_out *out, void *stream) {
     int rc = validate(h, in, out);
     if (rc != PQP_OK) return rc;
+    if (!map_index) return fail(h->err, PQP_E_INVALID, "pqp_bounds_compute_mapped_device: null map_index");
     pqp::DeviceGuard guard_(h->device);
-    const size_t B = in->batch, ns = B * PQP_STATE_ROWS * in->n_max, nsp = B * PQP_SPLINE_ROWS * in->k_max;
-    const size_t nb = B * PQP_BOUND_ROWS * in->n_max, nk = out->knots ? B * PQP_NFIELDS * in->n_max : 0;
-    PQP_CUDA(h->err, h->res.grow(h->d_states, ns));
-    PQP_CUDA(h->err, h->res.grow(h->d_bounds, nb));
-    PQP_CUDA(h->err, h->res.grow(h->d_spline, nsp));
-    if (nk) PQP_CUDA(h->err, h->res.grow(h->d_knots, nk));
-    PQP_CUDA(h->err, h->res.grow(h->d_n, B));
-    PQP_CUDA(h->err, h->res.grow(h->d_k, B));
-    PQP_CUDA(h->err, h->res.grow(h->d_nvalid, B));
-    cudaStream_t s = h->stream;
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_states, in->states, ns * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_spline, in->spline, nsp * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_n, in->n, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_k, in->k, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    if (nk) PQP_CUDA(h->err, cudaMemcpyAsync(h->d_knots, out->knots, nk * sizeof(double), cudaMemcpyHostToDevice, s));
-    pqp_bounds_in din = *in;
-    din.states = h->d_states;
-    din.spline = h->d_spline;
-    din.n = h->d_n;
-    din.k = h->d_k;
-    pqp_bounds_out dout;
-    dout.bounds = h->d_bounds;
-    dout.n_valid = h->d_nvalid;
-    dout.knots = nk ? h->d_knots : nullptr;
-    rc = launch(h, &din, &dout, s);
+    return launch(h, in, map_index, out, static_cast<cudaStream_t>(stream));
+}
+
+int pqp_bounds_compute_mapped(pqp_bounds_handle *h, const pqp_bounds_in *in, const int32_t *map_index,
+                              const pqp_bounds_out *out) {
+    const int rc = validate(h, in, out);
     if (rc != PQP_OK) return rc;
-    PQP_CUDA(h->err, cudaMemcpyAsync(out->bounds, h->d_bounds, nb * sizeof(double), cudaMemcpyDeviceToHost, s));
-    PQP_CUDA(h->err, cudaMemcpyAsync(out->n_valid, h->d_nvalid, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    if (nk) PQP_CUDA(h->err, cudaMemcpyAsync(out->knots, h->d_knots, nk * sizeof(double), cudaMemcpyDeviceToHost, s));
-    PQP_CUDA(h->err, cudaStreamSynchronize(s));
-    return PQP_OK;
+    if (!map_index) return fail(h->err, PQP_E_INVALID, "pqp_bounds_compute_mapped: null map_index");
+    return compute_host(h, in, map_index, out);
 }
 
 static int validate_states(pqp_bounds_handle *h, const pqp_states_in *in, const pqp_states_out *out) {
@@ -473,16 +702,7 @@ int pqp_bounds_last_kernel_ms(pqp_bounds_handle *h, float *ms) {
 const char *pqp_bounds_last_error(pqp_bounds_handle *h) { return h ? h->err.c_str() : g_bounds_create_error.c_str(); }
 
 int pqp_bounds_set_map_device(pqp_bounds_handle *h, const pqp_bounds_map *map, void *stream) {
-    const int rc = map ? validate_map(h, map, map->rows, map->cols, map->resolution, map->center_x, map->center_y,
-                                      map->distance, "pqp_bounds_set_map")
-                       : validate_map(h, nullptr, 0, 0, 0.0, 0.0, 0.0, nullptr, "pqp_bounds_set_map");
-    if (rc != PQP_OK) return rc;
-    pqp::DeviceGuard guard_(h->device);
-    const size_t cells = (size_t)map->rows * map->cols;
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_dist, map->distance, cells * sizeof(float), cudaMemcpyDefault,
-                                static_cast<cudaStream_t>(stream)));
-    set_meta(h, map->rows, map->cols, map->resolution, map->center_x, map->center_y);
-    return PQP_OK;
+    return set_map_slot(h, 0, map, static_cast<cudaStream_t>(stream), "pqp_bounds_set_map");
 }
 
 int pqp_bounds_set_map(pqp_bounds_handle *h, const pqp_bounds_map *map) {
@@ -493,45 +713,65 @@ int pqp_bounds_set_map(pqp_bounds_handle *h, const pqp_bounds_map *map) {
     return PQP_OK;
 }
 
+int pqp_bounds_set_map_slot_device(pqp_bounds_handle *h, int32_t slot, const pqp_bounds_map *map, void *stream) {
+    return set_map_slot(h, slot, map, static_cast<cudaStream_t>(stream), "pqp_bounds_set_map_slot");
+}
+
+int pqp_bounds_set_map_slot(pqp_bounds_handle *h, int32_t slot, const pqp_bounds_map *map) {
+    const int rc = pqp_bounds_set_map_slot_device(h, slot, map, h ? h->stream : nullptr);
+    if (rc != PQP_OK) return rc;
+    pqp::DeviceGuard guard_(h->device);
+    PQP_CUDA(h->err, cudaStreamSynchronize(h->stream));
+    return PQP_OK;
+}
+
 int pqp_bounds_set_occupancy_device(pqp_bounds_handle *h, const pqp_occupancy_map *occ, void *stream) {
     const int rc = validate_occupancy(h, occ, "pqp_bounds_set_occupancy_device");
     if (rc != PQP_OK) return rc;
     pqp::DeviceGuard guard_(h->device);
-    const int lrc = launch_edt(h, occ, occ->cells, static_cast<cudaStream_t>(stream));
-    if (lrc != PQP_OK) return lrc;
-    set_meta(h, occ->rows, occ->cols, occ->resolution, occ->center_x, occ->center_y);
-    return PQP_OK;
+    return set_occupancy0(h, occ, occ->cells, static_cast<cudaStream_t>(stream));
 }
 
 int pqp_bounds_set_occupancy(pqp_bounds_handle *h, const pqp_occupancy_map *occ) {
-    const int rc = validate_occupancy(h, occ, "pqp_bounds_set_occupancy");
+    int rc = validate_occupancy(h, occ, "pqp_bounds_set_occupancy");
     if (rc != PQP_OK) return rc;
     pqp::DeviceGuard guard_(h->device);
     const size_t cells = (size_t)occ->rows * occ->cols;
     PQP_CUDA(h->err, cudaMemcpyAsync(h->d_occ, occ->cells, cells, cudaMemcpyHostToDevice, h->stream));
-    const int lrc = launch_edt(h, occ, h->d_occ, h->stream);
-    if (lrc != PQP_OK) return lrc;
-    set_meta(h, occ->rows, occ->cols, occ->resolution, occ->center_x, occ->center_y);
+    rc = set_occupancy0(h, occ, h->d_occ, h->stream);
+    if (rc != PQP_OK) return rc;
+    PQP_CUDA(h->err, cudaStreamSynchronize(h->stream));
+    return PQP_OK;
+}
+
+int pqp_bounds_set_occupancy_slots_device(pqp_bounds_handle *h, int32_t first_slot, const pqp_occupancy_stack *stack,
+                                          void *stream) {
+    const int rc = validate_stack(h, first_slot, stack, "pqp_bounds_set_occupancy_slots_device");
+    if (rc != PQP_OK) return rc;
+    pqp::DeviceGuard guard_(h->device);
+    return set_occupancy_slots(h, first_slot, stack, stack->cells, static_cast<cudaStream_t>(stream));
+}
+
+int pqp_bounds_set_occupancy_slots(pqp_bounds_handle *h, int32_t first_slot, const pqp_occupancy_stack *stack) {
+    int rc = validate_stack(h, first_slot, stack, "pqp_bounds_set_occupancy_slots");
+    if (rc != PQP_OK) return rc;
+    pqp::DeviceGuard guard_(h->device);
+    // the images are consecutive in the slots' staging: count * rows * cols <= count * cap_cells bytes
+    uint8_t *staging = h->d_occ + (size_t)first_slot * h->cap_cells;
+    const size_t bytes = (size_t)stack->count * stack->rows * stack->cols;
+    PQP_CUDA(h->err, cudaMemcpyAsync(staging, stack->cells, bytes, cudaMemcpyHostToDevice, h->stream));
+    rc = set_occupancy_slots(h, first_slot, stack, staging, h->stream);
+    if (rc != PQP_OK) return rc;
     PQP_CUDA(h->err, cudaStreamSynchronize(h->stream));
     return PQP_OK;
 }
 
 int pqp_bounds_get_map(pqp_bounds_handle *h, pqp_bounds_map *meta, float *distance) {
-    if (!h) return PQP_E_INVALID;
-    if (!meta) return fail(h->err, PQP_E_INVALID, "pqp_bounds_get_map: null metadata");
-    pqp::DeviceGuard guard_(h->device);
-    meta->rows = h->map.rows;
-    meta->cols = h->map.cols;
-    meta->resolution = h->map.res;
-    meta->center_x = h->map.cx;
-    meta->center_y = h->map.cy;
-    meta->distance = nullptr;
-    if (distance) {
-        PQP_CUDA(h->err, cudaDeviceSynchronize());
-        PQP_CUDA(h->err, cudaMemcpy(distance, h->d_dist, (size_t)h->map.rows * h->map.cols * sizeof(float),
-                               cudaMemcpyDeviceToHost));
-    }
-    return PQP_OK;
+    return get_map_slot(h, 0, meta, distance, "pqp_bounds_get_map");
+}
+
+int pqp_bounds_get_map_slot(pqp_bounds_handle *h, int32_t slot, pqp_bounds_map *meta, float *distance) {
+    return get_map_slot(h, slot, meta, distance, "pqp_bounds_get_map_slot");
 }
 
 }  // extern "C"

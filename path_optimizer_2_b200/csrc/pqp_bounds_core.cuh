@@ -20,6 +20,14 @@ struct MapView {
     double res, inv_res, half_lx, half_ly, cx, cy;
 };
 
+// The map of path b under a per-path slot index (the *_mapped calls): &table[index[b]], or NULL when the index is
+// outside [0, n_maps). Every map-reading kernel looks its slot up here; the view stays in the table (global memory),
+// so a kernel reads its fields where it uses them rather than holding a copy in registers.
+PQB_HD const MapView *slot_view(const MapView *table, int n_maps, const int32_t *index, int b) {
+    const int32_t i = index[b];
+    return i >= 0 && i < n_maps ? table + i : nullptr;
+}
+
 struct Params {
     double front_length, rear_length, car_width, safety_margin, epsilon;
 };

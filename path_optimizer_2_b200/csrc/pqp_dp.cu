@@ -50,13 +50,33 @@ struct DpArgs {
     int8_t *parent;
     uint8_t *feasible;
     double *nx, *ny, *dis, *ref;
+    const pqb::MapView *table;  // per-path maps: path b reads table[map_index[b]]; map_index NULL: the shared map
+    const int32_t *map_index;
+    int n_maps;
 };
 
-__global__ void __launch_bounds__(kThreads) dp_search_kernel(const pqb::MapView map, const pqdp::Params prm, const DpArgs a) {
+// Three CTAs per SM, as before the per-path map: left free, ptxas gives the kernel 104 registers (two CTAs per SM)
+// once the view may come from the slot table; capped at 80 it keeps its occupancy with a 4-byte spill.
+__global__ void __launch_bounds__(kThreads, 3) dp_search_kernel(const pqb::MapView shared_map, const pqdp::Params prm,
+                                                             const DpArgs a) {
     __shared__ double shd[6 * pqdp::kJMax + 8];
     __shared__ int shi[8];
     const int b = blockIdx.x;
     if (b >= a.batch) return;
+    pqb::MapView map = shared_map;
+    if (a.map_index) {
+        const pqb::MapView *slot = pqb::slot_view(a.table, a.n_maps, a.map_index, b);
+        if (slot) {
+            map = *slot;
+        } else {  // no map to search: nothing sampled, nothing kept
+            if (threadIdx.x == 0) {
+                a.status[b] = PQP_DP_MAP_INDEX;
+                a.n_layers[b] = 0;
+                a.n_out[b] = 0;
+            }
+            return;
+        }
+    }
     pqdp::PathIO io;
     const double *row = a.spline + (size_t)b * PQP_SPLINE_ROWS * a.k_max;
     io.sp.sx = row;
@@ -110,6 +130,7 @@ struct pqp_dp_handle {
     double *d_spline = nullptr, *d_length = nullptr, *d_start = nullptr, *d_layer_s = nullptr, *d_lower = nullptr, *d_upper = nullptr;
     double *d_vehicle_l = nullptr, *d_target_s = nullptr;
     int32_t *d_k = nullptr, *d_status = nullptr, *d_n_layers = nullptr, *d_n_out = nullptr, *d_chosen = nullptr;
+    int32_t *d_map_index = nullptr;  // grown on demand
     float last_ms = 0.0f;
     std::string err;
     pqp::Resources res;  // last member: releasing clears the members above
@@ -118,6 +139,8 @@ struct pqp_dp_handle {
 namespace {
 
 using pqp::fail;
+
+int search_host(pqp_dp_handle *h, const pqp_dp_in *in, const int32_t *map_index, const pqp_dp_out *out);
 
 int validate(pqp_dp_handle *h, const pqp_dp_in *in, const pqp_dp_out *out) {
     if (!h) return PQP_E_INVALID;
@@ -131,8 +154,11 @@ int validate(pqp_dp_handle *h, const pqp_dp_in *in, const pqp_dp_out *out) {
     return PQP_OK;
 }
 
-int launch(pqp_dp_handle *h, const pqp_dp_in *in, const pqp_dp_out *out, cudaStream_t s) {
+int launch(pqp_dp_handle *h, const pqp_dp_in *in, const int32_t *map_index, const pqp_dp_out *out, cudaStream_t s) {
     DpArgs a;
+    a.table = pqb::handle_table(h->owner);
+    a.map_index = map_index;
+    a.n_maps = pqb::handle_map_count(h->owner);
     a.batch = in->batch;
     a.k_max = in->k_max;
     a.layers_max = h->layers_max;
@@ -256,12 +282,43 @@ int pqp_dp_search_device(pqp_dp_handle *h, const pqp_dp_in *in, const pqp_dp_out
     int rc = validate(h, in, out);
     if (rc != PQP_OK) return rc;
     pqp::DeviceGuard guard_(h->device);
-    return launch(h, in, out, static_cast<cudaStream_t>(stream));
+    return launch(h, in, nullptr, out, static_cast<cudaStream_t>(stream));
+}
+
+int pqp_dp_search_mapped_device(pqp_dp_handle *h, const pqp_dp_in *in, const int32_t *map_index, const pqp_dp_out *out,
+                                void *stream) {
+    int rc = validate(h, in, out);
+    if (rc != PQP_OK) return rc;
+    if (!map_index) return fail(h->err, PQP_E_INVALID, "null map_index");
+    pqp::DeviceGuard guard_(h->device);
+    return launch(h, in, map_index, out, static_cast<cudaStream_t>(stream));
 }
 
 int pqp_dp_search(pqp_dp_handle *h, const pqp_dp_in *in, const pqp_dp_out *out) {
-    int rc = validate(h, in, out);
+    const int rc = validate(h, in, out);
     if (rc != PQP_OK) return rc;
+    return search_host(h, in, nullptr, out);
+}
+
+int pqp_dp_search_mapped(pqp_dp_handle *h, const pqp_dp_in *in, const int32_t *map_index, const pqp_dp_out *out) {
+    const int rc = validate(h, in, out);
+    if (rc != PQP_OK) return rc;
+    if (!map_index) return fail(h->err, PQP_E_INVALID, "null map_index");
+    return search_host(h, in, map_index, out);
+}
+
+int pqp_dp_last_kernel_ms(pqp_dp_handle *h, float *ms) {
+    if (!h || !ms) return PQP_E_INVALID;
+    *ms = h->last_ms;
+    return PQP_OK;
+}
+
+}  // extern "C"
+
+namespace {
+
+int search_host(pqp_dp_handle *h, const pqp_dp_in *in, const int32_t *map_index, const pqp_dp_out *out) {
+    int rc = PQP_OK;
     pqp::DeviceGuard guard_(h->device);
     const size_t B = in->batch, nsp = B * PQP_SPLINE_ROWS * in->k_max, Ls = B * h->layers_max, T = Ls * h->J;
     PQP_CUDA(h->err, h->res.grow(h->d_spline, nsp));
@@ -277,7 +334,11 @@ int pqp_dp_search(pqp_dp_handle *h, const pqp_dp_in *in, const pqp_dp_out *out) 
     pqp_dp_in din = {in->batch, in->k_max, h->d_spline, h->d_k, h->d_length, h->d_start};
     pqp_dp_out dout = {h->d_status, h->d_n_layers, h->d_n_out, h->d_layer_s, h->d_lower, h->d_upper, h->d_chosen,
                        h->d_vehicle_l, h->d_target_s, nullptr, nullptr, nullptr};
-    rc = launch(h, &din, &dout, s);
+    if (map_index) {
+        PQP_CUDA(h->err, h->res.grow(h->d_map_index, B));
+        PQP_CUDA(h->err, cudaMemcpyAsync(h->d_map_index, map_index, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    }
+    rc = launch(h, &din, map_index ? h->d_map_index : nullptr, &dout, s);
     if (rc != PQP_OK) return rc;
     PQP_CUDA(h->err, cudaMemcpyAsync(out->status, h->d_status, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
     PQP_CUDA(h->err, cudaMemcpyAsync(out->n_layers, h->d_n_layers, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
@@ -296,10 +357,4 @@ int pqp_dp_search(pqp_dp_handle *h, const pqp_dp_in *in, const pqp_dp_out *out) 
     return PQP_OK;
 }
 
-int pqp_dp_last_kernel_ms(pqp_dp_handle *h, float *ms) {
-    if (!h || !ms) return PQP_E_INVALID;
-    *ms = h->last_ms;
-    return PQP_OK;
-}
-
-}  // extern "C"
+}  // namespace

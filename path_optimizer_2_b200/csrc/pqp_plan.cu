@@ -33,16 +33,30 @@ struct Dims {
     int B, R, P, L, N, in_r;
 };
 
+// per-path maps of a mapped plan call: path b reads table[map_index[b]]; map_index NULL: the shared map
+struct Slots {
+    const pqb::MapView *table;
+    const int32_t *map_index;
+    int n_maps;
+};
+
+// a mapped call's bad index is the path's status whatever else is wrong with it
+__device__ int map_index_status(const Slots &m, int b, int st) {
+    return m.map_index && !pqb::slot_view(m.table, m.n_maps, m.map_index, b) ? pqpl::kMapIndex : st;
+}
+
 // bSpline() up to its sample parameters (pqp_plan_points), one thread per path: the point-count and degree checks,
 // the control polygon's length and degree, and the t accumulation into the path's row of t_all (at most R values)
-__global__ void bspline_prep_kernel(Dims d, int m_max, const double *__restrict__ px, const double *__restrict__ py,
-                                    const int32_t *__restrict__ m, double *t_all, int32_t *raw_r, int32_t *degree,
-                                    int32_t *status) {
+__global__ void bspline_prep_kernel(Dims d, Slots slots, int m_max, const double *__restrict__ px,
+                                    const double *__restrict__ py, const int32_t *__restrict__ m, double *t_all,
+                                    int32_t *raw_r, int32_t *degree, int32_t *status) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= d.B) return;
-    int r, deg;
-    status[b] = pqpl::bspline_prepare(px + (size_t)b * m_max, py + (size_t)b * m_max, m[b], m_max, d.R,
-                                      t_all + (size_t)b * d.R, r, deg);
+    int r = 0, deg = 0, st = map_index_status(slots, b, pqpl::kOk);
+    if (st == pqpl::kOk)
+        st = pqpl::bspline_prepare(px + (size_t)b * m_max, py + (size_t)b * m_max, m[b], m_max, d.R,
+                                   t_all + (size_t)b * d.R, r, deg);
+    status[b] = st;
     raw_r[b] = r;
     degree[b] = deg;
 }
@@ -66,7 +80,8 @@ __global__ void bspline_eval_kernel(Dims d, int m_max, const double *__restrict_
 
 // raw samples -> s_list_ (chord length) into the raw spline rows, sample count of segmentRawReference. `prior`
 // (pqp_plan_points: the B-spline stage's status, possibly `status` itself) keeps an earlier failure; NULL under pqp_plan.
-__global__ void raw_prep_kernel(Dims d, const double *__restrict__ raw_x, const double *__restrict__ raw_y,
+// (pqp_plan_mapped: the map index is checked here, or by bspline_prep_kernel under pqp_plan_points_mapped)
+__global__ void raw_prep_kernel(Dims d, Slots slots, const double *__restrict__ raw_x, const double *__restrict__ raw_y,
                                 const int32_t *__restrict__ r, const double *__restrict__ start, const int32_t *prior,
                                 double *raw_rows, int32_t *raw_k, int32_t *seg_p, int32_t *status, double *start3) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
@@ -76,7 +91,7 @@ __global__ void raw_prep_kernel(Dims d, const double *__restrict__ raw_x, const 
     start3[3 * b + 2] = start[4 * b + 2];
     double *rows = raw_rows + (size_t)b * pqpl::kSplineRows * d.R;
     double *sx = rows, *x = rows + 4 * (size_t)d.R, *y = rows + 8 * (size_t)d.R;
-    int st = prior ? prior[b] : pqpl::kOk, p = 0;
+    int st = prior ? prior[b] : map_index_status(slots, b, pqpl::kOk), p = 0;
     const int rb = st == pqpl::kOk ? r[b] : 0;  // a path that failed before its samples has none to read
     if (st == pqpl::kOk && (rb < 3 || rb > d.R)) {
         st = pqpl::kSplineDegenerate;
@@ -132,14 +147,19 @@ __global__ void segment_kernel(Dims d, const double *__restrict__ raw_rows, cons
 
 // TENSION only: Map::getObstacleDistance at each resampled point (tension_smoother.cpp:166-168), the clearance of the
 // Cartesian tension QP; one thread per (path, point), paths without points (seg_p = 0) skipped
-__global__ void clearance_kernel(Dims d, const pqb::MapView map, const int32_t *__restrict__ seg_p,
+__global__ void clearance_kernel(Dims d, const pqb::MapView map, Slots slots, const int32_t *__restrict__ seg_p,
                                  const double *__restrict__ sx_, const double *__restrict__ sy_, double *clearance) {
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= (long long)d.B * d.P) return;
     const int b = (int)(t / d.P), j = (int)(t % d.P);
     if (j >= seg_p[b]) return;
     const size_t o = (size_t)b * d.P + j;
-    clearance[o] = pqb::map_distance(map, sx_[o], sy_[o]);
+    if (slots.map_index) {
+        const pqb::MapView *m = pqb::slot_view(slots.table, slots.n_maps, slots.map_index, b);
+        if (m) clearance[o] = pqb::map_distance(*m, sx_[o], sy_[o]);
+    } else {
+        clearance[o] = pqb::map_distance(map, sx_[o], sy_[o]);
+    }
 }
 
 __device__ void write_placeholder(double *rows, int stride, int32_t *k, double *length) {
@@ -373,6 +393,7 @@ struct pqp_plan_handle {
     // themselves go to in_x / in_y)
     double *pt_x = nullptr, *pt_y = nullptr, *bs_t = nullptr;
     int32_t *pt_m = nullptr, *raw_r = nullptr, *bs_deg = nullptr;
+    int32_t *in_map_index = nullptr;  // [B] the host mapped calls' slot per path
     double *states = nullptr, *curv = nullptr, *bnd = nullptr, *knots = nullptr, *knots2 = nullptr, *inst = nullptr,
            *ref_xyh = nullptr, *xyh = nullptr;
     int32_t *n_states = nullptr, *total = nullptr, *n_valid = nullptr, *n1 = nullptr, *n2 = nullptr, *p = nullptr;
@@ -504,23 +525,25 @@ int copy_results(pqp_plan_handle *h, const pqp_plan_out *out, int batch, cudaStr
 
 // `pts` (pqp_plan_points, device pointers): bSpline() first writes the samples of those points into `in`'s raw_x,
 // raw_y and r (the handle's in_x, in_y and raw_r) and its status into h->status
+// `map_index` (device, [B]) or NULL: the mapped calls' slot per path; the kernels and stage calls that read a map get it
 int run(pqp_plan_handle *h, const pqp_plan_in *in, const pqp_plan_out *out, cudaStream_t s,
-        const pqp_plan_points_in *pts = nullptr) {
+        const pqp_plan_points_in *pts = nullptr, const int32_t *map_index = nullptr) {
     const int B = in->batch;
     const Dims d{B, h->R, h->P, h->L, h->N, in->r_max};
+    const Slots slots{pqb::handle_table(h->bounds), map_index, pqb::handle_map_count(h->bounds)};
     const pqp_plan_trace *tr = out->trace;
     h->timed = true;
     PQP_CUDA(h->err, cudaEventRecord(h->ev[0], s));
     // ---- reference path smoothing (ReferencePathSmoother::solve) ----
     if (pts) {
-        bspline_prep_kernel<<<blocks_for(B), kThreads, 0, s>>>(d, pts->m_max, pts->ref_x, pts->ref_y, pts->m, h->bs_t,
+        bspline_prep_kernel<<<blocks_for(B), kThreads, 0, s>>>(d, slots, pts->m_max, pts->ref_x, pts->ref_y, pts->m, h->bs_t,
                                                                 h->raw_r, h->bs_deg, h->status);
         PQL_LAUNCH(h);
         bspline_eval_kernel<<<blocks_for((long long)B * h->R), kThreads, 0, s>>>(
             d, pts->m_max, pts->ref_x, pts->ref_y, pts->m, h->bs_t, h->raw_r, h->bs_deg, h->status, h->in_x, h->in_y);
         PQL_LAUNCH(h);
     }
-    raw_prep_kernel<<<blocks_for(B), kThreads, 0, s>>>(d, in->raw_x, in->raw_y, in->r, in->start,
+    raw_prep_kernel<<<blocks_for(B), kThreads, 0, s>>>(d, slots, in->raw_x, in->raw_y, in->r, in->start,
                                                         pts ? h->status : nullptr, h->raw_rows, h->raw_k, h->seg_p,
                                                         h->status, h->start3);
     PQL_LAUNCH(h);
@@ -530,7 +553,7 @@ int run(pqp_plan_handle *h, const pqp_plan_in *in, const pqp_plan_out *out, cuda
                                                                          h->seg[1], h->seg[2], h->seg[3], h->seg[4]);
     PQL_LAUNCH(h);
     if (h->prm.smoothing_method == PQP_PLAN_SMOOTH_TENSION) {
-        clearance_kernel<<<blocks_for((long long)B * h->P), kThreads, 0, s>>>(d, *pqb::handle_map(h->bounds), h->seg_p,
+        clearance_kernel<<<blocks_for((long long)B * h->P), kThreads, 0, s>>>(d, *pqb::handle_map(h->bounds), slots, h->seg_p,
                                                                                h->seg[0], h->seg[1], h->t_clear);
         PQL_LAUNCH(h);
         pqp_cartesian_tension_in ci = {B, h->P, h->seg_p, h->seg[0], h->seg[1], h->seg[2], h->t_clear};
@@ -550,7 +573,10 @@ int run(pqp_plan_handle *h, const pqp_plan_in *in, const pqp_plan_out *out, cuda
         pqp_dp_in di = {B, h->P, h->t_rows, h->tk, h->t_len, h->start3};
         pqp_dp_out dout = {h->dp_status, h->dp_nl, h->dp_nout, h->dp_ls, h->dp_lo, h->dp_up, h->dp_chosen,
                            h->dp_vl, h->dp_ts, nullptr, nullptr, nullptr};
-        PQL_SUB(h, pqp_dp_search_device(h->dp, &di, &dout, s), pqp_dp_last_error, h->dp);
+        if (map_index)
+            PQL_SUB(h, pqp_dp_search_mapped_device(h->dp, &di, map_index, &dout, s), pqp_dp_last_error, h->dp);
+        else
+            PQL_SUB(h, pqp_dp_search_device(h->dp, &di, &dout, s), pqp_dp_last_error, h->dp);
     }
     post_prep_kernel<<<blocks_for(B), kThreads, 0, s>>>(B, h->dp_status, h->dp_nout, h->status, h->post_p);
     PQL_LAUNCH(h);
@@ -580,7 +606,11 @@ int run(pqp_plan_handle *h, const pqp_plan_in *in, const pqp_plan_out *out, cuda
     {
         pqp_bounds_in bi = {B, h->N, h->L, h->states, h->n_states, h->r_rows, h->rk};
         pqp_bounds_out bo = {h->bnd, h->n_valid, h->knots};
-        PQL_SUB(h, pqp_bounds_compute_device(h->bounds, &bi, &bo, s), pqp_bounds_last_error, h->bounds);
+        if (map_index)
+            PQL_SUB(h, pqp_bounds_compute_mapped_device(h->bounds, &bi, map_index, &bo, s), pqp_bounds_last_error,
+                    h->bounds);
+        else
+            PQL_SUB(h, pqp_bounds_compute_device(h->bounds, &bi, &bo, s), pqp_bounds_last_error, h->bounds);
     }
     {
         InstArgs a;
@@ -653,9 +683,10 @@ int run(pqp_plan_handle *h, const pqp_plan_in *in, const pqp_plan_out *out, cuda
 }
 
 // pqp_plan_points(_device) on device points: the samples go to the handle's [B][R] sample storage
-int run_points(pqp_plan_handle *h, const pqp_plan_points_in *pts, const pqp_plan_out *out, cudaStream_t s) {
+int run_points(pqp_plan_handle *h, const pqp_plan_points_in *pts, const pqp_plan_out *out, cudaStream_t s,
+               const int32_t *map_index = nullptr) {
     const pqp_plan_in din = {pts->batch, h->R, h->in_x, h->in_y, h->raw_r, pts->start, pts->target};
-    return run(h, &din, out, s, pts);
+    return run(h, &din, out, s, pts, map_index);
 }
 
 }  // namespace
@@ -681,9 +712,15 @@ const char *pqp_plan_last_error(const pqp_plan_handle *h) { return h ? h->err.c_
 
 int pqp_plan_create(const pqp_bounds_map *map, const pqp_plan_params *params, int32_t r_max, int32_t p_max,
                     int32_t layers_max, int32_t n_max, int32_t batch_max, int32_t device, pqp_plan_handle **out) {
+    return pqp_plan_create_maps(map, map ? 1 : 0, params, r_max, p_max, layers_max, n_max, batch_max, device, out);
+}
+
+int pqp_plan_create_maps(const pqp_bounds_map *maps, int32_t n_maps, const pqp_plan_params *params, int32_t r_max,
+                         int32_t p_max, int32_t layers_max, int32_t n_max, int32_t batch_max, int32_t device,
+                         pqp_plan_handle **out) {
     if (!out) return PQP_E_INVALID;
     *out = nullptr;
-    if (!map) return fail(g_plan_create_error, PQP_E_INVALID, "pqp_plan_create: a map is required");
+    if (!maps || n_maps < 1) return fail(g_plan_create_error, PQP_E_INVALID, "pqp_plan_create: a map is required");
     if (r_max < 3 || p_max < 4 || layers_max < 4 || n_max < 2 || n_max > 511 || batch_max < 1)
         return fail(g_plan_create_error, PQP_E_INVALID,
                     "pqp_plan_create: r_max >= 3, p_max >= 4, layers_max >= 4, 2 <= n_max <= 511, batch_max >= 1");
@@ -707,7 +744,7 @@ int pqp_plan_create(const pqp_bounds_map *map, const pqp_plan_params *params, in
     std::string &err = g_plan_create_error;
     pqp::DeviceGuard guard_(device);
     const int rc = [&]() -> int {
-        PQL_SUB_CREATE(pqp_bounds_create(map, &h->prm.bounds, device, &h->bounds), pqp_bounds_last_error);
+        PQL_SUB_CREATE(pqp_bounds_create_maps(maps, n_maps, &h->prm.bounds, device, &h->bounds), pqp_bounds_last_error);
         PQL_SUB_CREATE(pqp_dp_create(h->bounds, &h->prm.dp, layers_max, batch_max, &h->dp), pqp_dp_last_error);
         PQL_SUB_CREATE(pqp_smoother_create(&h->prm.smoother, p_max, batch_max, device, &h->tension), pqp_smoother_last_error);
         PQL_SUB_CREATE(pqp_smoother_create(&h->prm.smoother, layers_max, batch_max, device, &h->post), pqp_smoother_last_error);
@@ -790,6 +827,7 @@ int pqp_plan_create(const pqp_bounds_map *map, const pqp_plan_params *params, in
         PQP_CUDA(err, r.alloc(h->bs_t, B * R));
         PQP_CUDA(err, r.alloc(h->raw_r, B));
         PQP_CUDA(err, r.alloc(h->bs_deg, B));
+        PQP_CUDA(err, r.alloc(h->in_map_index, B));
         // spline rows are zero beyond each path's k, so every row read past the end of a fit is defined
         PQP_CUDA(err, cudaMemset(h->raw_rows, 0, B * S * R * sizeof(double)));
         PQP_CUDA(err, cudaMemset(h->t_rows, 0, B * S * P * sizeof(double)));
@@ -871,11 +909,115 @@ int pqp_plan_points(pqp_plan_handle *h, const pqp_plan_points_in *in, const pqp_
     return copy_results(h, out, in->batch, s);
 }
 
+int pqp_plan_mapped_device(pqp_plan_handle *h, const pqp_plan_in *in, const int32_t *map_index, const pqp_plan_out *out,
+                           void *stream) {
+    int rc = validate(h, in, out);
+    if (rc != PQP_OK) return rc;
+    if (!map_index) return fail(h->err, PQP_E_INVALID, "null map_index");
+    pqp::DeviceGuard guard_(h->device);
+    return run(h, in, out, static_cast<cudaStream_t>(stream), nullptr, map_index);
+}
+
+int pqp_plan_mapped(pqp_plan_handle *h, const pqp_plan_in *in, const int32_t *map_index, const pqp_plan_out *out) {
+    int rc = validate(h, in, out);
+    if (rc != PQP_OK) return rc;
+    if (!map_index) return fail(h->err, PQP_E_INVALID, "null map_index");
+    pqp::DeviceGuard guard_(h->device);
+    cudaStream_t s = h->stream;
+    const size_t B = in->batch, R = in->r_max;
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_x, in->raw_x, B * R * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_y, in->raw_y, B * R * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_r, in->r, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_start, in->start, B * 4 * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_target, in->target, B * 3 * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_map_index, map_index, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    const pqp_plan_in din = {in->batch, in->r_max, h->in_x, h->in_y, h->in_r, h->in_start, h->in_target};
+    const pqp_plan_out dout = {h->o_status, h->o_n, h->o_path, h->o_cost, h->o_iters, out->trace};
+    rc = run(h, &din, &dout, s, nullptr, h->in_map_index);
+    if (rc != PQP_OK) return rc;
+    return copy_results(h, out, in->batch, s);
+}
+
+int pqp_plan_points_mapped_device(pqp_plan_handle *h, const pqp_plan_points_in *in, const int32_t *map_index,
+                                  const pqp_plan_out *out, void *stream) {
+    int rc = validate_points(h, in, out);
+    if (rc != PQP_OK) return rc;
+    if (!map_index) return fail(h->err, PQP_E_INVALID, "null map_index");
+    pqp::DeviceGuard guard_(h->device);
+    return run_points(h, in, out, static_cast<cudaStream_t>(stream), map_index);
+}
+
+int pqp_plan_points_mapped(pqp_plan_handle *h, const pqp_plan_points_in *in, const int32_t *map_index,
+                           const pqp_plan_out *out) {
+    int rc = validate_points(h, in, out);
+    if (rc != PQP_OK) return rc;
+    if (!map_index) return fail(h->err, PQP_E_INVALID, "null map_index");
+    pqp::DeviceGuard guard_(h->device);
+    cudaStream_t s = h->stream;
+    const size_t B = in->batch, M = in->m_max;
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->pt_x, in->ref_x, B * M * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->pt_y, in->ref_y, B * M * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->pt_m, in->m, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_start, in->start, B * 4 * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_target, in->target, B * 3 * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_map_index, map_index, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    const pqp_plan_points_in din = {in->batch, in->m_max, h->pt_x, h->pt_y, h->pt_m, h->in_start, h->in_target};
+    const pqp_plan_out dout = {h->o_status, h->o_n, h->o_path, h->o_cost, h->o_iters, out->trace};
+    rc = run_points(h, &din, &dout, s, h->in_map_index);
+    if (rc != PQP_OK) return rc;
+    return copy_results(h, out, in->batch, s);
+}
+
 int pqp_plan_set_map_device(pqp_plan_handle *h, const pqp_bounds_map *map, void *stream) {
     if (!h) return PQP_E_INVALID;
     PQL_SUB(h, pqp_bounds_set_map_device(h->bounds, map, stream), pqp_bounds_last_error, h->bounds);
+    h->launches += 1;  // the slot's table entry
     return PQP_OK;
 }
+
+int pqp_plan_set_map_slot_device(pqp_plan_handle *h, int32_t slot, const pqp_bounds_map *map, void *stream) {
+    if (!h) return PQP_E_INVALID;
+    PQL_SUB(h, pqp_bounds_set_map_slot_device(h->bounds, slot, map, stream), pqp_bounds_last_error, h->bounds);
+    h->launches += 1;
+    return PQP_OK;
+}
+
+int pqp_plan_set_map_slot(pqp_plan_handle *h, int32_t slot, const pqp_bounds_map *map) {
+    if (!h) return PQP_E_INVALID;
+    PQL_SUB(h, pqp_plan_set_map_slot_device(h, slot, map, h->stream), pqp_plan_last_error, h);
+    pqp::DeviceGuard guard_(h->device);
+    PQP_CUDA(h->err, cudaStreamSynchronize(h->stream));
+    return PQP_OK;
+}
+
+// column pass, row pass and the table entries, PQP_MAP_TABLE_CHUNK per launch
+static long long occupancy_slots_launches(const pqp_occupancy_stack *st) {
+    return 2 + (st->count + PQP_MAP_TABLE_CHUNK - 1) / PQP_MAP_TABLE_CHUNK;
+}
+
+int pqp_plan_set_occupancy_slots_device(pqp_plan_handle *h, int32_t first_slot, const pqp_occupancy_stack *stack,
+                                        void *stream) {
+    if (!h) return PQP_E_INVALID;
+    PQL_SUB(h, pqp_bounds_set_occupancy_slots_device(h->bounds, first_slot, stack, stream), pqp_bounds_last_error,
+            h->bounds);
+    h->launches += occupancy_slots_launches(stack);
+    return PQP_OK;
+}
+
+int pqp_plan_set_occupancy_slots(pqp_plan_handle *h, int32_t first_slot, const pqp_occupancy_stack *stack) {
+    if (!h) return PQP_E_INVALID;
+    PQL_SUB(h, pqp_bounds_set_occupancy_slots(h->bounds, first_slot, stack), pqp_bounds_last_error, h->bounds);
+    h->launches += occupancy_slots_launches(stack);
+    return PQP_OK;
+}
+
+int pqp_plan_get_map_slot(pqp_plan_handle *h, int32_t slot, pqp_bounds_map *meta, float *distance) {
+    if (!h) return PQP_E_INVALID;
+    PQL_SUB(h, pqp_bounds_get_map_slot(h->bounds, slot, meta, distance), pqp_bounds_last_error, h->bounds);
+    return PQP_OK;
+}
+
+int32_t pqp_plan_map_count(const pqp_plan_handle *h) { return h ? pqp_bounds_map_count(h->bounds) : 0; }
 
 int pqp_plan_set_map(pqp_plan_handle *h, const pqp_bounds_map *map) {
     if (!h) return PQP_E_INVALID;

@@ -18,7 +18,8 @@ namespace pqpl {
 enum {
     kOk = 0, kSplineDegenerate = 1, kTooManyPoints = 2, kTensionFailed = 3, kDpVehicleFar = 4, kPostTooShort = 5,
     kPostFailed = 6, kEmptyReference = 7, kInitHeading = 8, kTooManyKnots = 9, kBlockedAtStart = 10,
-    kPreSolveFailed = 11, kSolveFailed = 12, kPointCount = 13, kBsplineDegree = 14
+    kPreSolveFailed = 11, kSolveFailed = 12, kPointCount = 13, kBsplineDegree = 14,
+    kMapIndex = 15
 };
 
 constexpr int kSplineRows = 9;  // PQP_SPLINE_ROWS

@@ -8,8 +8,9 @@ import numpy as np
 from . import solver
 
 EXPORTED_SYMBOLS = ["pqp_dp_default_params", "pqp_dp_create", "pqp_dp_destroy", "pqp_dp_lateral_count", "pqp_dp_search",
-                    "pqp_dp_search_device", "pqp_dp_last_kernel_ms", "pqp_dp_last_error"]
-DP_OK, DP_VEHICLE_FAR, DP_TOO_MANY_LAYERS = 1, 0, -1
+                    "pqp_dp_search_device", "pqp_dp_last_kernel_ms", "pqp_dp_last_error", "pqp_dp_search_mapped",
+                    "pqp_dp_search_mapped_device"]
+DP_OK, DP_VEHICLE_FAR, DP_TOO_MANY_LAYERS, DP_MAP_INDEX = 1, 0, -1, -2
 
 
 class DpParams(C.Structure):
@@ -40,6 +41,8 @@ def _lib():
         L.pqp_dp_lateral_count.restype = C.c_int32
         L.pqp_dp_search.argtypes = [vp, C.POINTER(DpIn), C.POINTER(DpOut)]
         L.pqp_dp_search_device.argtypes = [vp, C.POINTER(DpIn), C.POINTER(DpOut), vp]
+        L.pqp_dp_search_mapped.argtypes = [vp, C.POINTER(DpIn), vp, C.POINTER(DpOut)]
+        L.pqp_dp_search_mapped_device.argtypes = [vp, C.POINTER(DpIn), vp, C.POINTER(DpOut), vp]
         L.pqp_dp_last_kernel_ms.argtypes = [vp, C.POINTER(C.c_float)]
         L.pqp_dp_last_error.argtypes = [vp]
         L.pqp_dp_last_error.restype = C.c_char_p
@@ -95,7 +98,8 @@ class DpSearch:
         if rc:
             raise solver.PqpError(rc, (self.L.pqp_dp_last_error(self.h) or b"").decode())
 
-    def search(self, spline, k, length, start, tables=True) -> DpResult:
+    def search(self, spline, k, length, start, tables=True, map_index=None) -> DpResult:
+        """`map_index` [b]: path b on map slot map_index[b] of the owner (out of range: status DP_MAP_INDEX)."""
         spline = np.ascontiguousarray(spline, dtype=np.float64)
         k = np.ascontiguousarray(k, dtype=np.int32)
         length = np.ascontiguousarray(length, dtype=np.float64)
@@ -104,7 +108,12 @@ class DpSearch:
         res = DpResult(B, self.layers_max, self.lateral, tables)
         din = DpIn(B, k_max, spline.ctypes.data, k.ctypes.data, length.ctypes.data, start.ctypes.data)
         dout = res.as_struct()
-        self._check(self.L.pqp_dp_search(self.h, C.byref(din), C.byref(dout)))
+        if map_index is None:
+            self._check(self.L.pqp_dp_search(self.h, C.byref(din), C.byref(dout)))
+        else:
+            idx = np.ascontiguousarray(map_index, dtype=np.int32)
+            assert idx.shape == (B,)
+            self._check(self.L.pqp_dp_search_mapped(self.h, C.byref(din), idx.ctypes.data, C.byref(dout)))
         return res
 
     def search_device(self, din: DpIn, dout: DpOut, stream=0):

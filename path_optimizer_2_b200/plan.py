@@ -11,15 +11,26 @@ from . import abi, bounds, dp, smoother, solver
 EXPORTED_SYMBOLS = ["pqp_plan_default_params", "pqp_plan_create", "pqp_plan_destroy", "pqp_plan", "pqp_plan_device",
                     "pqp_plan_points", "pqp_plan_points_device", "pqp_plan_last_stage_ms", "pqp_plan_launch_count",
                     "pqp_plan_last_error", "pqp_plan_set_map", "pqp_plan_set_map_device", "pqp_plan_set_occupancy",
-                    "pqp_plan_set_occupancy_device", "pqp_plan_get_map"]
+                    "pqp_plan_set_occupancy_device", "pqp_plan_get_map", "pqp_plan_create_maps", "pqp_plan_mapped",
+                    "pqp_plan_mapped_device", "pqp_plan_points_mapped", "pqp_plan_points_mapped_device",
+                    "pqp_plan_set_map_slot", "pqp_plan_set_map_slot_device", "pqp_plan_set_occupancy_slots",
+                    "pqp_plan_set_occupancy_slots_device", "pqp_plan_get_map_slot", "pqp_plan_map_count"]
 # kernel launches of one set_occupancy call (the distance transform's column and row pass)
 OCCUPANCY_LAUNCHES = 2
+# of one set_map / set_map_slot call (the slot's table entry; the layer is a copy)
+SET_MAP_LAUNCHES = 1
+
+
+def occupancy_slots_launches(count):
+    """kernel launches of one set_occupancy_slots call of `count` images: column pass, row pass, table entries."""
+    return 2 + -(-int(count) // bounds.MAP_TABLE_CHUNK)
 
 STATUS_NAMES = ("OK", "SPLINE_DEGENERATE", "TOO_MANY_POINTS", "TENSION_FAILED", "DP_VEHICLE_FAR", "POST_TOO_SHORT",
                 "POST_FAILED", "EMPTY_REFERENCE", "INIT_HEADING", "TOO_MANY_KNOTS", "BLOCKED_AT_START",
-                "PRE_SOLVE_FAILED", "SOLVE_FAILED", "POINT_COUNT", "BSPLINE_DEGREE")
+                "PRE_SOLVE_FAILED", "SOLVE_FAILED", "POINT_COUNT", "BSPLINE_DEGREE", "MAP_INDEX")
 (OK, SPLINE_DEGENERATE, TOO_MANY_POINTS, TENSION_FAILED, DP_VEHICLE_FAR, POST_TOO_SHORT, POST_FAILED, EMPTY_REFERENCE,
- INIT_HEADING, TOO_MANY_KNOTS, BLOCKED_AT_START, PRE_SOLVE_FAILED, SOLVE_FAILED, POINT_COUNT, BSPLINE_DEGREE) = range(15)
+ INIT_HEADING, TOO_MANY_KNOTS, BLOCKED_AT_START, PRE_SOLVE_FAILED, SOLVE_FAILED, POINT_COUNT, BSPLINE_DEGREE,
+ MAP_INDEX) = range(16)
 PATH_ROWS = ("x", "y", "heading", "k", "d_k", "l", "d_heading")
 STAGES = ("smoothing", "segmentation", "optimisation", "total")
 # PlanParams.smoothing_method: the reference's --smoothing_method
@@ -108,6 +119,19 @@ def _lib():
         L.pqp_plan_set_occupancy.argtypes = [vp, C.POINTER(bounds.OccupancyMap)]
         L.pqp_plan_set_occupancy_device.argtypes = [vp, C.POINTER(bounds.OccupancyMap), vp]
         L.pqp_plan_get_map.argtypes = [vp, C.POINTER(bounds.BoundsMap), vp]
+        L.pqp_plan_create_maps.argtypes = [C.POINTER(bounds.BoundsMap), C.c_int32, C.POINTER(PlanParams)] + \
+            [C.c_int32] * 6 + [C.POINTER(vp)]
+        L.pqp_plan_mapped.argtypes = [vp, C.POINTER(PlanIn), vp, C.POINTER(PlanOut)]
+        L.pqp_plan_mapped_device.argtypes = [vp, C.POINTER(PlanIn), vp, C.POINTER(PlanOut), vp]
+        L.pqp_plan_points_mapped.argtypes = [vp, C.POINTER(PlanPointsIn), vp, C.POINTER(PlanOut)]
+        L.pqp_plan_points_mapped_device.argtypes = [vp, C.POINTER(PlanPointsIn), vp, C.POINTER(PlanOut), vp]
+        L.pqp_plan_set_map_slot.argtypes = [vp, C.c_int32, C.POINTER(bounds.BoundsMap)]
+        L.pqp_plan_set_map_slot_device.argtypes = [vp, C.c_int32, C.POINTER(bounds.BoundsMap), vp]
+        L.pqp_plan_set_occupancy_slots.argtypes = [vp, C.c_int32, C.POINTER(bounds.OccupancyStack)]
+        L.pqp_plan_set_occupancy_slots_device.argtypes = [vp, C.c_int32, C.POINTER(bounds.OccupancyStack), vp]
+        L.pqp_plan_get_map_slot.argtypes = [vp, C.c_int32, C.POINTER(bounds.BoundsMap), vp]
+        L.pqp_plan_map_count.argtypes = [vp]
+        L.pqp_plan_map_count.restype = C.c_int32
         L._plan_declared = True
     return L
 
@@ -168,6 +192,31 @@ class Planner:
             raise solver.PqpError(rc, (self.L.pqp_plan_last_error(None) or b"").decode())
         self.h = h
 
+    @classmethod
+    def from_maps(cls, dists, resolutions, *, centers=None, r_max, p_max, layers_max=64, n_max=256, batch_max,
+                  params=None, device=0):
+        """A planner with one map slot per float32 layer in `dists` (each slot as large as the largest layer);
+        `resolutions` is one value or one per map, `centers` [(x, y)] per map (default: the origin). The calls with a
+        `map_index` plan path b on slot map_index[b]; the others use slot 0."""
+        self = cls.__new__(cls)
+        self.L = _lib()
+        arr, self._layers = bounds.map_list(dists, resolutions, centers)
+        self.dist = self._layers[0]
+        self.params = params if params is not None else default_params()
+        self.r_max, self.p_max, self.layers_max, self.n_max = int(r_max), int(p_max), int(layers_max), int(n_max)
+        self.batch_max, self.device = int(batch_max), int(device)
+        h = C.c_void_p()
+        rc = self.L.pqp_plan_create_maps(arr, len(self._layers), C.byref(self.params), self.r_max, self.p_max,
+                                         self.layers_max, self.n_max, self.batch_max, self.device, C.byref(h))
+        if rc:
+            raise solver.PqpError(rc, (self.L.pqp_plan_last_error(None) or b"").decode())
+        self.h = h
+        return self
+
+    @property
+    def n_maps(self):
+        return int(self.L.pqp_plan_map_count(self.h))
+
     def close(self):
         if getattr(self, "h", None):
             self.L.pqp_plan_destroy(self.h)
@@ -183,7 +232,7 @@ class Planner:
     def dims(self):
         return self.p_max, self.layers_max, self.n_max, self.r_max
 
-    def _host_call(self, fn, make_in, xs, ys, start, target, trace, stride, clip=False):
+    def _host_call(self, fn, make_in, xs, ys, start, target, trace, stride, clip=False, mapped_fn=None, map_index=None):
         B = len(xs)
         cnt = np.array([len(v) for v in xs], dtype=np.int32)
         rx, ry = np.zeros((B, stride)), np.zeros((B, stride))
@@ -200,35 +249,43 @@ class Planner:
             tr = _trace_struct(res.trace, lambda a: a.ctypes.data)
         pout = PlanOut(res.status.ctypes.data, res.n.ctypes.data, res.path.ctypes.data, res.cost.ctypes.data,
                        res.iters.ctypes.data, C.pointer(tr) if tr is not None else None)
-        self._check(fn(self.h, C.byref(pin), C.byref(pout)))
+        if map_index is None:
+            self._check(fn(self.h, C.byref(pin), C.byref(pout)))
+        else:
+            idx = bounds.index_array(map_index, B)
+            self._check(mapped_fn(self.h, C.byref(pin), idx.ctypes.data, C.byref(pout)))
         return res
 
-    def plan(self, raw_x, raw_y, start, target, trace=False) -> PlanResult:
+    def plan(self, raw_x, raw_y, start, target, trace=False, map_index=None) -> PlanResult:
         """Host call. raw_x, raw_y: lists of per-path sample arrays (x_list_, y_list_ of bSpline()); start [B][4]
-        (x, y, heading, k); target [B][3] (x, y, heading)."""
-        return self._host_call(self.L.pqp_plan, PlanIn, raw_x, raw_y, start, target, trace, self.r_max)
+        (x, y, heading, k); target [B][3] (x, y, heading). `map_index` [B]: path b on map slot map_index[b] (None:
+        every path on slot 0, the unmapped call)."""
+        return self._host_call(self.L.pqp_plan, PlanIn, raw_x, raw_y, start, target, trace, self.r_max,
+                               mapped_fn=self.L.pqp_plan_mapped, map_index=map_index)
 
-    def plan_points(self, ref_x, ref_y, start, target, trace=False, m_max=None) -> PlanResult:
+    def plan_points(self, ref_x, ref_y, start, target, trace=False, m_max=None, map_index=None) -> PlanResult:
         """Host call from the reference points (PathOptimizer::solve's reference_points): ref_x, ref_y are lists of
         per-path point arrays; bSpline() runs on the GPU. `m_max` (default r_max) is the row stride; a path with more
         points than that is reported as POINT_COUNT. start, target as `plan`."""
         m_max = self.r_max if m_max is None else int(m_max)
         return self._host_call(self.L.pqp_plan_points, PlanPointsIn, ref_x, ref_y, start, target, trace, m_max,
-                               clip=True)
+                               clip=True, mapped_fn=self.L.pqp_plan_points_mapped, map_index=map_index)
 
-    def plan_device(self, raw_x, raw_y, r, start, target, *, trace=False, stream=None):
+    def plan_device(self, raw_x, raw_y, r, start, target, *, trace=False, stream=None, map_index=None):
         """Device call on torch tensors (cuda, contiguous): raw_x / raw_y float64 [B][r_max'], r int32 [B], start
         float64 [B][4], target float64 [B][3]. Asynchronous on `stream` (default: the current stream); returns a dict of
-        output tensors (status, n, path, cost, iters, and `trace`: a dict of tensors when requested)."""
-        return self._device_call(self.L.pqp_plan_device, PlanIn, raw_x, raw_y, r, start, target, trace, stream)
+        output tensors (status, n, path, cost, iters, and `trace`: a dict of tensors when requested). `map_index`: an
+        int32 CUDA tensor [B], path b on map slot map_index[b]."""
+        return self._device_call(self.L.pqp_plan_device, PlanIn, raw_x, raw_y, r, start, target, trace, stream,
+                                 self.L.pqp_plan_mapped_device, map_index)
 
-    def plan_points_device(self, ref_x, ref_y, m, start, target, *, trace=False, stream=None):
+    def plan_points_device(self, ref_x, ref_y, m, start, target, *, trace=False, stream=None, map_index=None):
         """Device call from the reference points on torch tensors (cuda, contiguous): ref_x / ref_y float64
         [B][m_max], m int32 [B], start float64 [B][4], target float64 [B][3]; m_max <= r_max. As `plan_device`."""
         return self._device_call(self.L.pqp_plan_points_device, PlanPointsIn, ref_x, ref_y, m, start, target, trace,
-                                 stream)
+                                 stream, self.L.pqp_plan_points_mapped_device, map_index)
 
-    def _device_call(self, fn, make_in, xs, ys, cnt, start, target, trace, stream):
+    def _device_call(self, fn, make_in, xs, ys, cnt, start, target, trace, stream, mapped_fn=None, map_index=None):
         import torch
         B = int(xs.shape[0])
         dev = xs.device
@@ -248,20 +305,52 @@ class Planner:
         pout = PlanOut(out["status"].data_ptr(), out["n"].data_ptr(), out["path"].data_ptr(), out["cost"].data_ptr(),
                        out["iters"].data_ptr(), C.pointer(tr) if tr is not None else None)
         s = stream if stream is not None else torch.cuda.current_stream(dev)
-        self._check(fn(self.h, C.byref(pin), C.byref(pout), C.c_void_p(s.cuda_stream)))
+        if map_index is None:
+            self._check(fn(self.h, C.byref(pin), C.byref(pout), C.c_void_p(s.cuda_stream)))
+        else:
+            assert map_index.is_cuda and map_index.is_contiguous() and map_index.dtype == torch.int32
+            assert tuple(map_index.shape) == (B,)
+            self._check(mapped_fn(self.h, C.byref(pin), map_index.data_ptr(), C.byref(pout), C.c_void_p(s.cuda_stream)))
         return out
 
-    def set_map(self, dist, resolution, center=(0.0, 0.0)):
-        """Replace the map with a float32 distance layer [rows, cols] (host, synchronous); rows * cols may not exceed
-        the cells of the map the planner was created with."""
+    def set_map(self, dist, resolution, center=(0.0, 0.0), slot=0):
+        """Replace the map (of `slot`) with a float32 distance layer [rows, cols] (host, synchronous); rows * cols may
+        not exceed the cells of a slot."""
         m, _keep = bounds.distance_map(dist, resolution, center)
-        self._check(self.L.pqp_plan_set_map(self.h, C.byref(m)))
+        if slot:
+            self._check(self.L.pqp_plan_set_map_slot(self.h, int(slot), C.byref(m)))
+        else:
+            self._check(self.L.pqp_plan_set_map(self.h, C.byref(m)))
 
-    def set_occupancy(self, img, resolution, center=(0.0, 0.0), obstacle_max=0):
-        """Replace the map with the exact Euclidean distance transform, computed on the GPU, of a uint8 image
-        [rows, cols] (host, synchronous): cells <= obstacle_max are obstacles (0: the demo's zero pixels)."""
+    def set_occupancy(self, img, resolution, center=(0.0, 0.0), obstacle_max=0, slot=0):
+        """Replace the map (of `slot`) with the exact Euclidean distance transform, computed on the GPU, of a uint8
+        image [rows, cols] (host, synchronous): cells <= obstacle_max are obstacles (0: the demo's zero pixels)."""
+        if slot:
+            img = np.ascontiguousarray(img, dtype=np.uint8)
+            self.set_occupancy_slots(img[None], resolution, [center], obstacle_max, first_slot=slot)
+            return
         m, _keep = bounds.occupancy_map(img, resolution, center, obstacle_max)
         self._check(self.L.pqp_plan_set_occupancy(self.h, C.byref(m)))
+
+    def set_occupancy_slots(self, imgs, resolution, centers=None, obstacle_max=0, *, first_slot=0):
+        """The exact distance transforms of a uint8 stack [count, rows, cols] into slots first_slot .. + count - 1,
+        in one pair of launches (host, synchronous); `centers` [count, 2] (default: the origin)."""
+        imgs = np.ascontiguousarray(imgs, dtype=np.uint8)
+        assert imgs.ndim == 3
+        st, _keep = bounds.occupancy_stack(imgs.ctypes.data, imgs.shape, resolution, centers, obstacle_max)
+        self._check(self.L.pqp_plan_set_occupancy_slots(self.h, int(first_slot), C.byref(st)))
+
+    def set_occupancy_slots_device(self, imgs, resolution, centers=None, obstacle_max=0, *, first_slot=0,
+                                   stream=None):
+        """As `set_occupancy_slots` from a torch uint8 CUDA tensor [count, rows, cols], asynchronous on `stream`
+        (default: the current stream): plans enqueued before see the old slots, plans enqueued after the new ones. The
+        tensor must stay alive until the stream has run the transform."""
+        import torch
+        assert imgs.is_cuda and imgs.is_contiguous() and imgs.dtype == torch.uint8 and imgs.dim() == 3
+        st, _keep = bounds.occupancy_stack(imgs.data_ptr(), imgs.shape, resolution, centers, obstacle_max)
+        s = stream if stream is not None else torch.cuda.current_stream(imgs.device)
+        self._check(self.L.pqp_plan_set_occupancy_slots_device(self.h, int(first_slot), C.byref(st),
+                                                               C.c_void_p(s.cuda_stream)))
 
     def set_map_device(self, dist, resolution, center=(0.0, 0.0), *, stream=None):
         """As `set_map` from a torch float32 CUDA tensor [rows, cols], asynchronous on `stream` (default: the
@@ -283,10 +372,10 @@ class Planner:
         s = stream if stream is not None else torch.cuda.current_stream(img.device)
         self._check(self.L.pqp_plan_set_occupancy_device(self.h, C.byref(m), C.c_void_p(s.cuda_stream)))
 
-    def get_map(self):
-        """-> (float32 distance layer [rows, cols], resolution, (center_x, center_y)) of the current map; waits for
-        the device."""
-        return bounds.get_map(self.L.pqp_plan_get_map, self.h, self._check)
+    def get_map(self, slot=0):
+        """-> (float32 distance layer [rows, cols], resolution, (center_x, center_y)) of the current map (of `slot`);
+        waits for the device."""
+        return bounds.get_map(self.L.pqp_plan_get_map, self.h, self._check, self.L.pqp_plan_get_map_slot, slot)
 
     @property
     def last_stage_ms(self):
