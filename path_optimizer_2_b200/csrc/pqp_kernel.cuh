@@ -297,7 +297,7 @@ struct SmemStore {
     real *sm;
     int lane;
     // cyclic-reduction levels unrolled? Several warps share a scheduler and the hot loop should stay small: unrolled
-    // only at C <= 2 in FP32, where the levels are a large share of the work
+    // only at C <= 2 in FP32, where the levels are a large share of the work (QpWarp widens this for the increment form)
     static constexpr bool kUnrollCr = C <= 2 && sizeof(real) == 4;
     PQP_DEV SmemStore(real *s, int l) : sm(s), lane(l) {}
     PQP_DEV real ld(int f, int k) const { return sm[(((f >> 2) * C + k) * 32 + lane) * 4 + (f & 3)]; }
@@ -334,7 +334,8 @@ struct SmemStore {
 //    they make a hot loop of tens of KB that thrashes the instruction cache;
 //  * the substitution sweeps are fully unrolled: rolled, much of their instruction stream is register copies of the
 //    prefetched factor and address arithmetic;
-//  * the cyclic-reduction levels are unrolled per storage policy (Store::kUnrollCr).
+//  * the cyclic-reduction levels are unrolled per storage policy and form (QpWarp::kUnrollCr);
+//  * the hot stage-update loop of the increment form is unrolled by two (admm_update_incr<false, false>).
 #define PQP_ROLL _Pragma("unroll 1")
 #define PQP_SWEEP_UNROLL _Pragma("unroll")
 #define PQP_UPDATE_UNROLL _Pragma("unroll 1")
@@ -349,6 +350,11 @@ template <int C, typename real, typename Store = SmemStore<C, real>, bool Incr =
 struct QpWarp {
     typedef typename Vec4T<real>::type Vec4;
     typedef StagePredT<real> StagePred;
+    // cyclic-reduction levels unrolled (constant shuffle distances and lane masks, no loop bookkeeping between the
+    // dependent levels): as the storage policy asks, and in the FP32 increment form up to C = 8, where at most three
+    // QPs fit on an SM and each warp has a scheduler to itself (DESIGN §10: 5 % of a C = 8 launch). The textbook form
+    // keeps the rolled levels: unrolled, its persistent and one-CTA-per-instance builds round differently.
+    static constexpr bool kUnrollCr = Store::kUnrollCr || (Incr && C <= 8 && sizeof(real) == 4);
     const KernelArgs &ka;
     Store store;
     const int lane, qp;
@@ -1075,8 +1081,8 @@ struct QpWarp {
             bs[r] = bk[r] - fr;
         }
         // cyclic reduction over the 32 separators: 5 forward levels, 3x3 solve, 5 backward levels; unrolled with
-        // constant shuffle distances and lane masks where the storage policy asks for it (Store::kUnrollCr)
-        if (Store::kUnrollCr) {
+        // constant shuffle distances and lane masks where kUnrollCr asks for it
+        if (kUnrollCr) {
 #pragma unroll
             for (int t = 0; t < 5; ++t) cr_forward_level(t, bs);
         } else {
@@ -1089,7 +1095,7 @@ struct QpWarp {
             ts[r] = crAinv[SI(r, 0)] * bs[0] + crAinv[SI(r, 1)] * bs[1] + crAinv[SI(r, 2)] * bs[2];
             xs[r] = ts[r];
         }
-        if (Store::kUnrollCr) {
+        if (kUnrollCr) {
 #pragma unroll
             for (int t = 4; t >= 0; --t) cr_backward_level(t, ts, xs);
         } else {
@@ -1658,7 +1664,11 @@ struct QpWarp {
         store.ld4_nowait_next(GBV, 0, dwv);
         store.template ld_run_nowait_cur<GA0, 11>(0, loaded);
         store.wait_ld();
-        PQP_UPDATE_UNROLL
+        // the hot instantiation (no check, not the first iteration) is unrolled by two: the prefetched batch then
+        // lands in registers the next stage reads directly instead of being copied at every trip (44 + 4 moves),
+        // for one more copy of the stage body (DESIGN §10); the check and first-iteration loops stay rolled
+        constexpr int kUnroll = (!kCheck && !kMaybeFirst) ? 2 : 1;
+#pragma unroll (kUnroll)
         for (int k = 0; k < C; ++k) {
             store.seek(k);
             const StagePred sp = pred(k);
