@@ -90,18 +90,6 @@ def occupancy_map(img, resolution, center, obstacle_max):
                         img.ctypes.data, int(obstacle_max)), img
 
 
-def get_map(fn, h, check, slot_fn=None, slot=0):
-    """`fn`(h, meta, layer) read-back -> (float32 layer [rows, cols], resolution, (center_x, center_y)); a slot other
-    than 0 is read with `slot_fn`(h, slot, meta, layer)."""
-    if slot:
-        fn = lambda h_, m_, d_: slot_fn(h_, int(slot), m_, d_)  # noqa: E731
-    meta = BoundsMap()
-    check(fn(h, C.byref(meta), None))
-    dist = np.empty((meta.rows, meta.cols), dtype=np.float32)
-    check(fn(h, C.byref(meta), dist.ctypes.data))
-    return dist, meta.resolution, (meta.center_x, meta.center_y)
-
-
 class BoundsParams(C.Structure):
     _fields_ = [("front_length", C.c_double), ("rear_length", C.c_double), ("car_width", C.c_double),
                 ("safety_margin", C.c_double), ("epsilon", C.c_double)]
@@ -170,8 +158,96 @@ def _declare(L):
     return L
 
 
-class PathBounds:
+class MapSlots:
+    """The map surface of a handle that owns map slots, shared by `PathBounds` and `plan.Planner`: `_abi` is the prefix
+    of the handle's C entry points (pqp_bounds_, pqp_plan_), `L` the library and `h` the handle."""
+    _abi = None
+
+    def _fn(self, name):
+        return getattr(self.L, self._abi + name)
+
+    def _create(self, name, *args):
+        """`name` ("create" or "create_maps") with `args` and the out-pointer; raises with the ABI's create error."""
+        h = C.c_void_p()
+        rc = self._fn(name)(*args, C.byref(h))
+        if rc:
+            raise PqpError(rc, (self._fn("last_error")(None) or b"").decode())
+        self.h = h
+
+    def _create_maps(self, dists, resolutions, centers, *args):
+        """from_maps: one slot per float32 layer in `dists`; `args` are the create arguments after the maps."""
+        arr, self._layers = map_list(dists, resolutions, centers)
+        self.dist = self._layers[0]
+        self._create("create_maps", arr, len(self._layers), *args)
+
+    @property
+    def n_maps(self):
+        return int(self._fn("map_count")(self.h))
+
+    def close(self):
+        if getattr(self, "h", None):
+            self._fn("destroy")(self.h)
+            self.h = None
+
+    __del__ = close
+
+    def _check(self, rc):
+        if rc:
+            raise PqpError(rc, (self._fn("last_error")(self.h) or b"").decode())
+
+    def set_map(self, dist, resolution, center=(0.0, 0.0), slot=0):
+        """Replace the map (of `slot`) with a float32 distance layer [rows, cols] (host, synchronous); rows * cols may
+        not exceed the cells of a slot."""
+        m, _keep = distance_map(dist, resolution, center)
+        if slot:
+            self._check(self._fn("set_map_slot")(self.h, int(slot), C.byref(m)))
+        else:
+            self._check(self._fn("set_map")(self.h, C.byref(m)))
+
+    def set_occupancy(self, img, resolution, center=(0.0, 0.0), obstacle_max=0, slot=0):
+        """Replace the map (of `slot`) with the exact Euclidean distance transform, computed on the GPU, of a uint8
+        image [rows, cols] (host, synchronous): cells <= obstacle_max are obstacles (0: the demo's zero pixels)."""
+        if slot:
+            img = np.ascontiguousarray(img, dtype=np.uint8)
+            self.set_occupancy_slots(img[None], resolution, [center], obstacle_max, first_slot=slot)
+            return
+        m, _keep = occupancy_map(img, resolution, center, obstacle_max)
+        self._check(self._fn("set_occupancy")(self.h, C.byref(m)))
+
+    def set_occupancy_slots(self, imgs, resolution, centers=None, obstacle_max=0, *, first_slot=0):
+        """The exact distance transforms of a uint8 stack [count, rows, cols] into slots first_slot .. + count - 1,
+        in one pair of launches (host, synchronous); `centers` [count, 2] (default: the origin)."""
+        imgs = np.ascontiguousarray(imgs, dtype=np.uint8)
+        assert imgs.ndim == 3
+        st, _keep = occupancy_stack(imgs.ctypes.data, imgs.shape, resolution, centers, obstacle_max)
+        self._check(self._fn("set_occupancy_slots")(self.h, int(first_slot), C.byref(st)))
+
+    def set_occupancy_slots_device(self, imgs, resolution, centers=None, obstacle_max=0, *, first_slot=0, stream=0):
+        """As `set_occupancy_slots` from a torch uint8 CUDA tensor [count, rows, cols], asynchronous on `stream` (a raw
+        cudaStream_t): calls enqueued before see the old slots, calls enqueued after the new ones. The tensor must
+        stay alive until the stream has run the transform."""
+        import torch
+        assert imgs.is_cuda and imgs.is_contiguous() and imgs.dtype == torch.uint8 and imgs.dim() == 3
+        st, _keep = occupancy_stack(imgs.data_ptr(), imgs.shape, resolution, centers, obstacle_max)
+        self._check(self._fn("set_occupancy_slots_device")(self.h, int(first_slot), C.byref(st), C.c_void_p(stream)))
+
+    def get_map(self, slot=0):
+        """-> (float32 distance layer [rows, cols], resolution, (center_x, center_y)) of the current map (of `slot`);
+        waits for the device."""
+        if slot:
+            fn = lambda h_, m_, d_: self._fn("get_map_slot")(h_, int(slot), m_, d_)  # noqa: E731
+        else:
+            fn = self._fn("get_map")
+        meta = BoundsMap()
+        self._check(fn(self.h, C.byref(meta), None))
+        dist = np.empty((meta.rows, meta.cols), dtype=np.float32)
+        self._check(fn(self.h, C.byref(meta), dist.ctypes.data))
+        return dist, meta.resolution, (meta.center_x, meta.center_y)
+
+
+class PathBounds(MapSlots):
     """One obstacle map on one GPU; `dist` is the float32 distance layer [rows, cols]."""
+    _abi = "pqp_bounds_"
 
     def __init__(self, dist, resolution, *, center=(0.0, 0.0), params=None, device=0):
         self.L = _declare(load_library())
@@ -179,11 +255,7 @@ class PathBounds:
         self.params = params if params is not None else default_params()
         m = BoundsMap(self.dist.shape[0], self.dist.shape[1], float(resolution), float(center[0]), float(center[1]),
                       self.dist.ctypes.data)
-        h = C.c_void_p()
-        rc = self.L.pqp_bounds_create(C.byref(m), C.byref(self.params), int(device), C.byref(h))
-        if rc:
-            raise PqpError(rc, (self.L.pqp_bounds_last_error(None) or b"").decode())
-        self.h = h
+        self._create("create", C.byref(m), C.byref(self.params), int(device))
 
     @classmethod
     def from_maps(cls, dists, resolutions, *, centers=None, params=None, device=0):
@@ -191,30 +263,9 @@ class PathBounds:
         `resolutions` is one value or one per map, `centers` [(x, y)] per map (default: the origin)."""
         self = cls.__new__(cls)
         self.L = _declare(load_library())
-        arr, self._layers = map_list(dists, resolutions, centers)
-        self.dist = self._layers[0]
         self.params = params if params is not None else default_params()
-        h = C.c_void_p()
-        rc = self.L.pqp_bounds_create_maps(arr, len(self._layers), C.byref(self.params), int(device), C.byref(h))
-        if rc:
-            raise PqpError(rc, (self.L.pqp_bounds_last_error(None) or b"").decode())
-        self.h = h
+        self._create_maps(dists, resolutions, centers, C.byref(self.params), int(device))
         return self
-
-    @property
-    def n_maps(self):
-        return int(self.L.pqp_bounds_map_count(self.h))
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.L.pqp_bounds_destroy(self.h)
-            self.h = None
-
-    __del__ = close
-
-    def _check(self, rc):
-        if rc:
-            raise PqpError(rc, (self.L.pqp_bounds_last_error(self.h) or b"").decode())
 
     def compute(self, states, n, spline, k, *, knots=None, map_index=None):
         """Host buffers: states[b][4][n_max], n[b], spline[b][9][k_max], k[b] ->
@@ -270,43 +321,3 @@ class PathBounds:
         ms = C.c_float(0)
         self._check(self.L.pqp_bounds_last_kernel_ms(self.h, C.byref(ms)))
         return ms.value
-
-    def set_map(self, dist, resolution, center=(0.0, 0.0), slot=0):
-        """Replace the map (of `slot`) with a float32 distance layer [rows, cols] (rows * cols <= the cells at
-        construction)."""
-        m, _keep = distance_map(dist, resolution, center)
-        if slot:
-            self._check(self.L.pqp_bounds_set_map_slot(self.h, int(slot), C.byref(m)))
-        else:
-            self._check(self.L.pqp_bounds_set_map(self.h, C.byref(m)))
-
-    def set_occupancy(self, img, resolution, center=(0.0, 0.0), obstacle_max=0, slot=0):
-        """Replace the map (of `slot`) with the exact Euclidean distance transform of a uint8 image [rows, cols],
-        computed on the GPU: cells <= obstacle_max are obstacles (0: the demo's zero pixels)."""
-        if slot:
-            img = np.ascontiguousarray(img, dtype=np.uint8)
-            self.set_occupancy_slots(img[None], resolution, [center], obstacle_max, first_slot=slot)
-            return
-        m, _keep = occupancy_map(img, resolution, center, obstacle_max)
-        self._check(self.L.pqp_bounds_set_occupancy(self.h, C.byref(m)))
-
-    def set_occupancy_slots(self, imgs, resolution, centers=None, obstacle_max=0, *, first_slot=0):
-        """The distance transforms of a uint8 stack [count, rows, cols] into slots first_slot .. + count - 1 (host,
-        synchronous); `centers` [count, 2]."""
-        imgs = np.ascontiguousarray(imgs, dtype=np.uint8)
-        assert imgs.ndim == 3
-        st, _keep = occupancy_stack(imgs.ctypes.data, imgs.shape, resolution, centers, obstacle_max)
-        self._check(self.L.pqp_bounds_set_occupancy_slots(self.h, int(first_slot), C.byref(st)))
-
-    def set_occupancy_slots_device(self, imgs, resolution, centers=None, obstacle_max=0, *, first_slot=0, stream=0):
-        """As `set_occupancy_slots` from a torch uint8 CUDA tensor [count, rows, cols], asynchronous on `stream` (a raw
-        cudaStream_t; the tensor must live until the stream has run the transform)."""
-        import torch
-        assert imgs.is_cuda and imgs.is_contiguous() and imgs.dtype == torch.uint8 and imgs.dim() == 3
-        st, _keep = occupancy_stack(imgs.data_ptr(), imgs.shape, resolution, centers, obstacle_max)
-        self._check(self.L.pqp_bounds_set_occupancy_slots_device(self.h, int(first_slot), C.byref(st),
-                                                                 C.c_void_p(stream)))
-
-    def get_map(self, slot=0):
-        """-> (float32 distance layer [rows, cols], resolution, (center_x, center_y)) of the current map (of `slot`)."""
-        return get_map(self.L.pqp_bounds_get_map, self.h, self._check, self.L.pqp_bounds_get_map_slot, slot)

@@ -12,6 +12,7 @@
 #include <cstring>
 #include <memory>
 #include <new>
+#include <optional>
 #include <string>
 #include <vector>
 
@@ -469,7 +470,9 @@ int create(const pqp_bounds_map *maps, int n_maps, const pqp_bounds_params *para
     return PQP_OK;
 }
 
-int set_map_slot(pqp_bounds_handle *h, int slot, const pqp_bounds_map *map, cudaStream_t s, const char *what) {
+// pqp_bounds_set_map(_slot)(_device); `stream` empty: the host forms, which run on the handle's stream and wait
+int set_map_slot(pqp_bounds_handle *h, int slot, const pqp_bounds_map *map, std::optional<cudaStream_t> stream,
+                 const char *what) {
     if (!h) return PQP_E_INVALID;
     int rc = validate_slots(h, slot, 1, what);
     if (rc != PQP_OK) return rc;
@@ -478,6 +481,7 @@ int set_map_slot(pqp_bounds_handle *h, int slot, const pqp_bounds_map *map, cuda
              : validate_map(h, nullptr, 0, 0, 0.0, 0.0, 0.0, nullptr, what);
     if (rc != PQP_OK) return rc;
     pqp::DeviceGuard guard_(h->device);
+    const cudaStream_t s = stream ? *stream : h->stream;
     const size_t cells = (size_t)map->rows * map->cols;
     PQP_CUDA(h->err, cudaMemcpyAsync(slot_layer(h, slot), map->distance, cells * sizeof(float), cudaMemcpyDefault, s));
     const pqb::MapView m = make_view(slot_layer(h, slot), map->rows, map->cols, map->resolution, map->center_x,
@@ -485,6 +489,7 @@ int set_map_slot(pqp_bounds_handle *h, int slot, const pqp_bounds_map *map, cuda
     rc = write_table(h, slot, 1, m, &map->center_x, &map->center_y, s);
     if (rc != PQP_OK) return rc;
     h->maps[slot] = m;
+    if (!stream) PQP_CUDA(h->err, cudaStreamSynchronize(s));
     return PQP_OK;
 }
 
@@ -508,8 +513,18 @@ int get_map_slot(pqp_bounds_handle *h, int slot, pqp_bounds_map *meta, float *di
     return PQP_OK;
 }
 
-int compute_host(pqp_bounds_handle *h, const pqp_bounds_in *in, const int32_t *map_index, const pqp_bounds_out *out) {
+// every pqp_bounds_compute* entry point: `mapped` for the mapped forms (path b on slot map_index[b]), `stream` empty
+// for the host forms, which stage the inputs into the handle's buffers, run on the handle's stream, copy the outputs
+// back and wait
+int compute(pqp_bounds_handle *h, const pqp_bounds_in *in, bool mapped, const int32_t *map_index,
+            const pqp_bounds_out *out, std::optional<cudaStream_t> stream) {
+    int rc = validate(h, in, out);
+    if (rc != PQP_OK) return rc;
+    if (mapped && !map_index)
+        return fail(h->err, PQP_E_INVALID,
+                    stream ? "pqp_bounds_compute_mapped_device: null map_index" : "pqp_bounds_compute_mapped: null map_index");
     pqp::DeviceGuard guard_(h->device);
+    if (stream) return launch(h, in, map_index, out, *stream);
     const size_t B = in->batch, ns = B * PQP_STATE_ROWS * in->n_max, nsp = B * PQP_SPLINE_ROWS * in->k_max;
     const size_t nb = B * PQP_BOUND_ROWS * in->n_max, nk = out->knots ? B * PQP_NFIELDS * in->n_max : 0;
     PQP_CUDA(h->err, h->res.grow(h->d_states, ns));
@@ -519,14 +534,14 @@ int compute_host(pqp_bounds_handle *h, const pqp_bounds_in *in, const int32_t *m
     PQP_CUDA(h->err, h->res.grow(h->d_n, B));
     PQP_CUDA(h->err, h->res.grow(h->d_k, B));
     PQP_CUDA(h->err, h->res.grow(h->d_nvalid, B));
-    if (map_index) PQP_CUDA(h->err, h->res.grow(h->d_map_index, B));
+    if (mapped) PQP_CUDA(h->err, h->res.grow(h->d_map_index, B));
     cudaStream_t s = h->stream;
     PQP_CUDA(h->err, cudaMemcpyAsync(h->d_states, in->states, ns * sizeof(double), cudaMemcpyHostToDevice, s));
     PQP_CUDA(h->err, cudaMemcpyAsync(h->d_spline, in->spline, nsp * sizeof(double), cudaMemcpyHostToDevice, s));
     PQP_CUDA(h->err, cudaMemcpyAsync(h->d_n, in->n, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     PQP_CUDA(h->err, cudaMemcpyAsync(h->d_k, in->k, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     if (nk) PQP_CUDA(h->err, cudaMemcpyAsync(h->d_knots, out->knots, nk * sizeof(double), cudaMemcpyHostToDevice, s));
-    if (map_index)
+    if (mapped)
         PQP_CUDA(h->err, cudaMemcpyAsync(h->d_map_index, map_index, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     pqp_bounds_in din = *in;
     din.states = h->d_states;
@@ -537,7 +552,7 @@ int compute_host(pqp_bounds_handle *h, const pqp_bounds_in *in, const int32_t *m
     dout.bounds = h->d_bounds;
     dout.n_valid = h->d_nvalid;
     dout.knots = nk ? h->d_knots : nullptr;
-    const int rc = launch(h, &din, map_index ? h->d_map_index : nullptr, &dout, s);
+    rc = launch(h, &din, mapped ? h->d_map_index : nullptr, &dout, s);
     if (rc != PQP_OK) return rc;
     PQP_CUDA(h->err, cudaMemcpyAsync(out->bounds, h->d_bounds, nb * sizeof(double), cudaMemcpyDeviceToHost, s));
     PQP_CUDA(h->err, cudaMemcpyAsync(out->n_valid, h->d_nvalid, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
@@ -576,33 +591,21 @@ void pqp_bounds_destroy(pqp_bounds_handle *h) {
 int32_t pqp_bounds_map_count(const pqp_bounds_handle *h) { return h ? h->n_maps : 0; }
 
 int pqp_bounds_compute_device(pqp_bounds_handle *h, const pqp_bounds_in *in, const pqp_bounds_out *out, void *stream) {
-    int rc = validate(h, in, out);
-    if (rc != PQP_OK) return rc;
-    pqp::DeviceGuard guard_(h->device);
-    return launch(h, in, nullptr, out, static_cast<cudaStream_t>(stream));
+    return compute(h, in, false, nullptr, out, static_cast<cudaStream_t>(stream));
 }
 
 int pqp_bounds_compute(pqp_bounds_handle *h, const pqp_bounds_in *in, const pqp_bounds_out *out) {
-    const int rc = validate(h, in, out);
-    if (rc != PQP_OK) return rc;
-    return compute_host(h, in, nullptr, out);
+    return compute(h, in, false, nullptr, out, std::nullopt);
 }
 
 int pqp_bounds_compute_mapped_device(pqp_bounds_handle *h, const pqp_bounds_in *in, const int32_t *map_index,
                                      const pqp_bounds_out *out, void *stream) {
-    int rc = validate(h, in, out);
-    if (rc != PQP_OK) return rc;
-    if (!map_index) return fail(h->err, PQP_E_INVALID, "pqp_bounds_compute_mapped_device: null map_index");
-    pqp::DeviceGuard guard_(h->device);
-    return launch(h, in, map_index, out, static_cast<cudaStream_t>(stream));
+    return compute(h, in, true, map_index, out, static_cast<cudaStream_t>(stream));
 }
 
 int pqp_bounds_compute_mapped(pqp_bounds_handle *h, const pqp_bounds_in *in, const int32_t *map_index,
                               const pqp_bounds_out *out) {
-    const int rc = validate(h, in, out);
-    if (rc != PQP_OK) return rc;
-    if (!map_index) return fail(h->err, PQP_E_INVALID, "pqp_bounds_compute_mapped: null map_index");
-    return compute_host(h, in, map_index, out);
+    return compute(h, in, true, map_index, out, std::nullopt);
 }
 
 static int validate_states(pqp_bounds_handle *h, const pqp_states_in *in, const pqp_states_out *out) {
@@ -639,17 +642,13 @@ static int launch_states(pqp_bounds_handle *h, const pqp_states_in *in, const pq
     return PQP_OK;
 }
 
-int pqp_bounds_build_states_device(pqp_bounds_handle *h, const pqp_states_in *in, const pqp_states_out *out, void *stream) {
+// pqp_bounds_build_states(_device); `stream` empty: the host form, as compute's
+static int build_states(pqp_bounds_handle *h, const pqp_states_in *in, const pqp_states_out *out,
+                        std::optional<cudaStream_t> stream) {
     int rc = validate_states(h, in, out);
     if (rc != PQP_OK) return rc;
     pqp::DeviceGuard guard_(h->device);
-    return launch_states(h, in, out, static_cast<cudaStream_t>(stream));
-}
-
-int pqp_bounds_build_states(pqp_bounds_handle *h, const pqp_states_in *in, const pqp_states_out *out) {
-    int rc = validate_states(h, in, out);
-    if (rc != PQP_OK) return rc;
-    pqp::DeviceGuard guard_(h->device);
+    if (stream) return launch_states(h, in, out, *stream);
     const size_t B = in->batch, ns = B * PQP_STATE_ROWS * in->n_max, nsp = B * PQP_SPLINE_ROWS * in->k_max;
     const size_t nc = B * in->n_max, nk = out->knots ? B * PQP_NFIELDS * in->n_max : 0;
     PQP_CUDA(h->err, h->res.grow(h->d_states, ns));
@@ -688,6 +687,14 @@ int pqp_bounds_build_states(pqp_bounds_handle *h, const pqp_states_in *in, const
     return PQP_OK;
 }
 
+int pqp_bounds_build_states_device(pqp_bounds_handle *h, const pqp_states_in *in, const pqp_states_out *out, void *stream) {
+    return build_states(h, in, out, static_cast<cudaStream_t>(stream));
+}
+
+int pqp_bounds_build_states(pqp_bounds_handle *h, const pqp_states_in *in, const pqp_states_out *out) {
+    return build_states(h, in, out, std::nullopt);
+}
+
 int pqp_bounds_last_kernel_ms(pqp_bounds_handle *h, float *ms) {
     if (!h || !ms) return PQP_E_INVALID;
     if (!h->timed) {
@@ -706,11 +713,7 @@ int pqp_bounds_set_map_device(pqp_bounds_handle *h, const pqp_bounds_map *map, v
 }
 
 int pqp_bounds_set_map(pqp_bounds_handle *h, const pqp_bounds_map *map) {
-    const int rc = pqp_bounds_set_map_device(h, map, h ? h->stream : nullptr);
-    if (rc != PQP_OK) return rc;
-    pqp::DeviceGuard guard_(h->device);
-    PQP_CUDA(h->err, cudaStreamSynchronize(h->stream));
-    return PQP_OK;
+    return set_map_slot(h, 0, map, std::nullopt, "pqp_bounds_set_map");
 }
 
 int pqp_bounds_set_map_slot_device(pqp_bounds_handle *h, int32_t slot, const pqp_bounds_map *map, void *stream) {
@@ -718,11 +721,7 @@ int pqp_bounds_set_map_slot_device(pqp_bounds_handle *h, int32_t slot, const pqp
 }
 
 int pqp_bounds_set_map_slot(pqp_bounds_handle *h, int32_t slot, const pqp_bounds_map *map) {
-    const int rc = pqp_bounds_set_map_slot_device(h, slot, map, h ? h->stream : nullptr);
-    if (rc != PQP_OK) return rc;
-    pqp::DeviceGuard guard_(h->device);
-    PQP_CUDA(h->err, cudaStreamSynchronize(h->stream));
-    return PQP_OK;
+    return set_map_slot(h, slot, map, std::nullopt, "pqp_bounds_set_map_slot");
 }
 
 int pqp_bounds_set_occupancy_device(pqp_bounds_handle *h, const pqp_occupancy_map *occ, void *stream) {

@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 
 #include <new>
+#include <optional>
 #include <string>
 
 #include "../../include/pqp_dp.h"
@@ -140,7 +141,8 @@ namespace {
 
 using pqp::fail;
 
-int search_host(pqp_dp_handle *h, const pqp_dp_in *in, const int32_t *map_index, const pqp_dp_out *out);
+int search(pqp_dp_handle *h, const pqp_dp_in *in, bool mapped, const int32_t *map_index, const pqp_dp_out *out,
+           std::optional<cudaStream_t> stream);
 
 int validate(pqp_dp_handle *h, const pqp_dp_in *in, const pqp_dp_out *out) {
     if (!h) return PQP_E_INVALID;
@@ -279,32 +281,20 @@ void pqp_dp_destroy(pqp_dp_handle *h) {
 int32_t pqp_dp_lateral_count(const pqp_dp_handle *h) { return h ? h->J : 0; }
 
 int pqp_dp_search_device(pqp_dp_handle *h, const pqp_dp_in *in, const pqp_dp_out *out, void *stream) {
-    int rc = validate(h, in, out);
-    if (rc != PQP_OK) return rc;
-    pqp::DeviceGuard guard_(h->device);
-    return launch(h, in, nullptr, out, static_cast<cudaStream_t>(stream));
+    return search(h, in, false, nullptr, out, static_cast<cudaStream_t>(stream));
 }
 
 int pqp_dp_search_mapped_device(pqp_dp_handle *h, const pqp_dp_in *in, const int32_t *map_index, const pqp_dp_out *out,
                                 void *stream) {
-    int rc = validate(h, in, out);
-    if (rc != PQP_OK) return rc;
-    if (!map_index) return fail(h->err, PQP_E_INVALID, "null map_index");
-    pqp::DeviceGuard guard_(h->device);
-    return launch(h, in, map_index, out, static_cast<cudaStream_t>(stream));
+    return search(h, in, true, map_index, out, static_cast<cudaStream_t>(stream));
 }
 
 int pqp_dp_search(pqp_dp_handle *h, const pqp_dp_in *in, const pqp_dp_out *out) {
-    const int rc = validate(h, in, out);
-    if (rc != PQP_OK) return rc;
-    return search_host(h, in, nullptr, out);
+    return search(h, in, false, nullptr, out, std::nullopt);
 }
 
 int pqp_dp_search_mapped(pqp_dp_handle *h, const pqp_dp_in *in, const int32_t *map_index, const pqp_dp_out *out) {
-    const int rc = validate(h, in, out);
-    if (rc != PQP_OK) return rc;
-    if (!map_index) return fail(h->err, PQP_E_INVALID, "null map_index");
-    return search_host(h, in, map_index, out);
+    return search(h, in, true, map_index, out, std::nullopt);
 }
 
 int pqp_dp_last_kernel_ms(pqp_dp_handle *h, float *ms) {
@@ -317,9 +307,16 @@ int pqp_dp_last_kernel_ms(pqp_dp_handle *h, float *ms) {
 
 namespace {
 
-int search_host(pqp_dp_handle *h, const pqp_dp_in *in, const int32_t *map_index, const pqp_dp_out *out) {
-    int rc = PQP_OK;
+// every pqp_dp_search* entry point: `mapped` for the mapped forms (path b on slot map_index[b]), `stream` empty for
+// the host forms, which stage the inputs into the handle's buffers, search on the handle's stream, copy the outputs
+// back and wait
+int search(pqp_dp_handle *h, const pqp_dp_in *in, bool mapped, const int32_t *map_index, const pqp_dp_out *out,
+           std::optional<cudaStream_t> stream) {
+    int rc = validate(h, in, out);
+    if (rc != PQP_OK) return rc;
+    if (mapped && !map_index) return fail(h->err, PQP_E_INVALID, "null map_index");
     pqp::DeviceGuard guard_(h->device);
+    if (stream) return launch(h, in, map_index, out, *stream);
     const size_t B = in->batch, nsp = B * PQP_SPLINE_ROWS * in->k_max, Ls = B * h->layers_max, T = Ls * h->J;
     PQP_CUDA(h->err, h->res.grow(h->d_spline, nsp));
     cudaStream_t s = h->stream;
@@ -334,11 +331,11 @@ int search_host(pqp_dp_handle *h, const pqp_dp_in *in, const int32_t *map_index,
     pqp_dp_in din = {in->batch, in->k_max, h->d_spline, h->d_k, h->d_length, h->d_start};
     pqp_dp_out dout = {h->d_status, h->d_n_layers, h->d_n_out, h->d_layer_s, h->d_lower, h->d_upper, h->d_chosen,
                        h->d_vehicle_l, h->d_target_s, nullptr, nullptr, nullptr};
-    if (map_index) {
+    if (mapped) {
         PQP_CUDA(h->err, h->res.grow(h->d_map_index, B));
         PQP_CUDA(h->err, cudaMemcpyAsync(h->d_map_index, map_index, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     }
-    rc = launch(h, &din, map_index ? h->d_map_index : nullptr, &dout, s);
+    rc = launch(h, &din, mapped ? h->d_map_index : nullptr, &dout, s);
     if (rc != PQP_OK) return rc;
     PQP_CUDA(h->err, cudaMemcpyAsync(out->status, h->d_status, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
     PQP_CUDA(h->err, cudaMemcpyAsync(out->n_layers, h->d_n_layers, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));

@@ -10,6 +10,7 @@
 #include <cuda_runtime.h>
 
 #include <new>
+#include <optional>
 #include <string>
 
 #include "../../include/pqp_plan.h"
@@ -689,6 +690,67 @@ int run_points(pqp_plan_handle *h, const pqp_plan_points_in *pts, const pqp_plan
     return run(h, &din, out, s, pts, map_index);
 }
 
+// every pqp_plan* and pqp_plan_points* entry point: `pts` for the points forms (`in` is then NULL), `mapped` for the
+// mapped forms (path b on slot map_index[b]), `stream` empty for the host forms, which stage the inputs into the
+// handle's buffers, run on the handle's stream, copy the outputs back and wait
+int plan(pqp_plan_handle *h, const pqp_plan_in *in, const pqp_plan_points_in *pts, bool mapped,
+         const int32_t *map_index, const pqp_plan_out *out, std::optional<cudaStream_t> stream) {
+    int rc = pts ? validate_points(h, pts, out) : validate(h, in, out);
+    if (rc != PQP_OK) return rc;
+    if (mapped && !map_index) return fail(h->err, PQP_E_INVALID, "null map_index");
+    pqp::DeviceGuard guard_(h->device);
+    if (stream) return pts ? run_points(h, pts, out, *stream, map_index) : run(h, in, out, *stream, nullptr, map_index);
+    cudaStream_t s = h->stream;
+    const int batch = pts ? pts->batch : in->batch;
+    const size_t B = batch;
+    if (pts) {
+        const size_t M = pts->m_max;
+        PQP_CUDA(h->err, cudaMemcpyAsync(h->pt_x, pts->ref_x, B * M * sizeof(double), cudaMemcpyHostToDevice, s));
+        PQP_CUDA(h->err, cudaMemcpyAsync(h->pt_y, pts->ref_y, B * M * sizeof(double), cudaMemcpyHostToDevice, s));
+        PQP_CUDA(h->err, cudaMemcpyAsync(h->pt_m, pts->m, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    } else {
+        const size_t R = in->r_max;
+        PQP_CUDA(h->err, cudaMemcpyAsync(h->in_x, in->raw_x, B * R * sizeof(double), cudaMemcpyHostToDevice, s));
+        PQP_CUDA(h->err, cudaMemcpyAsync(h->in_y, in->raw_y, B * R * sizeof(double), cudaMemcpyHostToDevice, s));
+        PQP_CUDA(h->err, cudaMemcpyAsync(h->in_r, in->r, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    }
+    const double *start = pts ? pts->start : in->start, *target = pts ? pts->target : in->target;
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_start, start, B * 4 * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_target, target, B * 3 * sizeof(double), cudaMemcpyHostToDevice, s));
+    if (mapped)
+        PQP_CUDA(h->err, cudaMemcpyAsync(h->in_map_index, map_index, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    const int32_t *dmap_index = mapped ? h->in_map_index : nullptr;
+    const pqp_plan_out dout = {h->o_status, h->o_n, h->o_path, h->o_cost, h->o_iters, out->trace};
+    if (pts) {
+        const pqp_plan_points_in din = {batch, pts->m_max, h->pt_x, h->pt_y, h->pt_m, h->in_start, h->in_target};
+        rc = run_points(h, &din, &dout, s, dmap_index);
+    } else {
+        const pqp_plan_in din = {batch, in->r_max, h->in_x, h->in_y, h->in_r, h->in_start, h->in_target};
+        rc = run(h, &din, &dout, s, nullptr, dmap_index);
+    }
+    if (rc != PQP_OK) return rc;
+    return copy_results(h, out, batch, s);
+}
+
+// a map call of the plan forwarded to its bounds handle: the bounds handle's reason in h->err, `n` more kernel launches
+// on success; `sync`: a host form, which waits for the plan stream
+#define PQL_MAP(h, call, n, sync)                                                             \
+    do {                                                                                      \
+        if (!(h)) return PQP_E_INVALID;                                                       \
+        PQL_SUB(h, call, pqp_bounds_last_error, (h)->bounds);                                 \
+        (h)->launches += (n);                                                                 \
+        if (sync) {                                                                           \
+            pqp::DeviceGuard guard_((h)->device);                                             \
+            PQP_CUDA((h)->err, cudaStreamSynchronize((h)->stream));                           \
+        }                                                                                     \
+        return PQP_OK;                                                                        \
+    } while (0)
+
+// column pass, row pass and the table entries, PQP_MAP_TABLE_CHUNK per launch
+long long occupancy_slots_launches(const pqp_occupancy_stack *st) {
+    return 2 + (st->count + PQP_MAP_TABLE_CHUNK - 1) / PQP_MAP_TABLE_CHUNK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -860,192 +922,83 @@ void pqp_plan_destroy(pqp_plan_handle *h) {
 }
 
 int pqp_plan_device(pqp_plan_handle *h, const pqp_plan_in *in, const pqp_plan_out *out, void *stream) {
-    int rc = validate(h, in, out);
-    if (rc != PQP_OK) return rc;
-    pqp::DeviceGuard guard_(h->device);
-    return run(h, in, out, static_cast<cudaStream_t>(stream));
+    return plan(h, in, nullptr, false, nullptr, out, static_cast<cudaStream_t>(stream));
 }
 
 int pqp_plan(pqp_plan_handle *h, const pqp_plan_in *in, const pqp_plan_out *out) {
-    int rc = validate(h, in, out);
-    if (rc != PQP_OK) return rc;
-    pqp::DeviceGuard guard_(h->device);
-    cudaStream_t s = h->stream;
-    const size_t B = in->batch, R = in->r_max;
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_x, in->raw_x, B * R * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_y, in->raw_y, B * R * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_r, in->r, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_start, in->start, B * 4 * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_target, in->target, B * 3 * sizeof(double), cudaMemcpyHostToDevice, s));
-    const pqp_plan_in din = {in->batch, in->r_max, h->in_x, h->in_y, h->in_r, h->in_start, h->in_target};
-    const pqp_plan_out dout = {h->o_status, h->o_n, h->o_path, h->o_cost, h->o_iters, out->trace};
-    rc = run(h, &din, &dout, s);
-    if (rc != PQP_OK) return rc;
-    return copy_results(h, out, in->batch, s);
+    return plan(h, in, nullptr, false, nullptr, out, std::nullopt);
 }
 
 int pqp_plan_points_device(pqp_plan_handle *h, const pqp_plan_points_in *in, const pqp_plan_out *out, void *stream) {
-    int rc = validate_points(h, in, out);
-    if (rc != PQP_OK) return rc;
-    pqp::DeviceGuard guard_(h->device);
-    return run_points(h, in, out, static_cast<cudaStream_t>(stream));
+    return plan(h, nullptr, in, false, nullptr, out, static_cast<cudaStream_t>(stream));
 }
 
 int pqp_plan_points(pqp_plan_handle *h, const pqp_plan_points_in *in, const pqp_plan_out *out) {
-    int rc = validate_points(h, in, out);
-    if (rc != PQP_OK) return rc;
-    pqp::DeviceGuard guard_(h->device);
-    cudaStream_t s = h->stream;
-    const size_t B = in->batch, M = in->m_max;
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->pt_x, in->ref_x, B * M * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->pt_y, in->ref_y, B * M * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->pt_m, in->m, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_start, in->start, B * 4 * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_target, in->target, B * 3 * sizeof(double), cudaMemcpyHostToDevice, s));
-    const pqp_plan_points_in din = {in->batch, in->m_max, h->pt_x, h->pt_y, h->pt_m, h->in_start, h->in_target};
-    const pqp_plan_out dout = {h->o_status, h->o_n, h->o_path, h->o_cost, h->o_iters, out->trace};
-    rc = run_points(h, &din, &dout, s);
-    if (rc != PQP_OK) return rc;
-    return copy_results(h, out, in->batch, s);
+    return plan(h, nullptr, in, false, nullptr, out, std::nullopt);
 }
 
 int pqp_plan_mapped_device(pqp_plan_handle *h, const pqp_plan_in *in, const int32_t *map_index, const pqp_plan_out *out,
                            void *stream) {
-    int rc = validate(h, in, out);
-    if (rc != PQP_OK) return rc;
-    if (!map_index) return fail(h->err, PQP_E_INVALID, "null map_index");
-    pqp::DeviceGuard guard_(h->device);
-    return run(h, in, out, static_cast<cudaStream_t>(stream), nullptr, map_index);
+    return plan(h, in, nullptr, true, map_index, out, static_cast<cudaStream_t>(stream));
 }
 
 int pqp_plan_mapped(pqp_plan_handle *h, const pqp_plan_in *in, const int32_t *map_index, const pqp_plan_out *out) {
-    int rc = validate(h, in, out);
-    if (rc != PQP_OK) return rc;
-    if (!map_index) return fail(h->err, PQP_E_INVALID, "null map_index");
-    pqp::DeviceGuard guard_(h->device);
-    cudaStream_t s = h->stream;
-    const size_t B = in->batch, R = in->r_max;
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_x, in->raw_x, B * R * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_y, in->raw_y, B * R * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_r, in->r, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_start, in->start, B * 4 * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_target, in->target, B * 3 * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_map_index, map_index, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    const pqp_plan_in din = {in->batch, in->r_max, h->in_x, h->in_y, h->in_r, h->in_start, h->in_target};
-    const pqp_plan_out dout = {h->o_status, h->o_n, h->o_path, h->o_cost, h->o_iters, out->trace};
-    rc = run(h, &din, &dout, s, nullptr, h->in_map_index);
-    if (rc != PQP_OK) return rc;
-    return copy_results(h, out, in->batch, s);
+    return plan(h, in, nullptr, true, map_index, out, std::nullopt);
 }
 
 int pqp_plan_points_mapped_device(pqp_plan_handle *h, const pqp_plan_points_in *in, const int32_t *map_index,
                                   const pqp_plan_out *out, void *stream) {
-    int rc = validate_points(h, in, out);
-    if (rc != PQP_OK) return rc;
-    if (!map_index) return fail(h->err, PQP_E_INVALID, "null map_index");
-    pqp::DeviceGuard guard_(h->device);
-    return run_points(h, in, out, static_cast<cudaStream_t>(stream), map_index);
+    return plan(h, nullptr, in, true, map_index, out, static_cast<cudaStream_t>(stream));
 }
 
 int pqp_plan_points_mapped(pqp_plan_handle *h, const pqp_plan_points_in *in, const int32_t *map_index,
                            const pqp_plan_out *out) {
-    int rc = validate_points(h, in, out);
-    if (rc != PQP_OK) return rc;
-    if (!map_index) return fail(h->err, PQP_E_INVALID, "null map_index");
-    pqp::DeviceGuard guard_(h->device);
-    cudaStream_t s = h->stream;
-    const size_t B = in->batch, M = in->m_max;
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->pt_x, in->ref_x, B * M * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->pt_y, in->ref_y, B * M * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->pt_m, in->m, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_start, in->start, B * 4 * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_target, in->target, B * 3 * sizeof(double), cudaMemcpyHostToDevice, s));
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->in_map_index, map_index, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    const pqp_plan_points_in din = {in->batch, in->m_max, h->pt_x, h->pt_y, h->pt_m, h->in_start, h->in_target};
-    const pqp_plan_out dout = {h->o_status, h->o_n, h->o_path, h->o_cost, h->o_iters, out->trace};
-    rc = run_points(h, &din, &dout, s, h->in_map_index);
-    if (rc != PQP_OK) return rc;
-    return copy_results(h, out, in->batch, s);
+    return plan(h, nullptr, in, true, map_index, out, std::nullopt);
 }
 
 int pqp_plan_set_map_device(pqp_plan_handle *h, const pqp_bounds_map *map, void *stream) {
-    if (!h) return PQP_E_INVALID;
-    PQL_SUB(h, pqp_bounds_set_map_device(h->bounds, map, stream), pqp_bounds_last_error, h->bounds);
-    h->launches += 1;  // the slot's table entry
-    return PQP_OK;
+    PQL_MAP(h, pqp_bounds_set_map_device(h->bounds, map, stream), 1, false);  // the slot's table entry
+}
+
+int pqp_plan_set_map(pqp_plan_handle *h, const pqp_bounds_map *map) {
+    PQL_MAP(h, pqp_bounds_set_map_device(h->bounds, map, h->stream), 1, true);
 }
 
 int pqp_plan_set_map_slot_device(pqp_plan_handle *h, int32_t slot, const pqp_bounds_map *map, void *stream) {
-    if (!h) return PQP_E_INVALID;
-    PQL_SUB(h, pqp_bounds_set_map_slot_device(h->bounds, slot, map, stream), pqp_bounds_last_error, h->bounds);
-    h->launches += 1;
-    return PQP_OK;
+    PQL_MAP(h, pqp_bounds_set_map_slot_device(h->bounds, slot, map, stream), 1, false);
 }
 
 int pqp_plan_set_map_slot(pqp_plan_handle *h, int32_t slot, const pqp_bounds_map *map) {
-    if (!h) return PQP_E_INVALID;
-    PQL_SUB(h, pqp_plan_set_map_slot_device(h, slot, map, h->stream), pqp_plan_last_error, h);
-    pqp::DeviceGuard guard_(h->device);
-    PQP_CUDA(h->err, cudaStreamSynchronize(h->stream));
-    return PQP_OK;
+    PQL_MAP(h, pqp_bounds_set_map_slot_device(h->bounds, slot, map, h->stream), 1, true);
 }
 
-// column pass, row pass and the table entries, PQP_MAP_TABLE_CHUNK per launch
-static long long occupancy_slots_launches(const pqp_occupancy_stack *st) {
-    return 2 + (st->count + PQP_MAP_TABLE_CHUNK - 1) / PQP_MAP_TABLE_CHUNK;
+int pqp_plan_set_occupancy_device(pqp_plan_handle *h, const pqp_occupancy_map *occ, void *stream) {
+    PQL_MAP(h, pqp_bounds_set_occupancy_device(h->bounds, occ, stream), 2, false);  // column and row pass
+}
+
+int pqp_plan_set_occupancy(pqp_plan_handle *h, const pqp_occupancy_map *occ) {
+    PQL_MAP(h, pqp_bounds_set_occupancy(h->bounds, occ), 2, false);
 }
 
 int pqp_plan_set_occupancy_slots_device(pqp_plan_handle *h, int32_t first_slot, const pqp_occupancy_stack *stack,
                                         void *stream) {
-    if (!h) return PQP_E_INVALID;
-    PQL_SUB(h, pqp_bounds_set_occupancy_slots_device(h->bounds, first_slot, stack, stream), pqp_bounds_last_error,
-            h->bounds);
-    h->launches += occupancy_slots_launches(stack);
-    return PQP_OK;
+    PQL_MAP(h, pqp_bounds_set_occupancy_slots_device(h->bounds, first_slot, stack, stream),
+            occupancy_slots_launches(stack), false);
 }
 
 int pqp_plan_set_occupancy_slots(pqp_plan_handle *h, int32_t first_slot, const pqp_occupancy_stack *stack) {
-    if (!h) return PQP_E_INVALID;
-    PQL_SUB(h, pqp_bounds_set_occupancy_slots(h->bounds, first_slot, stack), pqp_bounds_last_error, h->bounds);
-    h->launches += occupancy_slots_launches(stack);
-    return PQP_OK;
-}
-
-int pqp_plan_get_map_slot(pqp_plan_handle *h, int32_t slot, pqp_bounds_map *meta, float *distance) {
-    if (!h) return PQP_E_INVALID;
-    PQL_SUB(h, pqp_bounds_get_map_slot(h->bounds, slot, meta, distance), pqp_bounds_last_error, h->bounds);
-    return PQP_OK;
-}
-
-int32_t pqp_plan_map_count(const pqp_plan_handle *h) { return h ? pqp_bounds_map_count(h->bounds) : 0; }
-
-int pqp_plan_set_map(pqp_plan_handle *h, const pqp_bounds_map *map) {
-    if (!h) return PQP_E_INVALID;
-    PQL_SUB(h, pqp_plan_set_map_device(h, map, h->stream), pqp_plan_last_error, h);
-    pqp::DeviceGuard guard_(h->device);
-    PQP_CUDA(h->err, cudaStreamSynchronize(h->stream));
-    return PQP_OK;
-}
-
-int pqp_plan_set_occupancy_device(pqp_plan_handle *h, const pqp_occupancy_map *occ, void *stream) {
-    if (!h) return PQP_E_INVALID;
-    PQL_SUB(h, pqp_bounds_set_occupancy_device(h->bounds, occ, stream), pqp_bounds_last_error, h->bounds);
-    h->launches += 2;  // column and row pass of the distance transform
-    return PQP_OK;
-}
-
-int pqp_plan_set_occupancy(pqp_plan_handle *h, const pqp_occupancy_map *occ) {
-    if (!h) return PQP_E_INVALID;
-    PQL_SUB(h, pqp_bounds_set_occupancy(h->bounds, occ), pqp_bounds_last_error, h->bounds);
-    h->launches += 2;
-    return PQP_OK;
+    PQL_MAP(h, pqp_bounds_set_occupancy_slots(h->bounds, first_slot, stack), occupancy_slots_launches(stack), false);
 }
 
 int pqp_plan_get_map(pqp_plan_handle *h, pqp_bounds_map *meta, float *distance) {
-    if (!h) return PQP_E_INVALID;
-    PQL_SUB(h, pqp_bounds_get_map(h->bounds, meta, distance), pqp_bounds_last_error, h->bounds);
-    return PQP_OK;
+    PQL_MAP(h, pqp_bounds_get_map(h->bounds, meta, distance), 0, false);
 }
+
+int pqp_plan_get_map_slot(pqp_plan_handle *h, int32_t slot, pqp_bounds_map *meta, float *distance) {
+    PQL_MAP(h, pqp_bounds_get_map_slot(h->bounds, slot, meta, distance), 0, false);
+}
+
+int32_t pqp_plan_map_count(const pqp_plan_handle *h) { return h ? pqp_bounds_map_count(h->bounds) : 0; }
 
 int pqp_plan_last_stage_ms(pqp_plan_handle *h, float *ms) {
     if (!h || !ms) return PQP_E_INVALID;

@@ -173,8 +173,15 @@ def _trace_struct(arrays, ptr):
     return PlanTrace(*(ptr(arrays[n]) for n, _, _ in _TRACE))
 
 
-class Planner:
+def _stream(stream, device):
+    """The raw cudaStream_t of a torch stream (None: the current stream of `device`)."""
+    import torch
+    return (stream if stream is not None else torch.cuda.current_stream(device)).cuda_stream
+
+
+class Planner(bounds.MapSlots):
     """Batched PathOptimizer::solve over one obstacle map (`dist`: float32 distance layer [rows, cols])."""
+    _abi = "pqp_plan_"
 
     def __init__(self, dist, resolution, *, r_max, p_max, layers_max=64, n_max=256, batch_max, center=(0.0, 0.0),
                  params=None, device=0):
@@ -185,12 +192,8 @@ class Planner:
         self.batch_max, self.device = int(batch_max), int(device)
         m = bounds.BoundsMap(self.dist.shape[0], self.dist.shape[1], float(resolution), float(center[0]),
                              float(center[1]), self.dist.ctypes.data)
-        h = C.c_void_p()
-        rc = self.L.pqp_plan_create(C.byref(m), C.byref(self.params), self.r_max, self.p_max, self.layers_max, self.n_max,
-                                    self.batch_max, self.device, C.byref(h))
-        if rc:
-            raise solver.PqpError(rc, (self.L.pqp_plan_last_error(None) or b"").decode())
-        self.h = h
+        self._create("create", C.byref(m), C.byref(self.params), self.r_max, self.p_max, self.layers_max, self.n_max,
+                     self.batch_max, self.device)
 
     @classmethod
     def from_maps(cls, dists, resolutions, *, centers=None, r_max, p_max, layers_max=64, n_max=256, batch_max,
@@ -200,33 +203,12 @@ class Planner:
         `map_index` plan path b on slot map_index[b]; the others use slot 0."""
         self = cls.__new__(cls)
         self.L = _lib()
-        arr, self._layers = bounds.map_list(dists, resolutions, centers)
-        self.dist = self._layers[0]
         self.params = params if params is not None else default_params()
         self.r_max, self.p_max, self.layers_max, self.n_max = int(r_max), int(p_max), int(layers_max), int(n_max)
         self.batch_max, self.device = int(batch_max), int(device)
-        h = C.c_void_p()
-        rc = self.L.pqp_plan_create_maps(arr, len(self._layers), C.byref(self.params), self.r_max, self.p_max,
-                                         self.layers_max, self.n_max, self.batch_max, self.device, C.byref(h))
-        if rc:
-            raise solver.PqpError(rc, (self.L.pqp_plan_last_error(None) or b"").decode())
-        self.h = h
+        self._create_maps(dists, resolutions, centers, C.byref(self.params), self.r_max, self.p_max, self.layers_max,
+                          self.n_max, self.batch_max, self.device)
         return self
-
-    @property
-    def n_maps(self):
-        return int(self.L.pqp_plan_map_count(self.h))
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.L.pqp_plan_destroy(self.h)
-            self.h = None
-
-    __del__ = close
-
-    def _check(self, rc):
-        if rc:
-            raise solver.PqpError(rc, (self.L.pqp_plan_last_error(self.h) or b"").decode())
 
     @property
     def dims(self):
@@ -304,53 +286,22 @@ class Planner:
                       target.data_ptr())
         pout = PlanOut(out["status"].data_ptr(), out["n"].data_ptr(), out["path"].data_ptr(), out["cost"].data_ptr(),
                        out["iters"].data_ptr(), C.pointer(tr) if tr is not None else None)
-        s = stream if stream is not None else torch.cuda.current_stream(dev)
+        s = C.c_void_p(_stream(stream, dev))
         if map_index is None:
-            self._check(fn(self.h, C.byref(pin), C.byref(pout), C.c_void_p(s.cuda_stream)))
+            self._check(fn(self.h, C.byref(pin), C.byref(pout), s))
         else:
             assert map_index.is_cuda and map_index.is_contiguous() and map_index.dtype == torch.int32
             assert tuple(map_index.shape) == (B,)
-            self._check(mapped_fn(self.h, C.byref(pin), map_index.data_ptr(), C.byref(pout), C.c_void_p(s.cuda_stream)))
+            self._check(mapped_fn(self.h, C.byref(pin), map_index.data_ptr(), C.byref(pout), s))
         return out
-
-    def set_map(self, dist, resolution, center=(0.0, 0.0), slot=0):
-        """Replace the map (of `slot`) with a float32 distance layer [rows, cols] (host, synchronous); rows * cols may
-        not exceed the cells of a slot."""
-        m, _keep = bounds.distance_map(dist, resolution, center)
-        if slot:
-            self._check(self.L.pqp_plan_set_map_slot(self.h, int(slot), C.byref(m)))
-        else:
-            self._check(self.L.pqp_plan_set_map(self.h, C.byref(m)))
-
-    def set_occupancy(self, img, resolution, center=(0.0, 0.0), obstacle_max=0, slot=0):
-        """Replace the map (of `slot`) with the exact Euclidean distance transform, computed on the GPU, of a uint8
-        image [rows, cols] (host, synchronous): cells <= obstacle_max are obstacles (0: the demo's zero pixels)."""
-        if slot:
-            img = np.ascontiguousarray(img, dtype=np.uint8)
-            self.set_occupancy_slots(img[None], resolution, [center], obstacle_max, first_slot=slot)
-            return
-        m, _keep = bounds.occupancy_map(img, resolution, center, obstacle_max)
-        self._check(self.L.pqp_plan_set_occupancy(self.h, C.byref(m)))
-
-    def set_occupancy_slots(self, imgs, resolution, centers=None, obstacle_max=0, *, first_slot=0):
-        """The exact distance transforms of a uint8 stack [count, rows, cols] into slots first_slot .. + count - 1,
-        in one pair of launches (host, synchronous); `centers` [count, 2] (default: the origin)."""
-        imgs = np.ascontiguousarray(imgs, dtype=np.uint8)
-        assert imgs.ndim == 3
-        st, _keep = bounds.occupancy_stack(imgs.ctypes.data, imgs.shape, resolution, centers, obstacle_max)
-        self._check(self.L.pqp_plan_set_occupancy_slots(self.h, int(first_slot), C.byref(st)))
 
     def set_occupancy_slots_device(self, imgs, resolution, centers=None, obstacle_max=0, *, first_slot=0,
                                    stream=None):
         """As `set_occupancy_slots` from a torch uint8 CUDA tensor [count, rows, cols], asynchronous on `stream`
         (default: the current stream): plans enqueued before see the old slots, plans enqueued after the new ones. The
         tensor must stay alive until the stream has run the transform."""
-        import torch
-        assert imgs.is_cuda and imgs.is_contiguous() and imgs.dtype == torch.uint8 and imgs.dim() == 3
-        st, _keep = bounds.occupancy_stack(imgs.data_ptr(), imgs.shape, resolution, centers, obstacle_max)
-        s = stream if stream is not None else torch.cuda.current_stream(imgs.device)
-        self._check(self.L.pqp_plan_set_occupancy_slots_device(self.h, int(first_slot), C.byref(st),
-                                                               C.c_void_p(s.cuda_stream)))
+        super().set_occupancy_slots_device(imgs, resolution, centers, obstacle_max, first_slot=first_slot,
+                                           stream=_stream(stream, imgs.device))
 
     def set_map_device(self, dist, resolution, center=(0.0, 0.0), *, stream=None):
         """As `set_map` from a torch float32 CUDA tensor [rows, cols], asynchronous on `stream` (default: the
@@ -359,8 +310,7 @@ class Planner:
         assert dist.is_cuda and dist.is_contiguous() and dist.dtype == torch.float32 and dist.dim() == 2
         m = bounds.BoundsMap(int(dist.shape[0]), int(dist.shape[1]), float(resolution), float(center[0]),
                              float(center[1]), dist.data_ptr())
-        s = stream if stream is not None else torch.cuda.current_stream(dist.device)
-        self._check(self.L.pqp_plan_set_map_device(self.h, C.byref(m), C.c_void_p(s.cuda_stream)))
+        self._check(self.L.pqp_plan_set_map_device(self.h, C.byref(m), C.c_void_p(_stream(stream, dist.device))))
 
     def set_occupancy_device(self, img, resolution, center=(0.0, 0.0), obstacle_max=0, *, stream=None):
         """As `set_occupancy` from a torch uint8 CUDA tensor [rows, cols], asynchronous on `stream` (default: the
@@ -369,13 +319,7 @@ class Planner:
         assert img.is_cuda and img.is_contiguous() and img.dtype == torch.uint8 and img.dim() == 2
         m = bounds.OccupancyMap(int(img.shape[0]), int(img.shape[1]), float(resolution), float(center[0]),
                                 float(center[1]), img.data_ptr(), int(obstacle_max))
-        s = stream if stream is not None else torch.cuda.current_stream(img.device)
-        self._check(self.L.pqp_plan_set_occupancy_device(self.h, C.byref(m), C.c_void_p(s.cuda_stream)))
-
-    def get_map(self, slot=0):
-        """-> (float32 distance layer [rows, cols], resolution, (center_x, center_y)) of the current map (of `slot`);
-        waits for the device."""
-        return bounds.get_map(self.L.pqp_plan_get_map, self.h, self._check, self.L.pqp_plan_get_map_slot, slot)
+        self._check(self.L.pqp_plan_set_occupancy_device(self.h, C.byref(m), C.c_void_p(_stream(stream, img.device))))
 
     @property
     def last_stage_ms(self):
