@@ -197,6 +197,45 @@ int pqp_bounds_compute_mapped(pqp_bounds_handle *h, const pqp_bounds_in *in, con
 int pqp_bounds_compute_mapped_device(pqp_bounds_handle *h, const pqp_bounds_in *in, const int32_t *map_index,
                                      const pqp_bounds_out *out, void *stream);
 
+/* Footprint collision check of a batch of poses against the map (CollisionChecker, src/tools/collision_checker.cpp:
+ * 17-59, with CarGeometry(car_width, |rear_length|, front_length), src/tools/car_geometry.cpp:10-73, from the handle's
+ * pqp_bounds_params). A pose is free under isSingleStateCollisionFreeImproved: the car's bounding circle, placed with
+ * local2Global (tools.cpp:50-55), must have its centre strictly inside the map; if its interpolated obstacle distance
+ * is not below its radius the pose is free, otherwise it is free only if each of the six footprint circles (rr, rl,
+ * fr, fl, fm, rm) has its centre inside the map and a distance not below its radius. The comparisons are the
+ * reference's: a NaN distance is not below a radius, and a pose the bounding circle clears is free even where a small
+ * circle's distance is below its radius. Nothing here changes a plan: a caller enqueues the check after a plan call on
+ * the same stream with the same map_index, e.g. on pqp_plan_out.path with row_stride PQP_PLAN_PATH_ROWS. */
+typedef struct pqp_collision_in {
+    int32_t batch, n_max;
+    int32_t row_stride;   /* rows per path: PQP_PLAN_PATH_ROWS for pqp_plan_out.path, PQP_STATE_ROWS for states */
+    const double *poses;  /* [b][row_stride][n_max]; rows 0, 1, 2 = x, y, heading. Reference states:
+                             states + n_max with row_stride PQP_STATE_ROWS */
+    const int32_t *n;     /* [b], clamped to [0, n_max] as the bounds kernel clamps it */
+} pqp_collision_in;
+
+typedef struct pqp_collision_out {
+    int32_t *first_hit;   /* [b]: index of the first pose that is not free, n[b] when all are (0 for n[b] = 0); -1 for
+                             a mapped call's index outside [0, n_maps) */
+    uint8_t *state_free;  /* optional [b][n_max]: the per-pose verdict (0 at i >= n[b]) */
+    double *clearance;    /* optional [b][n_max]: min over the six circles of d_i - r_i (the exact test's margin; it can
+                             be negative on a pose the bounding-circle shortcut passes; 0 at i >= n[b]) */
+} pqp_collision_out;
+
+/* One kernel launch per call, one CTA per path; pqp_bounds_last_kernel_ms reports it. The host form copies exactly the
+ * ((batch - 1) * row_stride + 3) * n_max doubles of poses the check reads, so states + n_max is a valid argument, and
+ * returns when the outputs are in place; the *_device forms take device buffers and are asynchronous on `stream`.
+ * The mapped forms check path b on slot map_index[b] (map_index [batch] in the memory space of the other buffers); a
+ * path whose index is outside [0, n_maps) reads no map. Refused with PQP_E_INVALID: batch <= 0, n_max <= 0,
+ * row_stride < 3, a NULL poses, n or first_hit, a NULL map_index in a mapped form. */
+int pqp_bounds_collision_check(pqp_bounds_handle *h, const pqp_collision_in *in, const pqp_collision_out *out);
+int pqp_bounds_collision_check_device(pqp_bounds_handle *h, const pqp_collision_in *in, const pqp_collision_out *out,
+                                      void *stream);
+int pqp_bounds_collision_check_mapped(pqp_bounds_handle *h, const pqp_collision_in *in, const int32_t *map_index,
+                                      const pqp_collision_out *out);
+int pqp_bounds_collision_check_mapped_device(pqp_bounds_handle *h, const pqp_collision_in *in,
+                                             const int32_t *map_index, const pqp_collision_out *out, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -221,6 +221,16 @@ int pqp_plan_set_occupancy_slots_device(pqp_plan_handle *h, int32_t first_slot, 
                                         void *stream);
 int pqp_plan_get_map_slot(pqp_plan_handle *h, int32_t slot, pqp_bounds_map *meta, float *distance);
 int32_t pqp_plan_map_count(const pqp_plan_handle *h);
+/* The footprint collision check of pqp_bounds.h on the plan's map slots, e.g. on a plan's final paths (out.path,
+ * row_stride PQP_PLAN_PATH_ROWS, out.n), enqueued after the plan call on the same stream with the same map_index. It
+ * changes no plan output; each call is 1 kernel launch, counted by pqp_plan_launch_count. */
+int pqp_plan_collision_check(pqp_plan_handle *h, const pqp_collision_in *in, const pqp_collision_out *out);
+int pqp_plan_collision_check_device(pqp_plan_handle *h, const pqp_collision_in *in, const pqp_collision_out *out,
+                                    void *stream);
+int pqp_plan_collision_check_mapped(pqp_plan_handle *h, const pqp_collision_in *in, const int32_t *map_index,
+                                    const pqp_collision_out *out);
+int pqp_plan_collision_check_mapped_device(pqp_plan_handle *h, const pqp_collision_in *in, const int32_t *map_index,
+                                           const pqp_collision_out *out, void *stream);
 /* ms[PQP_PLAN_NSTAGES] of the last call (CUDA events; waits for that call to finish). */
 int pqp_plan_last_stage_ms(pqp_plan_handle *h, float *ms);
 /* Kernel launches issued by the handle so far: the glue kernels plus those of every stage handle it owns. */

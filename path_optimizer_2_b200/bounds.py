@@ -23,6 +23,8 @@ EXPORTED_SYMBOLS = [
     "pqp_bounds_create_maps", "pqp_bounds_set_map_slot", "pqp_bounds_set_map_slot_device",
     "pqp_bounds_set_occupancy_slots", "pqp_bounds_set_occupancy_slots_device", "pqp_bounds_get_map_slot",
     "pqp_bounds_map_count", "pqp_bounds_compute_mapped", "pqp_bounds_compute_mapped_device",
+    "pqp_bounds_collision_check", "pqp_bounds_collision_check_device", "pqp_bounds_collision_check_mapped",
+    "pqp_bounds_collision_check_mapped_device",
 ]
 MAX_MAP_SLOTS = 65535
 MAP_TABLE_CHUNK = 1024  # table entries per table-write launch of a slot update
@@ -115,6 +117,15 @@ class StatesOut(C.Structure):
                 ("knots", C.c_void_p)]
 
 
+class CollisionIn(C.Structure):
+    _fields_ = [("batch", C.c_int32), ("n_max", C.c_int32), ("row_stride", C.c_int32), ("poses", C.c_void_p),
+                ("n", C.c_void_p)]
+
+
+class CollisionOut(C.Structure):
+    _fields_ = [("first_hit", C.c_void_p), ("state_free", C.c_void_p), ("clearance", C.c_void_p)]
+
+
 def default_params(**overrides):
     p = BoundsParams(3.9, -1.0, 2.0, 0.3, 1e-6)
     for k, v in overrides.items():
@@ -154,8 +165,18 @@ def _declare(L):
     L.pqp_bounds_map_count.restype = C.c_int32
     L.pqp_bounds_compute_mapped.argtypes = [vp, C.POINTER(BoundsIn), vp, C.POINTER(BoundsOut)]
     L.pqp_bounds_compute_mapped_device.argtypes = [vp, C.POINTER(BoundsIn), vp, C.POINTER(BoundsOut), vp]
+    declare_collision(L, "pqp_bounds_")
     L._pqp_bounds_declared = True
     return L
+
+
+def declare_collision(L, prefix):
+    """The four collision-check entry points of the ABI `prefix` (pqp_bounds_, pqp_plan_)."""
+    vp, cin, cout = C.c_void_p, C.POINTER(CollisionIn), C.POINTER(CollisionOut)
+    getattr(L, prefix + "collision_check").argtypes = [vp, cin, cout]
+    getattr(L, prefix + "collision_check_device").argtypes = [vp, cin, cout, vp]
+    getattr(L, prefix + "collision_check_mapped").argtypes = [vp, cin, vp, cout]
+    getattr(L, prefix + "collision_check_mapped_device").argtypes = [vp, cin, vp, cout, vp]
 
 
 class MapSlots:
@@ -243,6 +264,74 @@ class MapSlots:
         dist = np.empty((meta.rows, meta.cols), dtype=np.float32)
         self._check(fn(self.h, C.byref(meta), dist.ctypes.data))
         return dist, meta.resolution, (meta.center_x, meta.center_y)
+
+    def check_collision(self, poses, n, *, row_stride=None, map_index=None, clearance=False, per_state=False):
+        """CollisionChecker::isSingleStateCollisionFreeImproved for every pose (host, synchronous). `poses` float64
+        [B, rows, n_max] with rows 0, 1, 2 = x, y, heading (a plan's `path`, or `states[:, 1:]` of reference states);
+        its rows must be n_max elements apart, and `row_stride` (rows from one path to the next) is read from its
+        strides unless given. -> dict with first_hit int32 [B] (n[b] when all n[b] poses are free, -1 for a
+        `map_index` outside the slots), and when asked state_free uint8 [B, n_max] and clearance float64 [B, n_max]."""
+        poses = np.asarray(poses, dtype=np.float64)
+        rs = _pose_stride(poses.shape, [s // 8 for s in poses.strides], row_stride)
+        if rs is None:
+            poses = np.ascontiguousarray(poses)
+            rs = _pose_stride(poses.shape, [s // 8 for s in poses.strides], row_stride)
+        assert rs is not None, "row_stride disagrees with the layout of poses"
+        B, _, n_max = poses.shape
+        n = np.ascontiguousarray(n, dtype=np.int32)
+        assert n.shape == (B,)
+        out = {"first_hit": np.zeros(B, np.int32)}
+        if per_state:
+            out["state_free"] = np.zeros((B, n_max), np.uint8)
+        if clearance:
+            out["clearance"] = np.zeros((B, n_max))
+        ci = CollisionIn(B, n_max, rs, poses.ctypes.data, n.ctypes.data)
+        co = CollisionOut(*(out[k].ctypes.data if k in out else None for k in ("first_hit", "state_free", "clearance")))
+        if map_index is None:
+            self._check(self._fn("collision_check")(self.h, C.byref(ci), C.byref(co)))
+        else:
+            idx = index_array(map_index, B)
+            self._check(self._fn("collision_check_mapped")(self.h, C.byref(ci), idx.ctypes.data, C.byref(co)))
+        return out
+
+    def check_collision_device(self, poses, n, *, row_stride=None, map_index=None, clearance=False, per_state=False,
+                               stream=0):
+        """As `check_collision` on torch CUDA tensors (poses float64 with rows n_max apart, n and map_index int32 [B]),
+        asynchronous on `stream` (a raw cudaStream_t); returns a dict of CUDA tensors. Enqueued after a plan call on
+        the same stream, it checks that call's output."""
+        import torch
+        assert poses.is_cuda and poses.dtype == torch.float64 and poses.dim() == 3
+        B, _, n_max = poses.shape
+        rs = _pose_stride(poses.shape, poses.stride(), row_stride)
+        assert rs is not None, "poses: rows must be n_max elements apart"
+        assert n.is_cuda and n.is_contiguous() and n.dtype == torch.int32 and tuple(n.shape) == (B,)
+        out = {"first_hit": torch.zeros(B, dtype=torch.int32, device=poses.device)}
+        if per_state:
+            out["state_free"] = torch.zeros((B, n_max), dtype=torch.uint8, device=poses.device)
+        if clearance:
+            out["clearance"] = torch.zeros((B, n_max), dtype=torch.float64, device=poses.device)
+        ci = CollisionIn(B, n_max, rs, poses.data_ptr(), n.data_ptr())
+        co = CollisionOut(*(out[k].data_ptr() if k in out else None for k in ("first_hit", "state_free", "clearance")))
+        s = C.c_void_p(stream)
+        if map_index is None:
+            self._check(self._fn("collision_check_device")(self.h, C.byref(ci), C.byref(co), s))
+        else:
+            assert map_index.is_cuda and map_index.is_contiguous() and map_index.dtype == torch.int32
+            assert tuple(map_index.shape) == (B,)
+            self._check(self._fn("collision_check_mapped_device")(self.h, C.byref(ci), map_index.data_ptr(),
+                                                                  C.byref(co), s))
+        return out
+
+
+def _pose_stride(shape, strides, row_stride):
+    """Rows from one path to the next of a [B, rows, n_max] pose array with element `strides`, or None when its
+    rows are not n_max elements apart (or `row_stride` disagrees)."""
+    B, rows, n_max = shape
+    assert rows >= 3
+    if strides[2] != 1 or strides[1] != n_max or strides[0] % n_max:
+        return None
+    rs = strides[0] // n_max if B > 1 else rows
+    return rs if row_stride is None or int(row_stride) == rs else None
 
 
 class PathBounds(MapSlots):

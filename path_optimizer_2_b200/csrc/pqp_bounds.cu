@@ -19,6 +19,7 @@
 #include "../../include/pqp_bounds.h"
 #include "pqp_bounds_core.cuh"
 #include "pqp_bounds_internal.h"
+#include "pqp_collision_core.cuh"
 #include "pqp_host_handle.h"
 #include "pqp_map_core.cuh"
 
@@ -134,6 +135,56 @@ __global__ void __launch_bounds__(64) reference_states_kernel(const StatesArgs a
     }
 }
 
+struct CollisionArgs {
+    pqb::MapView map;             // the shared map, when map_index is NULL
+    const pqb::MapView *table;    // per-path maps: path b reads table[map_index[b]]
+    const int32_t *map_index;
+    int n_maps;
+    pqc::Footprint fp;
+    int n_max, row_stride;
+    const double *poses;
+    const int32_t *n;
+    int32_t *first_hit;
+    uint8_t *state_free;
+    double *clearance;
+};
+
+constexpr int kCollisionThreads = 128;
+
+// one CTA per path: the threads stride over its states and a block min-reduction gives the first state that is
+// not free (no atomics, so no initialisation launch, and the result does not depend on thread timing)
+__global__ void __launch_bounds__(kCollisionThreads) collision_check_kernel(const CollisionArgs a) {
+    __shared__ int warp_min[kCollisionThreads / 32];
+    const int b = blockIdx.x;
+    int nb = a.n[b];
+    nb = nb < 0 ? 0 : (nb > a.n_max ? a.n_max : nb);
+    pqb::MapView m = a.map;
+    if (a.map_index) {
+        const pqb::MapView *slot = pqb::slot_view(a.table, a.n_maps, a.map_index, b);
+        if (slot) m = *slot;
+        else nb = -1;  // reads no map; every state gets the i >= n outputs
+    }
+    const double *x = a.poses + (size_t)b * a.row_stride * a.n_max, *y = x + a.n_max, *h = y + a.n_max;
+    int hit = nb < 0 ? -1 : nb;
+    for (int i = threadIdx.x; i < a.n_max; i += kCollisionThreads) {
+        bool free_ = false;
+        double c = 0.0;
+        if (i < nb) {
+            free_ = pqc::state_free(m, a.fp, x[i], y[i], h[i], c);
+            if (!free_ && i < hit) hit = i;
+        }
+        if (a.state_free) a.state_free[(size_t)b * a.n_max + i] = free_ ? 1 : 0;
+        if (a.clearance) a.clearance[(size_t)b * a.n_max + i] = c;
+    }
+    hit = __reduce_min_sync(0xffffffffu, hit);
+    if ((threadIdx.x & 31) == 0) warp_min[threadIdx.x >> 5] = hit;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < kCollisionThreads / 32; ++w) hit = warp_min[w] < hit ? warp_min[w] : hit;
+        a.first_hit[b] = hit;
+    }
+}
+
 }  // namespace
 
 // The exact Euclidean distance transform of pqp_bounds_set_occupancy* (pqp_map_core.cuh), in place in the
@@ -221,6 +272,10 @@ struct pqp_bounds_handle {
     int32_t *d_n = nullptr, *d_k = nullptr, *d_nvalid = nullptr, *d_map_index = nullptr;
     double *d_maxs = nullptr, *d_curv = nullptr;
     int32_t *d_total = nullptr;
+    int32_t *d_hit = nullptr;   // the host collision check's outputs (its poses and n go to d_states, d_n)
+    uint8_t *d_free = nullptr;
+    double *d_clear = nullptr;
+    pqc::Footprint footprint{};  // of prm, at create
     bool timed = false;
     std::string err;
     pqp::Resources res;  // last member: releasing clears the members above
@@ -436,6 +491,8 @@ int create(const pqp_bounds_map *maps, int n_maps, const pqp_bounds_params *para
     h->prm.car_width = p.car_width;
     h->prm.safety_margin = p.safety_margin;
     h->prm.epsilon = p.epsilon;
+    // CollisionChecker's constructor (collision_checker.cpp:9-15)
+    h->footprint = pqc::car_footprint(p.car_width, fabs(p.rear_length), p.front_length);
     h->n_maps = n_maps;
     h->cap_cells = cap;
     pqp::DeviceGuard guard_(device);
@@ -561,6 +618,73 @@ int compute(pqp_bounds_handle *h, const pqp_bounds_in *in, bool mapped, const in
     return PQP_OK;
 }
 
+int launch_collision(pqp_bounds_handle *h, const pqp_collision_in *in, const int32_t *map_index,
+                     const pqp_collision_out *out, cudaStream_t s) {
+    CollisionArgs a;
+    a.map = h->maps[0];
+    a.table = h->d_table;
+    a.map_index = map_index;
+    a.n_maps = h->n_maps;
+    a.fp = h->footprint;
+    a.n_max = in->n_max;
+    a.row_stride = in->row_stride;
+    a.poses = in->poses;
+    a.n = in->n;
+    a.first_hit = out->first_hit;
+    a.state_free = out->state_free;
+    a.clearance = out->clearance;
+    PQP_CUDA(h->err, cudaEventRecord(h->ev0, s));
+    collision_check_kernel<<<in->batch, kCollisionThreads, 0, s>>>(a);
+    PQP_CUDA(h->err, cudaGetLastError());
+    PQP_CUDA(h->err, cudaEventRecord(h->ev1, s));
+    h->timed = true;
+    return PQP_OK;
+}
+
+// every pqp_bounds_collision_check* entry point, as compute: `mapped` for the mapped forms, `stream` empty for the
+// host forms
+int collision_check(pqp_bounds_handle *h, const pqp_collision_in *in, bool mapped, const int32_t *map_index,
+                    const pqp_collision_out *out, std::optional<cudaStream_t> stream) {
+    if (!h) return PQP_E_INVALID;
+    if (!in || !out || !in->poses || !in->n || !out->first_hit)
+        return fail(h->err, PQP_E_INVALID, "pqp_bounds_collision_check: null in, out, poses, n or first_hit");
+    if (in->batch <= 0 || in->n_max <= 0 || in->row_stride < 3)
+        return fail(h->err, PQP_E_INVALID, "pqp_bounds_collision_check: batch, n_max > 0 and row_stride >= 3 required");
+    if (mapped && !map_index)
+        return fail(h->err, PQP_E_INVALID,
+                    stream ? "pqp_bounds_collision_check_mapped_device: null map_index"
+                           : "pqp_bounds_collision_check_mapped: null map_index");
+    pqp::DeviceGuard guard_(h->device);
+    if (stream) return launch_collision(h, in, map_index, out, *stream);
+    // the extent the kernel reads: rows 0 .. 2 of the last path, so states + n_max needs no padding row
+    const size_t B = in->batch, np = ((B - 1) * in->row_stride + 3) * in->n_max, ns = B * in->n_max;
+    PQP_CUDA(h->err, h->res.grow(h->d_states, np));
+    PQP_CUDA(h->err, h->res.grow(h->d_n, B));
+    PQP_CUDA(h->err, h->res.grow(h->d_hit, B));
+    if (out->state_free) PQP_CUDA(h->err, h->res.grow(h->d_free, ns));
+    if (out->clearance) PQP_CUDA(h->err, h->res.grow(h->d_clear, ns));
+    if (mapped) PQP_CUDA(h->err, h->res.grow(h->d_map_index, B));
+    cudaStream_t s = h->stream;
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_states, in->poses, np * sizeof(double), cudaMemcpyHostToDevice, s));
+    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_n, in->n, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    if (mapped)
+        PQP_CUDA(h->err, cudaMemcpyAsync(h->d_map_index, map_index, B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    pqp_collision_in din = *in;
+    din.poses = h->d_states;
+    din.n = h->d_n;
+    const pqp_collision_out dout = {h->d_hit, out->state_free ? h->d_free : nullptr,
+                                    out->clearance ? h->d_clear : nullptr};
+    const int rc = launch_collision(h, &din, mapped ? h->d_map_index : nullptr, &dout, s);
+    if (rc != PQP_OK) return rc;
+    PQP_CUDA(h->err, cudaMemcpyAsync(out->first_hit, h->d_hit, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    if (out->state_free)
+        PQP_CUDA(h->err, cudaMemcpyAsync(out->state_free, h->d_free, ns, cudaMemcpyDeviceToHost, s));
+    if (out->clearance)
+        PQP_CUDA(h->err, cudaMemcpyAsync(out->clearance, h->d_clear, ns * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PQP_CUDA(h->err, cudaStreamSynchronize(s));
+    return PQP_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -606,6 +730,25 @@ int pqp_bounds_compute_mapped_device(pqp_bounds_handle *h, const pqp_bounds_in *
 int pqp_bounds_compute_mapped(pqp_bounds_handle *h, const pqp_bounds_in *in, const int32_t *map_index,
                               const pqp_bounds_out *out) {
     return compute(h, in, true, map_index, out, std::nullopt);
+}
+
+int pqp_bounds_collision_check(pqp_bounds_handle *h, const pqp_collision_in *in, const pqp_collision_out *out) {
+    return collision_check(h, in, false, nullptr, out, std::nullopt);
+}
+
+int pqp_bounds_collision_check_device(pqp_bounds_handle *h, const pqp_collision_in *in, const pqp_collision_out *out,
+                                      void *stream) {
+    return collision_check(h, in, false, nullptr, out, static_cast<cudaStream_t>(stream));
+}
+
+int pqp_bounds_collision_check_mapped(pqp_bounds_handle *h, const pqp_collision_in *in, const int32_t *map_index,
+                                      const pqp_collision_out *out) {
+    return collision_check(h, in, true, map_index, out, std::nullopt);
+}
+
+int pqp_bounds_collision_check_mapped_device(pqp_bounds_handle *h, const pqp_collision_in *in,
+                                             const int32_t *map_index, const pqp_collision_out *out, void *stream) {
+    return collision_check(h, in, true, map_index, out, static_cast<cudaStream_t>(stream));
 }
 
 static int validate_states(pqp_bounds_handle *h, const pqp_states_in *in, const pqp_states_out *out) {

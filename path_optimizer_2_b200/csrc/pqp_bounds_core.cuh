@@ -39,6 +39,11 @@ struct SplineView {
     int k;
 };
 
+// grid_map's isInside: strictly inside the map's rectangle (false for NaN), the test map_distance makes
+PQB_HD bool map_inside(const MapView &m, double x, double y) {
+    return fabs(x - m.cx) < m.half_lx && fabs(y - m.cy) < m.half_ly;
+}
+
 // Map::getObstacleDistance (src/tools/Map.cpp:16-22): 0 outside the map, otherwise grid_map's
 // INTER_LINEAR lookup of the float "distance" layer - bilinear between the four cell centres
 // around the position (grid_map itself is not in the tree; at the outermost half cell it falls

@@ -89,9 +89,7 @@ PQB_HD double projection_s(const pqb::SplineView &sp, double tx, double ty, doub
     return projection_newton(sp, tx, ty, max_s, min_s);
 }
 
-PQB_HD bool map_inside(const pqb::MapView &m, double x, double y) {
-    return fabs(x - m.cx) < m.half_lx && fabs(y - m.cy) < m.half_ly;
-}
+using pqb::map_inside;
 
 // The j-th lateral offset by repeated addition, as the reference accumulates cur_l (:185,213)
 PQB_HD double lateral_offset(const Params &p, int j) {

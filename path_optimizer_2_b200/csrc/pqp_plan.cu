@@ -1000,6 +1000,25 @@ int pqp_plan_get_map_slot(pqp_plan_handle *h, int32_t slot, pqp_bounds_map *meta
 
 int32_t pqp_plan_map_count(const pqp_plan_handle *h) { return h ? pqp_bounds_map_count(h->bounds) : 0; }
 
+int pqp_plan_collision_check(pqp_plan_handle *h, const pqp_collision_in *in, const pqp_collision_out *out) {
+    PQL_MAP(h, pqp_bounds_collision_check(h->bounds, in, out), 1, false);
+}
+
+int pqp_plan_collision_check_device(pqp_plan_handle *h, const pqp_collision_in *in, const pqp_collision_out *out,
+                                    void *stream) {
+    PQL_MAP(h, pqp_bounds_collision_check_device(h->bounds, in, out, stream), 1, false);
+}
+
+int pqp_plan_collision_check_mapped(pqp_plan_handle *h, const pqp_collision_in *in, const int32_t *map_index,
+                                    const pqp_collision_out *out) {
+    PQL_MAP(h, pqp_bounds_collision_check_mapped(h->bounds, in, map_index, out), 1, false);
+}
+
+int pqp_plan_collision_check_mapped_device(pqp_plan_handle *h, const pqp_collision_in *in, const int32_t *map_index,
+                                           const pqp_collision_out *out, void *stream) {
+    PQL_MAP(h, pqp_bounds_collision_check_mapped_device(h->bounds, in, map_index, out, stream), 1, false);
+}
+
 int pqp_plan_last_stage_ms(pqp_plan_handle *h, float *ms) {
     if (!h || !ms) return PQP_E_INVALID;
     if (!h->timed) return fail(h->err, PQP_E_STATE, "no plan has run yet");

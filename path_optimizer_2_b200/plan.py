@@ -14,7 +14,11 @@ EXPORTED_SYMBOLS = ["pqp_plan_default_params", "pqp_plan_create", "pqp_plan_dest
                     "pqp_plan_set_occupancy_device", "pqp_plan_get_map", "pqp_plan_create_maps", "pqp_plan_mapped",
                     "pqp_plan_mapped_device", "pqp_plan_points_mapped", "pqp_plan_points_mapped_device",
                     "pqp_plan_set_map_slot", "pqp_plan_set_map_slot_device", "pqp_plan_set_occupancy_slots",
-                    "pqp_plan_set_occupancy_slots_device", "pqp_plan_get_map_slot", "pqp_plan_map_count"]
+                    "pqp_plan_set_occupancy_slots_device", "pqp_plan_get_map_slot", "pqp_plan_map_count",
+                    "pqp_plan_collision_check", "pqp_plan_collision_check_device", "pqp_plan_collision_check_mapped",
+                    "pqp_plan_collision_check_mapped_device"]
+# kernel launches of one collision_check call
+COLLISION_LAUNCHES = 1
 # kernel launches of one set_occupancy call (the distance transform's column and row pass)
 OCCUPANCY_LAUNCHES = 2
 # of one set_map / set_map_slot call (the slot's table entry; the layer is a copy)
@@ -132,6 +136,7 @@ def _lib():
         L.pqp_plan_get_map_slot.argtypes = [vp, C.c_int32, C.POINTER(bounds.BoundsMap), vp]
         L.pqp_plan_map_count.argtypes = [vp]
         L.pqp_plan_map_count.restype = C.c_int32
+        bounds.declare_collision(L, "pqp_plan_")
         L._plan_declared = True
     return L
 
