@@ -69,48 +69,18 @@ inline int32_t handleCapacity(size_t n) {
     return static_cast<int32_t>(n < cap ? cap - 1 : cap);
 }
 
-// Process-wide pool of solver handles. The reference constructs a BaseSolver per plan at 30 Hz
-// (path_optimizer.cpp:138); a pqp_handle owns device buffers, streams and events, so creating one
-// per plan would put a few milliseconds of cudaMalloc / cudaFree (device-synchronising) around a
-// 0.3 ms solve. BaseSolverT borrows a handle of matching (device, capacity, params) and gives it
-// back in its destructor; idle handles are kept (at most kMaxIdle) until clear(). A handle is used
-// by one solver object at a time, which is the threading contract of the reference (one call at a
-// time per solver); the pool itself is thread-safe.
-class HandlePool {
+// Borrow / return bookkeeping of a process-wide pool of library handles. A handle is lent to one object at a
+// time; returned handles stay idle (at most max_idle, the oldest idle one is destroyed first) until clear().
+// The pool that derives from this decides which stored key fits a request and how a handle is made. Thread-safe.
+template <class Key, class Handle>
+class IdlePool {
  public:
-    static HandlePool &instance() {
-        static HandlePool *pool = new HandlePool;  // never destroyed: no CUDA calls during static teardown
-        return *pool;
-    }
-    pqp_handle *acquire(const pqp_params &params, int32_t n_max, int device, std::string *error) {
-        {
-            std::lock_guard<std::mutex> lock(mutex_);
-            for (auto &e : entries_) {
-                if (!e.busy && e.n_max == n_max && e.device == device && std::memcmp(&e.params, &params, sizeof(params)) == 0) {
-                    e.busy = true;
-                    ++hits_;
-                    return e.handle;
-                }
-            }
-        }
-        pqp_handle *h = nullptr;
-        if (pqp_create(&params, n_max, 1, device, &h) != PQP_OK) {
-            if (error) *error = pqp_last_error(nullptr);
-            return nullptr;
-        }
-        std::lock_guard<std::mutex> lock(mutex_);
-        Entry e;
-        e.params = params;
-        e.n_max = n_max;
-        e.device = device;
-        e.handle = h;
-        e.busy = true;
-        entries_.push_back(e);
-        ++creates_;
-        return h;
-    }
-    void release(pqp_handle *h) {
-        pqp_handle *victim = nullptr;
+    typedef void (*DestroyFn)(Handle *);
+    IdlePool(size_t max_idle, DestroyFn destroy) : max_idle_(max_idle), destroy_(destroy) {}
+    IdlePool(const IdlePool &) = delete;
+    IdlePool &operator=(const IdlePool &) = delete;
+    void release(Handle *h) {
+        Handle *victim = nullptr;
         {
             std::lock_guard<std::mutex> lock(mutex_);
             size_t idle = 0;
@@ -118,7 +88,7 @@ class HandlePool {
                 if (e.handle == h) e.busy = false;
                 if (!e.busy) ++idle;
             }
-            if (idle > kMaxIdle) {  // drop the oldest idle handle
+            if (idle > max_idle_) {  // drop the oldest idle handle
                 for (size_t i = 0; i < entries_.size(); ++i) {
                     if (!entries_[i].busy && entries_[i].handle != h) {
                         victim = entries_[i].handle;
@@ -128,11 +98,11 @@ class HandlePool {
                 }
             }
         }
-        if (victim) pqp_destroy(victim);
+        if (victim) destroy_(victim);
     }
     // destroy every idle handle (call before cudaDeviceReset / at shutdown if desired)
     void clear() {
-        std::vector<pqp_handle *> idle;
+        std::vector<Handle *> idle;
         {
             std::lock_guard<std::mutex> lock(mutex_);
             for (size_t i = entries_.size(); i-- > 0;) {
@@ -142,24 +112,112 @@ class HandlePool {
                 }
             }
         }
-        for (pqp_handle *h : idle) pqp_destroy(h);
+        for (Handle *h : idle) destroy_(h);
     }
     size_t creates() const { return creates_; }
     size_t hits() const { return hits_; }
 
+ protected:
+    // lend the first idle handle whose key satisfies fits(key), or nullptr
+    template <class Fits>
+    Handle *take(Fits fits) {
+        std::lock_guard<std::mutex> lock(mutex_);
+        for (auto &e : entries_) {
+            if (!e.busy && fits(e.key)) {
+                e.busy = true;
+                ++hits_;
+                return e.handle;
+            }
+        }
+        return nullptr;
+    }
+    // record a handle just created for `key`, lent to the caller
+    Handle *add(const Key &key, Handle *h) {
+        std::lock_guard<std::mutex> lock(mutex_);
+        Entry e;
+        e.key = key;
+        e.handle = h;
+        e.busy = true;
+        entries_.push_back(e);
+        ++creates_;
+        return h;
+    }
+
  private:
-    static constexpr size_t kMaxIdle = 8;
     struct Entry {
-        pqp_params params;
-        int32_t n_max;
-        int device;
-        pqp_handle *handle;
+        Key key;
+        Handle *handle;
         bool busy;
     };
+    const size_t max_idle_;
+    const DestroyFn destroy_;
     std::mutex mutex_;
     std::vector<Entry> entries_;
     size_t creates_ = 0, hits_ = 0;
 };
+
+struct SolverHandleKey {
+    pqp_params params;
+    int32_t n_max;
+    int device;
+};
+
+inline void destroySolverHandle(pqp_handle *h) { pqp_destroy(h); }
+
+// Process-wide pool of solver handles. The reference constructs a BaseSolver per plan at 30 Hz
+// (path_optimizer.cpp:138); a pqp_handle owns device buffers, streams and events, so creating one
+// per plan would put a few milliseconds of cudaMalloc / cudaFree (device-synchronising) around a
+// 0.3 ms solve. BaseSolverT borrows a handle of matching (device, capacity, params) and gives it
+// back in its destructor; idle handles are kept (at most 8) until clear(). A handle is used
+// by one solver object at a time, which is the threading contract of the reference (one call at a
+// time per solver); the pool itself is thread-safe.
+class HandlePool : public IdlePool<SolverHandleKey, pqp_handle> {
+ public:
+    static HandlePool &instance() {
+        static HandlePool *pool = new HandlePool;  // never destroyed: no CUDA calls during static teardown
+        return *pool;
+    }
+    pqp_handle *acquire(const pqp_params &params, int32_t n_max, int device, std::string *error) {
+        pqp_handle *h = take([&](const SolverHandleKey &k) {
+            return k.n_max == n_max && k.device == device && std::memcmp(&k.params, &params, sizeof(params)) == 0;
+        });
+        if (h) return h;
+        if (pqp_create(&params, n_max, 1, device, &h) != PQP_OK) {
+            if (error) *error = pqp_last_error(nullptr);
+            return nullptr;
+        }
+        SolverHandleKey key;
+        key.params = params;
+        key.n_max = n_max;
+        key.device = device;
+        return add(key, h);
+    }
+
+ private:
+    HandlePool() : IdlePool(8, destroySolverHandle) {}
+};
+
+// BaseSolver::getOptimizedPath (base_solver.cpp:263-288): the Cartesian path of a solution sol[f * stride + i]
+// (f = 0: l, 1: psi, 2: kappa, 3: d_k) over the first n reference states; s, v and a stay 0.
+template <class StateT, class SlStateT>
+void getOptimizedPath(const std::vector<StateT> &ref_states, const double *sol, size_t stride, size_t n,
+                      std::vector<SlStateT> *optimized_path) {
+    optimized_path->clear();
+    for (size_t i = 0; i != n; ++i) {
+        SlStateT pt;
+        const double angle = ref_states[i].heading;
+        const double l = sol[i], psi = sol[stride + i];
+        pt.heading = constrainAngle(angle + psi);
+        pt.d_heading = psi;
+        pt.l = l;
+        const double new_angle = constrainAngle(angle + M_PI_2);
+        pt.x = ref_states[i].x + l * std::cos(new_angle);
+        pt.y = ref_states[i].y + l * std::sin(new_angle);
+        pt.k = sol[2 * stride + i];
+        if (i < n - 1) pt.d_k = sol[3 * stride + i];
+        optimized_path->push_back(pt);
+    }
+}
 
 template <class ReferencePathT, class VehicleStateT, class SlStateT>
 class BaseSolverT {
@@ -280,7 +338,8 @@ class BaseSolverT {
         }
         pqp_last_stage_ms(handle_, stage_ms_);
         if (status_ != PQP_SOLVED) return false;  // osqp-eigen: solve() fails unless OSQP_SOLVED
-        get_optimized_path(optimized_path);
+        getOptimizedPath(reference_path_.getReferenceStates(), sol_.data(), static_cast<size_t>(n_max_), n_,
+                         optimized_path);
         return true;
     }
 
