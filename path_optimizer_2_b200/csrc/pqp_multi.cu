@@ -9,11 +9,11 @@
 #include <algorithm>
 #include <new>
 #include <string>
-#include <thread>
 #include <vector>
 
 #include "../../include/pqp_multi.h"
 #include "pqp_host_handle.h"
+#include "pqp_shard.h"
 
 namespace {
 
@@ -93,13 +93,13 @@ int run(pqp_multi *m, const pqp_batch_in *in, const pqp_batch_out *out, bool war
     }
     if (warm && B != m->last_batch) return fail(m->err, PQP_E_STATE, "resolve needs a previous solve of the same batch");
     const int G = m->n_dev, nmax = m->n_max;
-    const int per = (B + G - 1) / G;
+    const int per = pqp::shard_per(B, G);
     const size_t nvm = 6 * (size_t)nmax - 1, mm = 6 * (size_t)nmax + 2;
     std::vector<int> rc(G, PQP_OK);
-    std::vector<std::thread> workers;
     // one host thread per device: each runs that device's own (pipelined, synchronous) host call
-    auto work = [&](int d) {
-        const int lo = std::min(B, d * per), hi = std::min(B, lo + per);
+    pqp::fan_out(G, [&](int d) {
+        const pqp::Shard sh = pqp::shard_of(B, per, d);
+        const int lo = sh.first, hi = sh.first + sh.count;
         if (lo >= hi) return;
         pqp_batch_in din;
         pqp_batch_out dout = {};
@@ -120,10 +120,7 @@ int run(pqp_multi *m, const pqp_batch_in *in, const pqp_batch_out *out, bool war
             din.p = in->p ? in->p + lo : nullptr;
         }
         rc[d] = warm ? pqp_resolve(m->h[d], in ? &din : nullptr, &dout) : pqp_solve(m->h[d], &din, &dout);
-    };
-    for (int d = 1; d < G; ++d) workers.emplace_back(work, d);
-    work(0);
-    for (auto &t : workers) t.join();
+    });
     for (int d = 0; d < G; ++d)
         if (rc[d] != PQP_OK) return fail(m->err, rc[d], std::string("device ") + std::to_string(m->dev[d]) + ": " + pqp_last_error(m->h[d]));
     m->last_batch = B;
@@ -131,7 +128,8 @@ int run(pqp_multi *m, const pqp_batch_in *in, const pqp_batch_out *out, bool war
     // pack on every device, then one all-gather of per * 16 bytes per device
     for (int d = 0; d < G; ++d) {
         pqp::DeviceGuard g(m->dev[d]);
-        const int lo = std::min(B, d * per), hi = std::min(B, lo + per);
+        const pqp::Shard sh = pqp::shard_of(B, per, d);
+        const int lo = sh.first, hi = sh.first + sh.count;
         cudaEventRecord(m->ev0[d], m->stream[d]);
         cudaMemsetAsync(m->d_send[d], 0, (size_t)per * sizeof(pqp_result_rec), m->stream[d]);
         if (hi > lo) {
@@ -259,9 +257,9 @@ int pqp_multi_gathered(pqp_multi *m, int32_t i, const pqp_result_rec **table, in
 
 int pqp_multi_shard(pqp_multi *m, int32_t i, int32_t *first, int32_t *count) {
     if (!m || i < 0 || i >= m->n_dev) return PQP_E_INVALID;
-    const int lo = std::min(m->last_batch, i * m->last_per), hi = std::min(m->last_batch, lo + m->last_per);
-    if (first) *first = lo;
-    if (count) *count = hi - lo;
+    const pqp::Shard sh = pqp::shard_of(m->last_batch, m->last_per, i);
+    if (first) *first = sh.first;
+    if (count) *count = sh.count;
     return PQP_OK;
 }
 

@@ -17,6 +17,7 @@
 #include "pqp_bounds_internal.h"
 #include "pqp_host_handle.h"
 #include "pqp_plan_core.cuh"
+#include "pqp_plan_trace.h"
 #include "pqp_smoother_internal.h"
 
 namespace {
@@ -455,60 +456,61 @@ int copy_out(pqp_plan_handle *h, void *dst, const void *src, size_t bytes, cudaS
 
 int copy_trace(pqp_plan_handle *h, const pqp_plan_trace *t, int B, bool points, cudaStream_t s) {
     if (!t) return PQP_OK;
-    const size_t b = B, d = sizeof(double), i4 = sizeof(int32_t), P = h->P, L = h->L, N = h->N, R = h->R;
-    int rc = PQP_OK;
-#define PQL_T(dst, src, bytes) \
-    if ((rc = copy_out(h, (dst), (src), (bytes), s)) != PQP_OK) return rc
-    PQL_T(t->raw_spline, h->raw_rows, b * PQP_SPLINE_ROWS * R * d);
-    PQL_T(t->seg_p, h->seg_p, b * i4);
-    PQL_T(t->seg_x, h->seg[0], b * P * d);
-    PQL_T(t->seg_y, h->seg[1], b * P * d);
-    PQL_T(t->seg_angle, h->seg[2], b * P * d);
-    PQL_T(t->seg_k, h->seg[3], b * P * d);
-    PQL_T(t->seg_s, h->seg[4], b * P * d);
-    PQL_T(t->tension_x, h->t_x, b * P * d);
-    PQL_T(t->tension_y, h->t_y, b * P * d);
-    PQL_T(t->tension_s, h->t_s, b * P * d);
-    PQL_T(t->tension_status, h->t_status, b * i4);
-    PQL_T(t->tension_iters, h->t_iters, b * i4);
-    PQL_T(t->tension_spline, h->t_rows, b * PQP_SPLINE_ROWS * P * d);
-    PQL_T(t->tension_length, h->t_len, b * d);
-    PQL_T(t->dp_status, h->dp_status, b * i4);
-    PQL_T(t->dp_n_out, h->dp_nout, b * i4);
-    PQL_T(t->dp_layer_s, h->dp_ls, b * L * d);
-    PQL_T(t->dp_lower, h->dp_lo, b * L * d);
-    PQL_T(t->dp_upper, h->dp_up, b * L * d);
-    PQL_T(t->dp_chosen, h->dp_chosen, b * L * i4);
-    PQL_T(t->dp_vehicle_l, h->dp_vl, b * d);
-    PQL_T(t->post_offsets, h->post_off, b * L * d);
-    PQL_T(t->post_status, h->post_status, b * i4);
-    PQL_T(t->post_iters, h->post_iters, b * i4);
-    PQL_T(t->ref_spline, h->r_rows, b * PQP_SPLINE_ROWS * L * d);
-    PQL_T(t->max_s, h->max_s, b * d);
-    PQL_T(t->states, h->states, b * PQP_STATE_ROWS * N * d);
-    PQL_T(t->curvature, h->curv, b * N * d);
-    PQL_T(t->total, h->total, b * i4);
-    PQL_T(t->bounds, h->bnd, b * PQP_BOUND_ROWS * N * d);
-    PQL_T(t->n_valid, h->n_valid, b * i4);
-    PQL_T(t->knots, h->knots, b * PQP_NFIELDS * N * d);
-    PQL_T(t->inst, h->inst, b * PQP_NINST * d);
-    PQL_T(t->p, h->p, b * i4);
-    PQL_T(t->sol1, h->sol1, b * 4 * N * d);
-    PQL_T(t->status1, h->status1, b * i4);
-    PQL_T(t->iters1, h->iters1, b * i4);
-    const size_t nv = 6 * N - 1, m = 6 * N + 2;  // pqp_batch_out's x_full / y_full / z_full strides
-    PQL_T(t->x_full1, h->full[0], b * nv * d);
-    PQL_T(t->y_full1, h->full[1], b * m * d);
-    PQL_T(t->z_full1, h->full[2], b * m * d);
-    PQL_T(t->x_full2, h->full[3], b * nv * d);
-    PQL_T(t->y_full2, h->full[4], b * m * d);
-    PQL_T(t->z_full2, h->full[5], b * m * d);
-    if (h->t_clear) PQL_T(t->tension_clearance, h->t_clear, b * P * d);
-    if (points) {
-        PQL_T(t->raw_r, h->raw_r, b * i4);
-        PQL_T(t->bspline_degree, h->bs_deg, b * i4);
+    // the handle's buffer behind each trace member; NULL where the call has none (tension_clearance under TENSION2,
+    // the B-spline fields outside pqp_plan_points)
+    pqp_plan_trace src{};
+    src.raw_spline = h->raw_rows;
+    src.seg_p = h->seg_p;
+    src.seg_x = h->seg[0];
+    src.seg_y = h->seg[1];
+    src.seg_angle = h->seg[2];
+    src.seg_k = h->seg[3];
+    src.seg_s = h->seg[4];
+    src.tension_x = h->t_x;
+    src.tension_y = h->t_y;
+    src.tension_s = h->t_s;
+    src.tension_status = h->t_status;
+    src.tension_iters = h->t_iters;
+    src.tension_spline = h->t_rows;
+    src.tension_length = h->t_len;
+    src.dp_status = h->dp_status;
+    src.dp_n_out = h->dp_nout;
+    src.dp_layer_s = h->dp_ls;
+    src.dp_lower = h->dp_lo;
+    src.dp_upper = h->dp_up;
+    src.dp_chosen = h->dp_chosen;
+    src.dp_vehicle_l = h->dp_vl;
+    src.post_offsets = h->post_off;
+    src.post_status = h->post_status;
+    src.post_iters = h->post_iters;
+    src.ref_spline = h->r_rows;
+    src.max_s = h->max_s;
+    src.states = h->states;
+    src.curvature = h->curv;
+    src.total = h->total;
+    src.bounds = h->bnd;
+    src.n_valid = h->n_valid;
+    src.knots = h->knots;
+    src.inst = h->inst;
+    src.p = h->p;
+    src.sol1 = h->sol1;
+    src.status1 = h->status1;
+    src.iters1 = h->iters1;
+    src.x_full1 = h->full[0];
+    src.y_full1 = h->full[1];
+    src.z_full1 = h->full[2];
+    src.x_full2 = h->full[3];
+    src.y_full2 = h->full[4];
+    src.z_full2 = h->full[5];
+    src.tension_clearance = h->t_clear;
+    src.raw_r = points ? h->raw_r : nullptr;
+    src.bspline_degree = points ? h->bs_deg : nullptr;
+    for (const pqpl::TraceField &f : pqpl::trace_fields(h->P, h->L, h->N, h->R)) {
+        const void *from = pqpl::trace_get(src, f);
+        if (!from) continue;
+        const int rc = copy_out(h, pqpl::trace_get(*t, f), from, (size_t)B * f.per_path, s);
+        if (rc != PQP_OK) return rc;
     }
-#undef PQL_T
     return PQP_OK;
 }
 

@@ -34,13 +34,15 @@ class PqpError(RuntimeError):
 def build_library(force=False, verbose=False):
     """nvcc-compile the CUDA library in-tree for sm_90a (no GPU needed to compile)."""
     root = os.path.dirname(_PKG)
-    cu = [os.path.join(_CSRC, f) for f in ("pqp_api.cu", "pqp_bounds.cu", "pqp_multi.cu", "pqp_smoother.cu")]
+    cu = [os.path.join(_CSRC, f) for f in ("pqp_api.cu", "pqp_bounds.cu", "pqp_multi.cu", "pqp_plan_multi.cu",
+                                         "pqp_smoother.cu")]
     deps = cu + [os.path.join(_CSRC, f) for f in ("pqp_kernel.cuh", "pqp_host_common.h", "pqp_bounds_core.cuh", "pqp_host_handle.h",
                                                   "pqp_dp.cu", "pqp_dp_core.cuh", "pqp_bounds_internal.h", "pqp_smoother_core.cuh",
                                                   "pqp_plan.cu", "pqp_plan_core.cuh", "pqp_smoother_internal.h",
-                                                  "pqp_map_core.cuh", "pqp_collision_core.cuh")]
+                                                  "pqp_map_core.cuh", "pqp_collision_core.cuh", "pqp_shard.h",
+                                                  "pqp_plan_trace.h")]
     deps += [os.path.join(root, "include", f) for f in ("pqp.h", "pqp_bounds.h", "pqp_multi.h", "pqp_dp.h", "pqp_smoother.h",
-                                                        "pqp_plan.h")]
+                                                        "pqp_plan.h", "pqp_plan_multi.h")]
     stale = not os.path.exists(LIB_PATH) or any(
         os.path.getmtime(s) > os.path.getmtime(LIB_PATH) for s in deps)
     if force or stale:
