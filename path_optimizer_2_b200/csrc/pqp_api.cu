@@ -19,6 +19,7 @@
 #include <vector>
 
 #include "../../include/pqp_multi.h"
+#include "pqp_batch_layout.h"
 #include "pqp_host_common.h"
 #include "pqp_host_handle.h"
 
@@ -276,6 +277,8 @@ __global__ void pack_results_kernel(int batch, const double *__restrict__ cost, 
     out[b] = r;
 }
 
+using SolveKernel = void (*)(pqp::KernelArgs);
+
 }  // namespace
 
 // ------------------------------------------------------------------ handle
@@ -307,6 +310,8 @@ struct pqp_handle {
     bool cold_only = false;        // params.reserved bit 128: no warm state is kept (pqp_resolve* is refused)
     float stage_ms[PQP_NSTAGES] = {0, 0, 0, 0, 0};
     cudaEvent_t ev_st[4] = {};     // stage boundaries of the single-stream host call
+    SolveKernel kernel = nullptr;  // the handle's solve kernel, chosen and prepared at create
+    SolveKernel kernel64 = nullptr;  // the FP64 kernel of the escalation (nullptr at C = 16), prepared on first use
     size_t smem_bytes64 = 0;
     bool prepared64 = false;
     int *d_flags = nullptr;
@@ -333,94 +338,37 @@ namespace {
 using pqp::DeviceGuard;
 using pqp::fail;
 
-// the increment form is only instantiated for FP32 (the FP64 kernel is exact in either form)
-template <int C, typename real, bool Incr>
-cudaError_t launch(const pqp::KernelArgs &ka, size_t smem, cudaStream_t s) {
-    pqp_admm_kernel<C, real, Incr><<<ka.batch, 32, smem, s>>>(ka);
-    return cudaGetLastError();
-}
-template <int C, typename real>
-cudaError_t launch_form(const pqp::KernelArgs &ka, size_t smem, cudaStream_t s, bool incr) {
-    if (incr && sizeof(real) == 4) return launch<C, float, true>(ka, smem, s);
-    return launch<C, real, false>(ka, smem, s);
-}
-// C = 16 exists for FP32 only under the shared-memory policy (144 KB per QP); FP64 uses the
-// global-memory kernel above
-template <typename real> struct Has16 { static constexpr bool value = sizeof(real) == 4; };
-template <typename real>
-cudaError_t launch_chunk(int chunk, const pqp::KernelArgs &ka, size_t smem, cudaStream_t s, bool incr = false) {
-    switch (chunk) {
-        case 1: return launch_form<1, real>(ka, smem, s, incr);
-        case 2: return launch_form<2, real>(ka, smem, s, incr);
-        case 4: return launch_form<4, real>(ka, smem, s, incr);
-        case 8: return launch_form<8, real>(ka, smem, s, incr);
-        default:
-            if constexpr (Has16<real>::value) return launch_form<16, real>(ka, smem, s, incr);
-            else return cudaErrorInvalidConfiguration;
+// The solve kernel of C stages for (FP64, increment form, persistent launch). The increment form is only instantiated
+// for FP32 (the FP64 kernel is exact in either form), and so is the persistent launch. FP64 at C = 16 has no
+// shared-memory kernel (288 KB per QP): nullptr, run_device launches pqp_admm_kernel_gmem instead.
+template <int C>
+SolveKernel kernel_for(bool fp64, bool incr, bool persistent) {
+    if (fp64) {
+        if constexpr (C == 16) return nullptr;
+        else return pqp_admm_kernel<C, double, false>;
     }
+    if (persistent) return incr ? pqp_admm_kernel_persistent<C, true> : pqp_admm_kernel_persistent<C, false>;
+    return incr ? pqp_admm_kernel<C, float, true> : pqp_admm_kernel<C, float, false>;
 }
-template <int C, typename real, bool Incr>
-cudaError_t prepare(size_t smem, int *blocks_per_sm) {
-    cudaError_t e = cudaFuncSetAttribute(pqp_admm_kernel<C, real, Incr>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    return cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks_per_sm, pqp_admm_kernel<C, real, Incr>, 32, smem);
-}
-template <int C, typename real>
-cudaError_t prepare_form(size_t smem, int *bps, bool incr) {
-    if (incr && sizeof(real) == 4) return prepare<C, float, true>(smem, bps);
-    return prepare<C, real, false>(smem, bps);
-}
-template <typename real>
-cudaError_t prepare_chunk(int chunk, size_t smem, int *bps, bool incr = false) {
+SolveKernel select_kernel(int chunk, bool fp64, bool incr, bool persistent) {
     switch (chunk) {
-        case 1: return prepare_form<1, real>(smem, bps, incr);
-        case 2: return prepare_form<2, real>(smem, bps, incr);
-        case 4: return prepare_form<4, real>(smem, bps, incr);
-        case 8: return prepare_form<8, real>(smem, bps, incr);
-        default:
-            if constexpr (Has16<real>::value) return prepare_form<16, real>(smem, bps, incr);
-            else { *bps = 2; return cudaSuccess; }  // global-memory kernel: nothing to prepare
+        case 1: return kernel_for<1>(fp64, incr, persistent);
+        case 2: return kernel_for<2>(fp64, incr, persistent);
+        case 4: return kernel_for<4>(fp64, incr, persistent);
+        case 8: return kernel_for<8>(fp64, incr, persistent);
+        default: return kernel_for<16>(fp64, incr, persistent);
     }
 }
 
-// persistent variant: min(batch, resident) one-warp CTAs, resident = SMs x CTAs per SM at this shared-memory size
-template <int C, bool Incr>
-cudaError_t launch_persistent(const pqp::KernelArgs &ka, size_t smem, cudaStream_t s, int resident) {
-    const int ctas = ka.batch < resident ? ka.batch : resident;
-    pqp_admm_kernel_persistent<C, Incr><<<ctas, 32, smem, s>>>(ka);
-    return cudaGetLastError();
-}
-template <int C>
-cudaError_t launch_persistent_form(const pqp::KernelArgs &ka, size_t smem, cudaStream_t s, int resident, bool incr) {
-    return incr ? launch_persistent<C, true>(ka, smem, s, resident) : launch_persistent<C, false>(ka, smem, s, resident);
-}
-cudaError_t launch_persistent_chunk(int chunk, const pqp::KernelArgs &ka, size_t smem, cudaStream_t s, int resident, bool incr) {
-    switch (chunk) {
-        case 1: return launch_persistent_form<1>(ka, smem, s, resident, incr);
-        case 2: return launch_persistent_form<2>(ka, smem, s, resident, incr);
-        case 4: return launch_persistent_form<4>(ka, smem, s, resident, incr);
-        case 8: return launch_persistent_form<8>(ka, smem, s, resident, incr);
-        default: return launch_persistent_form<16>(ka, smem, s, resident, incr);
+// opts `k` in to `smem` bytes of dynamic shared memory and counts its resident CTAs per SM
+cudaError_t prepare(SolveKernel k, size_t smem, int *blocks_per_sm) {
+    if (!k) {  // the global-memory kernel: nothing to prepare
+        *blocks_per_sm = 2;
+        return cudaSuccess;
     }
-}
-template <int C, bool Incr>
-cudaError_t prepare_persistent(size_t smem, int *blocks_per_sm) {
-    cudaError_t e = cudaFuncSetAttribute(pqp_admm_kernel_persistent<C, Incr>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    return cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks_per_sm, pqp_admm_kernel_persistent<C, Incr>, 32, smem);
-}
-template <int C>
-cudaError_t prepare_persistent_form(size_t smem, int *bps, bool incr) {
-    return incr ? prepare_persistent<C, true>(smem, bps) : prepare_persistent<C, false>(smem, bps);
-}
-cudaError_t prepare_persistent_chunk(int chunk, size_t smem, int *bps, bool incr) {
-    switch (chunk) {
-        case 1: return prepare_persistent_form<1>(smem, bps, incr);
-        case 2: return prepare_persistent_form<2>(smem, bps, incr);
-        case 4: return prepare_persistent_form<4>(smem, bps, incr);
-        case 8: return prepare_persistent_form<8>(smem, bps, incr);
-        default: return prepare_persistent_form<16>(smem, bps, incr);
-    }
+    return cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks_per_sm, k, 32, smem);
 }
 
 int validate_batch(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *out) {
@@ -475,29 +423,29 @@ int run_device(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *out, 
     ka.dy = esc ? h->e_dy : h->d_dy;
     ka.rho_state = esc ? h->e_rho : h->d_rho;
     if (timed) PQP_CUDA(h->err, cudaEventRecord(h->ev0, s));
-    if (esc || h->fp64) {
-        if (!h->prepared64) {
-            int bps = 0;
-            PQP_CUDA(h->err, prepare_chunk<double>(h->chunk, h->smem_bytes64, &bps));
-            h->prepared64 = true;
-        }
-        if (h->chunk == 16) {
-            const int ctas = std::min(ka.batch, 2 * h->sm_count);
-            if (!h->d_state64) PQP_CUDA(h->err, h->res.alloc(h->d_state64, (size_t)2 * h->sm_count * pqp::smem_floats(16)));
-            pqp_admm_kernel_gmem<16, double, false><<<ctas, 32, 0, s>>>(ka, h->d_state64);
-            PQP_CUDA(h->err, cudaGetLastError());
-        } else {
-            PQP_CUDA(h->err, launch_chunk<double>(h->chunk, ka, h->smem_bytes64, s));
-        }
-    } else if (h->persistent) {
-        // one work counter per concurrently running launch (pipeline chunk); counters rotate
-        int *ctr = h->d_counters + (h->counter_next++ % pqp_handle::kCounters);
-        PQP_CUDA(h->err, cudaMemsetAsync(ctr, 0, sizeof(int), s));
-        ka.work_counter = ctr;
-        PQP_CUDA(h->err, launch_persistent_chunk(h->chunk, ka, h->smem_bytes, s, h->sm_count * h->warps_per_sm, h->incr));
-    } else {
-        PQP_CUDA(h->err, launch_chunk<float>(h->chunk, ka, h->smem_bytes, s, h->incr));
+    const bool fp64 = esc || h->fp64;
+    if (fp64 && !h->prepared64) {
+        int bps = 0;
+        PQP_CUDA(h->err, prepare(h->kernel64, h->smem_bytes64, &bps));
+        h->prepared64 = true;
     }
+    if (fp64 && h->chunk == 16) {
+        const int ctas = std::min(ka.batch, 2 * h->sm_count);
+        if (!h->d_state64) PQP_CUDA(h->err, h->res.alloc(h->d_state64, (size_t)2 * h->sm_count * pqp::smem_floats(16)));
+        pqp_admm_kernel_gmem<16, double, false><<<ctas, 32, 0, s>>>(ka, h->d_state64);
+    } else {
+        int ctas = ka.batch;
+        if (!fp64 && h->persistent) {
+            // one work counter per concurrently running launch (pipeline chunk); counters rotate; min(batch, resident)
+            // one-warp CTAs, resident = SMs x CTAs per SM at this shared-memory size
+            int *ctr = h->d_counters + (h->counter_next++ % pqp_handle::kCounters);
+            PQP_CUDA(h->err, cudaMemsetAsync(ctr, 0, sizeof(int), s));
+            ka.work_counter = ctr;
+            ctas = std::min(ka.batch, h->sm_count * h->warps_per_sm);
+        }
+        (fp64 ? h->kernel64 : h->kernel)<<<ctas, 32, fp64 ? h->smem_bytes64 : h->smem_bytes, s>>>(ka);
+    }
+    PQP_CUDA(h->err, cudaGetLastError());
     if (timed) PQP_CUDA(h->err, cudaEventRecord(h->ev1, s));
     h->launches++;
     if (!esc) {
@@ -510,21 +458,22 @@ int run_device(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *out, 
 // The FP64 escalation's side batch of esc_cap instances, all or nothing: after a failed allocation it has no
 // buffers, so the next escalation allocates again instead of running with a missing one.
 cudaError_t alloc_escalation(pqp_handle *h) {
-    const size_t E = h->esc_cap, nmax = h->n_max, c = h->chunk, nvm = 6 * nmax - 1, mm = 6 * nmax + 2;
+    const size_t E = h->esc_cap, c = h->chunk;
+    const auto batch_of = [&](auto member) { return E * pqp::per_instance(member, h->n_max); };
     pqp::Resources &r = h->res;
     return r.group([&] {
-        cudaError_t e = r.alloc(h->e_knots, E * PQP_NFIELDS * nmax);
-        if (e == cudaSuccess) e = r.alloc(h->e_inst, E * PQP_NINST);
-        if (e == cudaSuccess) e = r.alloc(h->e_n, E);
-        if (e == cudaSuccess) e = r.alloc(h->e_p, E);
-        if (e == cudaSuccess) e = r.alloc(h->e_sol, E * 4 * nmax);
-        if (e == cudaSuccess) e = r.alloc(h->e_cost, E);
-        if (e == cudaSuccess) e = r.alloc(h->e_status, E);
-        if (e == cudaSuccess) e = r.alloc(h->e_iters, E);
-        if (e == cudaSuccess) e = r.alloc(h->e_info, E * PQP_NINFO);
-        if (e == cudaSuccess) e = r.alloc(h->e_xf, E * nvm);
-        if (e == cudaSuccess) e = r.alloc(h->e_yf, E * mm);
-        if (e == cudaSuccess) e = r.alloc(h->e_zf, E * mm);
+        cudaError_t e = r.alloc(h->e_knots, batch_of(&pqp_batch_in::knots));
+        if (e == cudaSuccess) e = r.alloc(h->e_inst, batch_of(&pqp_batch_in::inst));
+        if (e == cudaSuccess) e = r.alloc(h->e_n, batch_of(&pqp_batch_in::n));
+        if (e == cudaSuccess) e = r.alloc(h->e_p, batch_of(&pqp_batch_in::p));
+        if (e == cudaSuccess) e = r.alloc(h->e_sol, batch_of(&pqp_batch_out::sol));
+        if (e == cudaSuccess) e = r.alloc(h->e_cost, batch_of(&pqp_batch_out::cost));
+        if (e == cudaSuccess) e = r.alloc(h->e_status, batch_of(&pqp_batch_out::status));
+        if (e == cudaSuccess) e = r.alloc(h->e_iters, batch_of(&pqp_batch_out::iters));
+        if (e == cudaSuccess) e = r.alloc(h->e_info, batch_of(&pqp_batch_out::info));
+        if (e == cudaSuccess) e = r.alloc(h->e_xf, batch_of(&pqp_batch_out::x_full));
+        if (e == cudaSuccess) e = r.alloc(h->e_yf, batch_of(&pqp_batch_out::y_full));
+        if (e == cudaSuccess) e = r.alloc(h->e_zf, batch_of(&pqp_batch_out::z_full));
         if (e == cudaSuccess) e = r.alloc(h->e_warm, E * pqp::warm_floats(c) * sizeof(double));
         if (e == cudaSuccess) e = r.alloc(h->e_scal, E * pqp::scal_floats(c) * sizeof(double));
         if (e == cudaSuccess) e = r.alloc(h->e_dy, E * pqp::dy_floats(c) * sizeof(double));
@@ -539,7 +488,7 @@ cudaError_t alloc_escalation(pqp_handle *h) {
 // the FP64 instantiation of the same kernel: FP32 iterates resolve |A'dy| < 1e-4 |dy| only to
 // ~5e-4 (DESIGN.md), FP64 ones reproduce the reference's PRIMAL_INFEASIBLE status. Rare path,
 // plain synchronous copies.
-int escalate_fp64(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *out, int B) {
+int escalate_fp64(pqp_handle *h, const pqp_batch_in &dev_in, const pqp_batch_out *out, int B) {
     std::vector<int> idx;
     for (int b = 0; b < B; ++b)
         // also an "inaccurate" certificate at the iteration cap: in FP32 the 10x-tolerance test can
@@ -550,45 +499,30 @@ int escalate_fp64(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *ou
     if (idx.empty()) return PQP_OK;
     const int nmax = h->n_max;
     const size_t c = h->chunk;
-    const size_t nvm = 6 * (size_t)nmax - 1, mm = 6 * (size_t)nmax + 2;
     if (!h->e_knots) {
         h->esc_cap = h->batch_max < 256 ? h->batch_max : 256;
         PQP_CUDA(h->err, alloc_escalation(h));
     }
     cudaStream_t s = h->stream;
-    const size_t kb = (size_t)PQP_NFIELDS * nmax;
+    // inputs come from the handle's device copy dev_in (valid for both host-batch and NULL-batch calls)
+    const pqp_batch_in e_in = {h->esc_cap, nmax, h->e_knots, h->e_inst, h->e_n, h->d_p_valid ? h->e_p : nullptr};
+    const pqp_batch_out e_out = {h->e_sol, h->e_cost, h->e_status, h->e_iters, h->e_xf, h->e_yf, h->e_zf, h->e_info};
+    const pqp_batch_out e_full = {nullptr, nullptr, nullptr, nullptr, h->e_xf, h->e_yf, h->e_zf, nullptr};
+    // the device-resident results are kept coherent too (resolve(NULL) linearises about d_sol)
+    const pqp_batch_out resident = {h->d_sol, h->d_cost, h->d_status, h->d_iters, nullptr, nullptr, nullptr, nullptr};
     for (size_t start = 0; start < idx.size(); start += h->esc_cap) {
         const int E = (int)std::min(idx.size() - start, (size_t)h->esc_cap);
-        for (int j = 0; j < E; ++j) {
-            const int b = idx[start + j];
-            // inputs come from the handle's device copy (valid for both host-batch and NULL-batch calls)
-            PQP_CUDA(h->err, cudaMemcpyAsync(h->e_knots + j * kb, h->d_knots + b * kb, kb * sizeof(double), cudaMemcpyDeviceToDevice, s));
-            PQP_CUDA(h->err, cudaMemcpyAsync(h->e_inst + (size_t)j * PQP_NINST, h->d_inst + (size_t)b * PQP_NINST, PQP_NINST * sizeof(double), cudaMemcpyDeviceToDevice, s));
-            PQP_CUDA(h->err, cudaMemcpyAsync(h->e_n + j, h->d_n + b, sizeof(int), cudaMemcpyDeviceToDevice, s));
-            if (h->d_p_valid) PQP_CUDA(h->err, cudaMemcpyAsync(h->e_p + j, h->d_p + b, sizeof(int), cudaMemcpyDeviceToDevice, s));
-        }
-        PQP_CUDA(h->err, cudaMemsetAsync(h->e_xf, 0, (size_t)E * nvm * sizeof(double), s));
-        PQP_CUDA(h->err, cudaMemsetAsync(h->e_yf, 0, (size_t)E * mm * sizeof(double), s));
-        PQP_CUDA(h->err, cudaMemsetAsync(h->e_zf, 0, (size_t)E * mm * sizeof(double), s));
-        pqp_batch_in din = {E, nmax, h->e_knots, h->e_inst, h->e_n, h->d_p_valid ? h->e_p : nullptr};
-        pqp_batch_out dout = {h->e_sol, h->e_cost, h->e_status, h->e_iters, h->e_xf, h->e_yf, h->e_zf, h->e_info};
-        int rc = run_device(h, &din, &dout, 0, s, false, 0, true, nullptr);
+        for (int j = 0; j < E; ++j)
+            PQP_CUDA(h->err, pqp::copy_batch(e_in, j, dev_in, idx[start + j], 1, nmax, cudaMemcpyDeviceToDevice, s));
+        PQP_CUDA(h->err, pqp::zero_batch(e_full, 0, E, nmax, s));
+        pqp_batch_in din = e_in;
+        din.batch = E;
+        int rc = run_device(h, &din, &e_out, 0, s, false, 0, true, nullptr);
         if (rc) return rc;
         for (int j = 0; j < E; ++j) {
             const int b = idx[start + j];
-            PQP_CUDA(h->err, cudaMemcpyAsync(out->sol + (size_t)b * 4 * nmax, h->e_sol + (size_t)j * 4 * nmax, 4 * (size_t)nmax * sizeof(double), cudaMemcpyDeviceToHost, s));
-            if (out->cost) PQP_CUDA(h->err, cudaMemcpyAsync(out->cost + b, h->e_cost + j, sizeof(double), cudaMemcpyDeviceToHost, s));
-            if (out->status) PQP_CUDA(h->err, cudaMemcpyAsync(out->status + b, h->e_status + j, sizeof(int), cudaMemcpyDeviceToHost, s));
-            if (out->iters) PQP_CUDA(h->err, cudaMemcpyAsync(out->iters + b, h->e_iters + j, sizeof(int), cudaMemcpyDeviceToHost, s));
-            if (out->info) PQP_CUDA(h->err, cudaMemcpyAsync(out->info + (size_t)b * PQP_NINFO, h->e_info + (size_t)j * PQP_NINFO, PQP_NINFO * sizeof(double), cudaMemcpyDeviceToHost, s));
-            if (out->x_full) PQP_CUDA(h->err, cudaMemcpyAsync(out->x_full + b * nvm, h->e_xf + j * nvm, nvm * sizeof(double), cudaMemcpyDeviceToHost, s));
-            if (out->y_full) PQP_CUDA(h->err, cudaMemcpyAsync(out->y_full + b * mm, h->e_yf + j * mm, mm * sizeof(double), cudaMemcpyDeviceToHost, s));
-            if (out->z_full) PQP_CUDA(h->err, cudaMemcpyAsync(out->z_full + b * mm, h->e_zf + j * mm, mm * sizeof(double), cudaMemcpyDeviceToHost, s));
-            // keep the device-resident results coherent too (resolve(NULL) linearises about d_sol)
-            PQP_CUDA(h->err, cudaMemcpyAsync(h->d_sol + (size_t)b * 4 * nmax, h->e_sol + (size_t)j * 4 * nmax, 4 * (size_t)nmax * sizeof(double), cudaMemcpyDeviceToDevice, s));
-            PQP_CUDA(h->err, cudaMemcpyAsync(h->d_status + b, h->e_status + j, sizeof(int), cudaMemcpyDeviceToDevice, s));
-            PQP_CUDA(h->err, cudaMemcpyAsync(h->d_cost + b, h->e_cost + j, sizeof(double), cudaMemcpyDeviceToDevice, s));
-            PQP_CUDA(h->err, cudaMemcpyAsync(h->d_iters + b, h->e_iters + j, sizeof(int), cudaMemcpyDeviceToDevice, s));
+            PQP_CUDA(h->err, pqp::copy_batch(*out, b, e_out, j, 1, nmax, cudaMemcpyDeviceToHost, s));
+            PQP_CUDA(h->err, pqp::copy_batch(resident, b, e_out, j, 1, nmax, cudaMemcpyDeviceToDevice, s));
         }
         // the warm slots of these instances adopt the FP64 run's scaled iterates and rho
         if (!h->cold_only) {
@@ -612,9 +546,9 @@ int escalate_fp64(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *ou
 // chunk its next instance belongs to has landed; finished chunks are announced through mapped
 // host memory (host_done[chunk]) so their D2H copies overlap the rest of the solve. Compared
 // with one launch per chunk this removes the per-launch tail of a persistent kernel.
-int run_host_streamed(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *out, int mode, int B) {
+int run_host_streamed(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *out, const pqp_batch_in &dev_in,
+                      const pqp_batch_out &dev_out, const pqp_batch_out &dev_full, int mode, int B) {
     const int nmax = h->n_max;
-    const size_t nvm = 6 * (size_t)nmax - 1, mm = 6 * (size_t)nmax + 2;
     // up to kStreams chunks of >= 256 instances: small batches (configs[1]: 1024) still overlap
     // their copies with the solve, large ones (8192) move 1024 instances per chunk
     const int min_chunk = 256;
@@ -641,15 +575,10 @@ int run_host_streamed(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out
     for (int c = 0; c < pqp_handle::kStreams; ++c) h->h_done[c] = 0;
     PQP_CUDA(h->err, cudaMemsetAsync(h->d_ready, 0, pqp_handle::kStreams * sizeof(int), sk));
     PQP_CUDA(h->err, cudaMemsetAsync(h->d_done, 0, pqp_handle::kStreams * sizeof(int), sk));
-    if (out->x_full) PQP_CUDA(h->err, cudaMemsetAsync(h->d_xf, 0, (size_t)B * nvm * sizeof(double), sk));
-    if (out->y_full) PQP_CUDA(h->err, cudaMemsetAsync(h->d_yf, 0, (size_t)B * mm * sizeof(double), sk));
-    if (out->z_full) PQP_CUDA(h->err, cudaMemsetAsync(h->d_zf, 0, (size_t)B * mm * sizeof(double), sk));
+    PQP_CUDA(h->err, pqp::zero_batch(dev_full, 0, B, nmax, sk));
     PQP_CUDA(h->err, cudaEventRecord(h->ev0, sk));
     PQP_CUDA(h->err, cudaStreamWaitEvent(sc, h->ev0, 0));
     PQP_CUDA(h->err, cudaStreamWaitEvent(sd, h->ev0, 0));
-    pqp_batch_in din = {B, nmax, h->d_knots, h->d_inst, h->d_n, (h->d_p_valid = in->p != nullptr) ? h->d_p : nullptr};
-    pqp_batch_out dout = {h->d_sol, h->d_cost, h->d_status, h->d_iters, out->x_full ? h->d_xf : nullptr,
-                          out->y_full ? h->d_yf : nullptr, out->z_full ? h->d_zf : nullptr, h->d_info};
     StreamedLaunch sl;
     sl.ready = h->d_ready;
     sl.done = h->d_done;
@@ -660,17 +589,11 @@ int run_host_streamed(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out
     // kernel still overlaps them, and a tool that makes launches blocking (ncu serialises kernels)
     // cannot leave the kernel waiting for copies the host has not issued yet.
     for (int c = 0; c < nchunks; ++c) {
-        const int lo = lo_of[c], hi = lo_of[c + 1];
-        const size_t nb = (size_t)(hi - lo);
-        PQP_CUDA(h->err, cudaMemcpyAsync(h->d_knots + (size_t)lo * PQP_NFIELDS * nmax, in->knots + (size_t)lo * PQP_NFIELDS * nmax,
-                                    nb * PQP_NFIELDS * nmax * sizeof(double), cudaMemcpyHostToDevice, sc));
-        PQP_CUDA(h->err, cudaMemcpyAsync(h->d_inst + (size_t)lo * PQP_NINST, in->inst + (size_t)lo * PQP_NINST,
-                                    nb * PQP_NINST * sizeof(double), cudaMemcpyHostToDevice, sc));
-        PQP_CUDA(h->err, cudaMemcpyAsync(h->d_n + lo, in->n + lo, nb * sizeof(int), cudaMemcpyHostToDevice, sc));
-        if (in->p) PQP_CUDA(h->err, cudaMemcpyAsync(h->d_p + lo, in->p + lo, nb * sizeof(int), cudaMemcpyHostToDevice, sc));
+        const int lo = lo_of[c];
+        PQP_CUDA(h->err, pqp::copy_batch(dev_in, lo, *in, lo, lo_of[c + 1] - lo, nmax, cudaMemcpyHostToDevice, sc));
         PQP_CUDA(h->err, cudaMemsetAsync(h->d_ready + c, 1, sizeof(int), sc));  // "chunk c has landed"
     }
-    int rc = run_device(h, &din, &dout, mode, sk, false, 0, false, h->d_flags, &sl);
+    int rc = run_device(h, &dev_in, &dev_out, mode, sk, false, 0, false, h->d_flags, &sl);
     if (rc) return rc;
     h->host_inputs_resident = true;
     for (int c = 0; c < nchunks; ++c) {
@@ -688,14 +611,7 @@ int run_host_streamed(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out
         }
         PQP_CUDA(h->err, cudaMemcpyAsync(h->h_status + lo, h->d_status + lo, nb * sizeof(int), cudaMemcpyDeviceToHost, sd));
         PQP_CUDA(h->err, cudaMemcpyAsync(h->h_flags + lo, h->d_flags + lo, nb * sizeof(int), cudaMemcpyDeviceToHost, sd));
-        PQP_CUDA(h->err, cudaMemcpyAsync(out->sol + (size_t)lo * 4 * nmax, h->d_sol + (size_t)lo * 4 * nmax, nb * 4 * nmax * sizeof(double), cudaMemcpyDeviceToHost, sd));
-        if (out->cost) PQP_CUDA(h->err, cudaMemcpyAsync(out->cost + lo, h->d_cost + lo, nb * sizeof(double), cudaMemcpyDeviceToHost, sd));
-        if (out->status) PQP_CUDA(h->err, cudaMemcpyAsync(out->status + lo, h->d_status + lo, nb * sizeof(int), cudaMemcpyDeviceToHost, sd));
-        if (out->iters) PQP_CUDA(h->err, cudaMemcpyAsync(out->iters + lo, h->d_iters + lo, nb * sizeof(int), cudaMemcpyDeviceToHost, sd));
-        if (out->info) PQP_CUDA(h->err, cudaMemcpyAsync(out->info + (size_t)lo * PQP_NINFO, h->d_info + (size_t)lo * PQP_NINFO, nb * PQP_NINFO * sizeof(double), cudaMemcpyDeviceToHost, sd));
-        if (out->x_full) PQP_CUDA(h->err, cudaMemcpyAsync(out->x_full + lo * nvm, h->d_xf + lo * nvm, nb * nvm * sizeof(double), cudaMemcpyDeviceToHost, sd));
-        if (out->y_full) PQP_CUDA(h->err, cudaMemcpyAsync(out->y_full + lo * mm, h->d_yf + lo * mm, nb * mm * sizeof(double), cudaMemcpyDeviceToHost, sd));
-        if (out->z_full) PQP_CUDA(h->err, cudaMemcpyAsync(out->z_full + lo * mm, h->d_zf + lo * mm, nb * mm * sizeof(double), cudaMemcpyDeviceToHost, sd));
+        PQP_CUDA(h->err, pqp::copy_batch(*out, lo, dev_out, lo, nb, nmax, cudaMemcpyDeviceToHost, sd));
     }
     h->last_batch = B;
     PQP_CUDA(h->err, cudaStreamSynchronize(sk));
@@ -705,7 +621,7 @@ int run_host_streamed(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out
     PQP_CUDA(h->err, cudaEventElapsedTime(&h->last_ms, h->ev0, h->ev1));
     for (int i = 0; i < PQP_NSTAGES; ++i) h->stage_ms[i] = -1.0f;  // copies and kernel overlap: only the total is defined
     h->stage_ms[PQP_STAGE_TOTAL] = h->last_ms;
-    if (!h->fp64 && h->escalate && mode == 0) return escalate_fp64(h, in, out, B);
+    if (!h->fp64 && h->escalate && mode == 0) return escalate_fp64(h, dev_in, out, B);
     return PQP_OK;
 }
 
@@ -740,13 +656,6 @@ int run_host(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *out, in
         if (mode == 1 && (!h->solved || B != h->last_batch)) return fail(h->err, PQP_E_STATE, "resolve needs a previous solve of the same batch");
         h->host_inputs_resident = true;
         h->d_p_valid = in->p != nullptr;
-        if (h->persistent && B >= 512) {
-            const size_t nvm0 = 6 * (size_t)nmax - 1, mm0 = 6 * (size_t)nmax + 2;
-            if (out->x_full && !h->d_xf) PQP_CUDA(h->err, h->res.alloc(h->d_xf, (size_t)h->batch_max * nvm0));
-            if (out->y_full && !h->d_yf) PQP_CUDA(h->err, h->res.alloc(h->d_yf, (size_t)h->batch_max * mm0));
-            if (out->z_full && !h->d_zf) PQP_CUDA(h->err, h->res.alloc(h->d_zf, (size_t)h->batch_max * mm0));
-            return run_host_streamed(h, in, out, mode, B);
-        }
     } else {
         if (mode != 1) return fail(h->err, PQP_E_INVALID, "null batch");
         if (h->cold_only) return fail(h->err, PQP_E_STATE, "cold-only handle (option bit 128) keeps no warm state");
@@ -759,10 +668,18 @@ int run_host(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *out, in
         h->launches++;
     }
     // optional full outputs are allocated on first use
-    const size_t nvm = 6 * (size_t)nmax - 1, mm = 6 * (size_t)nmax + 2;
-    if (out->x_full && !h->d_xf) PQP_CUDA(h->err, h->res.alloc(h->d_xf, (size_t)h->batch_max * nvm));
-    if (out->y_full && !h->d_yf) PQP_CUDA(h->err, h->res.alloc(h->d_yf, (size_t)h->batch_max * mm));
-    if (out->z_full && !h->d_zf) PQP_CUDA(h->err, h->res.alloc(h->d_zf, (size_t)h->batch_max * mm));
+    const auto batch_of = [&](auto member) { return (size_t)h->batch_max * pqp::per_instance(member, nmax); };
+    if (out->x_full && !h->d_xf) PQP_CUDA(h->err, h->res.alloc(h->d_xf, batch_of(&pqp_batch_out::x_full)));
+    if (out->y_full && !h->d_yf) PQP_CUDA(h->err, h->res.alloc(h->d_yf, batch_of(&pqp_batch_out::y_full)));
+    if (out->z_full && !h->d_zf) PQP_CUDA(h->err, h->res.alloc(h->d_zf, batch_of(&pqp_batch_out::z_full)));
+    // the handle's device buffers as one batch: inputs, outputs, and the requested full outputs alone (zeroed before a
+    // solve: the kernel writes an instance's first nv / m entries only)
+    const pqp_batch_in dev_in = {B, nmax, h->d_knots, h->d_inst, h->d_n, h->d_p_valid ? h->d_p : nullptr};
+    const pqp_batch_out dev_full = {nullptr, nullptr, nullptr, nullptr, out->x_full ? h->d_xf : nullptr,
+                                    out->y_full ? h->d_yf : nullptr, out->z_full ? h->d_zf : nullptr, nullptr};
+    const pqp_batch_out dev_out = {h->d_sol,         h->d_cost,       h->d_status,     h->d_iters,
+                                   dev_full.x_full, dev_full.y_full, dev_full.z_full, h->d_info};
+    if (in && h->persistent && B >= 512) return run_host_streamed(h, in, out, dev_in, dev_out, dev_full, mode, B);
     // Chunked pipeline, one stream per chunk: chunk c+1's H2D copy and chunk c-1's D2H copy
     // overlap chunk c's kernel (fully asynchronous when the caller's buffers are pinned), and
     // because every chunk's kernel sits in its own stream the block scheduler back-fills SMs
@@ -783,47 +700,18 @@ int run_host(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *out, in
         if (lo >= hi) break;
         const size_t nb = (size_t)(hi - lo);
         cudaStream_t s = streams[c];
-        if (in) {
-            PQP_CUDA(h->err, cudaMemcpyAsync(h->d_knots + (size_t)lo * PQP_NFIELDS * nmax, in->knots + (size_t)lo * PQP_NFIELDS * nmax,
-                                        nb * PQP_NFIELDS * nmax * sizeof(double), cudaMemcpyHostToDevice, s));
-            PQP_CUDA(h->err, cudaMemcpyAsync(h->d_inst + (size_t)lo * PQP_NINST, in->inst + (size_t)lo * PQP_NINST,
-                                        nb * PQP_NINST * sizeof(double), cudaMemcpyHostToDevice, s));
-            PQP_CUDA(h->err, cudaMemcpyAsync(h->d_n + lo, in->n + lo, nb * sizeof(int), cudaMemcpyHostToDevice, s));
-            if (in->p) PQP_CUDA(h->err, cudaMemcpyAsync(h->d_p + lo, in->p + lo, nb * sizeof(int), cudaMemcpyHostToDevice, s));
-        }
-        if (out->x_full) PQP_CUDA(h->err, cudaMemsetAsync(h->d_xf + lo * nvm, 0, nb * nvm * sizeof(double), s));
-        if (out->y_full) PQP_CUDA(h->err, cudaMemsetAsync(h->d_yf + lo * mm, 0, nb * mm * sizeof(double), s));
-        if (out->z_full) PQP_CUDA(h->err, cudaMemsetAsync(h->d_zf + lo * mm, 0, nb * mm * sizeof(double), s));
+        if (in) PQP_CUDA(h->err, pqp::copy_batch(dev_in, lo, *in, lo, nb, nmax, cudaMemcpyHostToDevice, s));
+        PQP_CUDA(h->err, pqp::zero_batch(dev_full, lo, nb, nmax, s));
         if (nchunks == 1) PQP_CUDA(h->err, cudaEventRecord(h->ev_st[0], s));
-        pqp_batch_in din;
+        pqp_batch_in din = pqp::batch_from(dev_in, lo, nmax);
         din.batch = (int32_t)nb;
-        din.n_max = nmax;
-        din.knots = h->d_knots + (size_t)lo * PQP_NFIELDS * nmax;
-        din.inst = h->d_inst + (size_t)lo * PQP_NINST;
-        din.n = h->d_n + lo;
-        din.p = h->d_p_valid ? h->d_p + lo : nullptr;
-        pqp_batch_out dout;
-        dout.sol = h->d_sol + (size_t)lo * 4 * nmax;
-        dout.cost = h->d_cost + lo;
-        dout.status = h->d_status + lo;
-        dout.iters = h->d_iters + lo;
-        dout.x_full = out->x_full ? h->d_xf + lo * nvm : nullptr;
-        dout.y_full = out->y_full ? h->d_yf + lo * mm : nullptr;
-        dout.z_full = out->z_full ? h->d_zf + lo * mm : nullptr;
-        dout.info = h->d_info + (size_t)lo * PQP_NINFO;
+        const pqp_batch_out dout = pqp::batch_from(dev_out, lo, nmax);
         rc = run_device(h, &din, &dout, mode, s, false, lo, false, h->d_flags + lo);
         if (rc) return rc;
         if (nchunks == 1) PQP_CUDA(h->err, cudaEventRecord(h->ev_st[1], s));
         PQP_CUDA(h->err, cudaMemcpyAsync(h->h_status + lo, dout.status, nb * sizeof(int), cudaMemcpyDeviceToHost, s));
         PQP_CUDA(h->err, cudaMemcpyAsync(h->h_flags + lo, h->d_flags + lo, nb * sizeof(int), cudaMemcpyDeviceToHost, s));
-        PQP_CUDA(h->err, cudaMemcpyAsync(out->sol + (size_t)lo * 4 * nmax, dout.sol, nb * 4 * nmax * sizeof(double), cudaMemcpyDeviceToHost, s));
-        if (out->cost) PQP_CUDA(h->err, cudaMemcpyAsync(out->cost + lo, dout.cost, nb * sizeof(double), cudaMemcpyDeviceToHost, s));
-        if (out->status) PQP_CUDA(h->err, cudaMemcpyAsync(out->status + lo, dout.status, nb * sizeof(int), cudaMemcpyDeviceToHost, s));
-        if (out->iters) PQP_CUDA(h->err, cudaMemcpyAsync(out->iters + lo, dout.iters, nb * sizeof(int), cudaMemcpyDeviceToHost, s));
-        if (out->info) PQP_CUDA(h->err, cudaMemcpyAsync(out->info + (size_t)lo * PQP_NINFO, dout.info, nb * PQP_NINFO * sizeof(double), cudaMemcpyDeviceToHost, s));
-        if (out->x_full) PQP_CUDA(h->err, cudaMemcpyAsync(out->x_full + lo * nvm, dout.x_full, nb * nvm * sizeof(double), cudaMemcpyDeviceToHost, s));
-        if (out->y_full) PQP_CUDA(h->err, cudaMemcpyAsync(out->y_full + lo * mm, dout.y_full, nb * mm * sizeof(double), cudaMemcpyDeviceToHost, s));
-        if (out->z_full) PQP_CUDA(h->err, cudaMemcpyAsync(out->z_full + lo * mm, dout.z_full, nb * mm * sizeof(double), cudaMemcpyDeviceToHost, s));
+        PQP_CUDA(h->err, pqp::copy_batch(*out, lo, dev_out, lo, nb, nmax, cudaMemcpyDeviceToHost, s));
     }
     h->last_batch = B;
     // join: stream[0] waits for every chunk stream; ev1 marks the end of the whole pipeline
@@ -848,7 +736,7 @@ int run_host(pqp_handle *h, const pqp_batch_in *in, const pqp_batch_out *out, in
     // cap (receding horizon) is; the increment-form kernel certifies infeasibility by itself there
     if (!h->fp64 && h->escalate && mode == 0) {
         PQP_CUDA(h->err, cudaEventRecord(h->ev_st[2], streams[0]));
-        rc = escalate_fp64(h, in, out, B);
+        rc = escalate_fp64(h, dev_in, out, B);
         if (rc) return rc;
         PQP_CUDA(h->err, cudaEventRecord(h->ev_st[3], streams[0]));
         PQP_CUDA(h->err, cudaEventSynchronize(h->ev_st[3]));
@@ -915,15 +803,11 @@ int pqp_create(const pqp_params *params, int32_t n_max, int32_t batch_max, int32
         // increment form for n_max >= 64, textbook form below; bits 32 / 64 force one or the other.
         h->incr = !h->fp64 && ((params->reserved & 32) != 0 || ((params->reserved & 64) == 0 && h->chunk >= 4));
         h->smem_bytes64 = pqp::smem_floats(h->chunk) * sizeof(double) + 16;
+        h->kernel = select_kernel(h->chunk, h->fp64, h->incr, h->persistent);
+        h->kernel64 = select_kernel(h->chunk, true, false, false);
+        h->prepared64 = h->fp64;
         int bps = 0;
-        if (h->fp64) {
-            PQP_CUDA(g_create_error, prepare_chunk<double>(h->chunk, h->smem_bytes64, &bps));
-            h->prepared64 = true;
-        } else if (h->persistent) {
-            PQP_CUDA(g_create_error, prepare_persistent_chunk(h->chunk, h->smem_bytes, &bps, h->incr));
-        } else {
-            PQP_CUDA(g_create_error, prepare_chunk<float>(h->chunk, h->smem_bytes, &bps, h->incr));
-        }
+        PQP_CUDA(g_create_error, prepare(h->kernel, h->fp64 ? h->smem_bytes64 : h->smem_bytes, &bps));
         if (bps < 1) return fail(g_create_error, PQP_E_CUDA, "the solve kernel does not fit on an SM");
         h->warps_per_sm = bps;
         pqp::Resources &r = h->res;
@@ -935,15 +819,16 @@ int pqp_create(const pqp_params *params, int32_t n_max, int32_t batch_max, int32
         PQP_CUDA(g_create_error, r.event(h->ev0));
         PQP_CUDA(g_create_error, r.event(h->ev1));
         const size_t B = batch_max, c = h->chunk;
-        PQP_CUDA(g_create_error, r.alloc(h->d_knots, B * PQP_NFIELDS * n_max));
-        PQP_CUDA(g_create_error, r.alloc(h->d_inst, B * PQP_NINST));
-        PQP_CUDA(g_create_error, r.alloc(h->d_n, B));
-        PQP_CUDA(g_create_error, r.alloc(h->d_p, B));
-        PQP_CUDA(g_create_error, r.alloc(h->d_sol, B * 4 * n_max));
-        PQP_CUDA(g_create_error, r.alloc(h->d_cost, B));
-        PQP_CUDA(g_create_error, r.alloc(h->d_status, B));
-        PQP_CUDA(g_create_error, r.alloc(h->d_iters, B));
-        PQP_CUDA(g_create_error, r.alloc(h->d_info, B * PQP_NINFO));
+        const auto batch_of = [&](auto member) { return B * pqp::per_instance(member, n_max); };
+        PQP_CUDA(g_create_error, r.alloc(h->d_knots, batch_of(&pqp_batch_in::knots)));
+        PQP_CUDA(g_create_error, r.alloc(h->d_inst, batch_of(&pqp_batch_in::inst)));
+        PQP_CUDA(g_create_error, r.alloc(h->d_n, batch_of(&pqp_batch_in::n)));
+        PQP_CUDA(g_create_error, r.alloc(h->d_p, batch_of(&pqp_batch_in::p)));
+        PQP_CUDA(g_create_error, r.alloc(h->d_sol, batch_of(&pqp_batch_out::sol)));
+        PQP_CUDA(g_create_error, r.alloc(h->d_cost, batch_of(&pqp_batch_out::cost)));
+        PQP_CUDA(g_create_error, r.alloc(h->d_status, batch_of(&pqp_batch_out::status)));
+        PQP_CUDA(g_create_error, r.alloc(h->d_iters, batch_of(&pqp_batch_out::iters)));
+        PQP_CUDA(g_create_error, r.alloc(h->d_info, batch_of(&pqp_batch_out::info)));
         const size_t esz = h->fp64 ? sizeof(double) : sizeof(float);
         // Warm state (scaled x, z, y and rho: the OSQP workspace that persists between solve and
         // updateProblemFormulationAndSolve) is per instance; a cold-only handle keeps none. The Ruiz
@@ -967,7 +852,7 @@ int pqp_create(const pqp_params *params, int32_t n_max, int32_t batch_max, int32
         PQP_CUDA(g_create_error, cudaMemset(h->d_flags, 0, B * sizeof(int)));
         PQP_CUDA(g_create_error, r.alloc_host(h->h_status, B));
         PQP_CUDA(g_create_error, r.alloc_host(h->h_flags, B));
-        PQP_CUDA(g_create_error, cudaMemset(h->d_sol, 0, B * 4 * n_max * sizeof(double)));
+        PQP_CUDA(g_create_error, cudaMemset(h->d_sol, 0, batch_of(&pqp_batch_out::sol) * sizeof(double)));
         return PQP_OK;
     }();
     if (rc != PQP_OK) {

@@ -12,6 +12,7 @@
 #include <vector>
 
 #include "../../include/pqp_multi.h"
+#include "pqp_batch_layout.h"
 #include "pqp_host_handle.h"
 #include "pqp_shard.h"
 
@@ -94,31 +95,15 @@ int run(pqp_multi *m, const pqp_batch_in *in, const pqp_batch_out *out, bool war
     if (warm && B != m->last_batch) return fail(m->err, PQP_E_STATE, "resolve needs a previous solve of the same batch");
     const int G = m->n_dev, nmax = m->n_max;
     const int per = pqp::shard_per(B, G);
-    const size_t nvm = 6 * (size_t)nmax - 1, mm = 6 * (size_t)nmax + 2;
     std::vector<int> rc(G, PQP_OK);
     // one host thread per device: each runs that device's own (pipelined, synchronous) host call
     pqp::fan_out(G, [&](int d) {
         const pqp::Shard sh = pqp::shard_of(B, per, d);
         const int lo = sh.first, hi = sh.first + sh.count;
         if (lo >= hi) return;
-        pqp_batch_in din;
-        pqp_batch_out dout = {};
-        dout.sol = out->sol + (size_t)lo * 4 * nmax;
-        dout.cost = out->cost ? out->cost + lo : nullptr;
-        dout.status = out->status ? out->status + lo : nullptr;
-        dout.iters = out->iters ? out->iters + lo : nullptr;
-        dout.x_full = out->x_full ? out->x_full + (size_t)lo * nvm : nullptr;
-        dout.y_full = out->y_full ? out->y_full + (size_t)lo * mm : nullptr;
-        dout.z_full = out->z_full ? out->z_full + (size_t)lo * mm : nullptr;
-        dout.info = out->info ? out->info + (size_t)lo * PQP_NINFO : nullptr;
-        if (in) {
-            din.batch = hi - lo;
-            din.n_max = nmax;
-            din.knots = in->knots + (size_t)lo * PQP_NFIELDS * nmax;
-            din.inst = in->inst + (size_t)lo * PQP_NINST;
-            din.n = in->n + lo;
-            din.p = in->p ? in->p + lo : nullptr;
-        }
+        pqp_batch_in din = in ? pqp::batch_from(*in, lo, nmax) : pqp_batch_in{};
+        din.batch = hi - lo;
+        const pqp_batch_out dout = pqp::batch_from(*out, lo, nmax);
         rc[d] = warm ? pqp_resolve(m->h[d], in ? &din : nullptr, &dout) : pqp_solve(m->h[d], &din, &dout);
     });
     for (int d = 0; d < G; ++d)

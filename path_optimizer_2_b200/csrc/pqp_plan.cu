@@ -883,7 +883,8 @@ int pqp_plan_create_maps(const pqp_bounds_map *maps, int32_t n_maps, const pqp_p
         PQP_CUDA(err, r.alloc(h->iters1, B));
         PQP_CUDA(err, r.alloc(h->status2, B));
         PQP_CUDA(err, r.alloc(h->iters2, B));
-        for (int i = 0; i < 6; ++i) PQP_CUDA(err, r.alloc(h->full[i], B * (i % 3 == 0 ? 6 * N - 1 : 6 * N + 2)));
+        for (int i = 0; i < 6; ++i)
+            PQP_CUDA(err, r.alloc(h->full[i], B * pqp::per_instance(i % 3 == 0 ? &pqp_batch_out::x_full : &pqp_batch_out::y_full, N)));
         if (h->prm.smoothing_method == PQP_PLAN_SMOOTH_TENSION) PQP_CUDA(err, r.alloc(h->t_clear, B * P));
         PQP_CUDA(err, r.alloc(h->pt_x, B * R));
         PQP_CUDA(err, r.alloc(h->pt_y, B * R));

@@ -8,6 +8,7 @@
 #include <cstring>
 
 #include "../../include/pqp_plan.h"
+#include "pqp_batch_layout.h"
 
 namespace pqpl {
 
@@ -22,7 +23,7 @@ constexpr int kTraceFields = (int)(sizeof(pqp_plan_trace) / sizeof(void *));
 // in the member order of pqp_plan_trace
 inline std::array<TraceField, kTraceFields> trace_fields(size_t P, size_t L, size_t N, size_t R) {
     const size_t d = sizeof(double), i4 = sizeof(int32_t);
-    const size_t nv = 6 * N - 1, m = 6 * N + 2;  // pqp_batch_out's x_full / y_full / z_full strides
+    const size_t nv = pqp::per_instance(&pqp_batch_out::x_full, N), m = pqp::per_instance(&pqp_batch_out::y_full, N);
 #define PQL_F(member, bytes) TraceField{offsetof(pqp_plan_trace, member), (bytes)}
     const TraceField f[] = {
         PQL_F(raw_spline, PQP_SPLINE_ROWS * R * d), PQL_F(seg_p, i4), PQL_F(seg_x, P * d), PQL_F(seg_y, P * d),

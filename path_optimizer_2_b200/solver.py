@@ -40,7 +40,7 @@ def build_library(force=False, verbose=False):
                                                   "pqp_dp.cu", "pqp_dp_core.cuh", "pqp_bounds_internal.h", "pqp_smoother_core.cuh",
                                                   "pqp_plan.cu", "pqp_plan_core.cuh", "pqp_smoother_internal.h",
                                                   "pqp_map_core.cuh", "pqp_collision_core.cuh", "pqp_shard.h",
-                                                  "pqp_plan_trace.h")]
+                                                  "pqp_plan_trace.h", "pqp_batch_layout.h")]
     deps += [os.path.join(root, "include", f) for f in ("pqp.h", "pqp_bounds.h", "pqp_multi.h", "pqp_dp.h", "pqp_smoother.h",
                                                         "pqp_plan.h", "pqp_plan_multi.h")]
     stale = not os.path.exists(LIB_PATH) or any(
