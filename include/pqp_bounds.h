@@ -152,7 +152,9 @@ int pqp_bounds_get_map(pqp_bounds_handle *h, pqp_bounds_map *meta, float *distan
 /* Per-path maps: a handle holds n_maps map slots (1 <= n_maps <= PQP_MAX_MAP_SLOTS), each with the capacity of the
  * largest of the maps it was created with; the *_mapped calls plan path b on slot map_index[b]. A handle made by
  * pqp_bounds_create has one slot, and every call above acts on slot 0. Memory: 5 bytes per cell per slot (the float
- * layer and the 1-byte occupancy staging), allocated at create; a failed allocation returns PQP_E_CUDA.
+ * layer and the 1-byte occupancy staging), plus the staging of the host set_occupancy_boxes call: PQP_MAX_BOXES *
+ * PQP_BOX_FIELDS doubles (2.5 MiB) and 4 bytes per slot; all allocated at create, a failed allocation returns
+ * PQP_E_CUDA.
  *
  * The map-reading kernels index a device table of the slots' metadata. Slot updates write their entries with a
  * kernel launch on the update's stream, so they keep the ordering of the calls above: work enqueued before an update
@@ -160,6 +162,7 @@ int pqp_bounds_get_map(pqp_bounds_handle *h, pqp_bounds_map *meta, float *distan
  *   set_map_slot(_device), and pqp_bounds_set_map(_device):        1 (the table entry; the layer is a copy)
  *   pqp_bounds_set_occupancy(_device):                             2 (the entry is written by the column pass)
  *   set_occupancy_slots(_device):   2 + ceil(count / PQP_MAP_TABLE_CHUNK) (column pass, row pass, table entries)
+ *   set_occupancy_boxes(_device):   the same (the boxes are stamped inside the column pass)
  *
  * A slot update is refused (PQP_E_INVALID, every slot untouched) for a slot outside [0, n_maps) or anything
  * pqp_bounds_set_map / pqp_bounds_set_occupancy refuse. */
@@ -187,6 +190,45 @@ int pqp_bounds_set_map_slot_device(pqp_bounds_handle *h, int32_t slot, const pqp
 int pqp_bounds_set_occupancy_slots(pqp_bounds_handle *h, int32_t first_slot, const pqp_occupancy_stack *stack);
 int pqp_bounds_set_occupancy_slots_device(pqp_bounds_handle *h, int32_t first_slot, const pqp_occupancy_stack *stack,
                                           void *stream);
+/* Obstacle boxes per slot on a static occupancy image (a tick of tracked vehicles and pedestrians on a fixed map).
+ *
+ * A box is PQP_BOX_FIELDS doubles x, y, heading, length, width in the map's world frame (the frame of the paths),
+ * placed like the car of the collision check: centred at (x, y), its length along the heading. Cell (i, j) of a slot
+ * is an obstacle when its base image byte is <= obstacle_max (as in pqp_bounds_set_occupancy), or when its centre
+ * lies inside or on the boundary of any box of that slot:
+ *     px = cx + (half_lx - (i + 0.5) res)     py = cy + (half_ly - (j + 0.5) res)     (the pqp_bounds_map convention,
+ *                                              half_lx = 0.5 * rows * res, half_ly = 0.5 * cols * res)
+ *     dx = px - x   dy = py - y   c = cos(heading)   s = sin(heading)
+ *     u  = dx c + dy s              v = dy c - dx s
+ *     inside  <=>  |u| <= 0.5 length  &&  |v| <= 0.5 width
+ * Every product and sum rounds on its own (no fused multiply-add); c and s are computed in FP64 on the device. So a
+ * box with a NaN field or a negative length or width stamps nothing, a box of zero size stamps only a cell whose
+ * centre it hits exactly, and a box partly or wholly off the map stamps the cells it covers, or none. The slot's layer
+ * is then the exact distance transform of the combined obstacles, as pqp_bounds_set_occupancy documents it (scipy's
+ * distance_transform_edt bit for bit). The base image is read and never written.
+ *
+ * base: count, rows, cols, resolution, obstacle_max and the per-slot centres as in pqp_bounds_set_occupancy_slots, into
+ *   slots first_slot .. first_slot + count - 1. shared_base = 1: base->cells is one [rows][cols] image every slot starts
+ *   from; 0: count images [count][rows][cols].
+ * boxes: slot first_slot + s gets boxes->boxes[s][0 .. k[s] - 1].
+ * The host form takes host pointers, stages the image(s) and the boxes into buffers allocated at create and returns
+ * when done; the device form takes device pointers (base->cells, k and boxes; the centres stay host arrays) and is
+ * asynchronous on `stream`, with the ordering of set_occupancy_slots_device and no host synchronisation. The device
+ * form clamps k[s] to [0, k_max]; the host form refuses a k[s] outside it.
+ * Refused with PQP_E_INVALID, every slot untouched: anything set_occupancy_slots refuses, shared_base not 0 or 1, a
+ * NULL boxes, k_max < 0, count * k_max > PQP_MAX_BOXES, k_max > 0 with a NULL k or boxes->boxes, and (host form) a
+ * k[s] outside [0, k_max]. */
+#define PQP_BOX_FIELDS 5      /* x, y, heading, length, width */
+#define PQP_MAX_BOXES 65536   /* count * k_max per call, every form */
+typedef struct pqp_obstacle_boxes {
+    int32_t k_max;            /* row stride of boxes, >= 0; k and boxes may be NULL when 0 */
+    const int32_t *k;         /* [count]: boxes of slot first_slot + s */
+    const double *boxes;      /* [count][k_max][PQP_BOX_FIELDS] */
+} pqp_obstacle_boxes;
+int pqp_bounds_set_occupancy_boxes(pqp_bounds_handle *h, int32_t first_slot, const pqp_occupancy_stack *base,
+                                   int32_t shared_base, const pqp_obstacle_boxes *boxes);
+int pqp_bounds_set_occupancy_boxes_device(pqp_bounds_handle *h, int32_t first_slot, const pqp_occupancy_stack *base,
+                                          int32_t shared_base, const pqp_obstacle_boxes *boxes, void *stream);
 /* As pqp_bounds_get_map for one slot. */
 int pqp_bounds_get_map_slot(pqp_bounds_handle *h, int32_t slot, pqp_bounds_map *meta, float *distance);
 int32_t pqp_bounds_map_count(const pqp_bounds_handle *h);

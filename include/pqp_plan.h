@@ -202,8 +202,8 @@ int pqp_plan_get_map(pqp_plan_handle *h, pqp_bounds_map *meta, float *distance);
  * checked in the chain's first glue kernel, so a mapped call takes the launches of the unmapped one (23 / 24 / 25 /
  * 26); a path with an index outside [0, n_maps) gets PQP_PLAN_MAP_INDEX and no other path changes. Slot updates
  * are ordered like pqp_plan_set_map_device and counted by pqp_plan_launch_count: set_map(_device) and
- * set_map_slot(_device) 1 launch, set_occupancy(_device) 2, set_occupancy_slots(_device)
- * 2 + ceil(count / PQP_MAP_TABLE_CHUNK). */
+ * set_map_slot(_device) 1 launch, set_occupancy(_device) 2, set_occupancy_slots(_device) and
+ * set_occupancy_boxes(_device) 2 + ceil(count / PQP_MAP_TABLE_CHUNK). */
 int pqp_plan_create_maps(const pqp_bounds_map *maps, int32_t n_maps, const pqp_plan_params *params, int32_t r_max,
                          int32_t p_max, int32_t layers_max, int32_t n_max, int32_t batch_max, int32_t device,
                          pqp_plan_handle **out);
@@ -219,6 +219,11 @@ int pqp_plan_set_map_slot_device(pqp_plan_handle *h, int32_t slot, const pqp_bou
 int pqp_plan_set_occupancy_slots(pqp_plan_handle *h, int32_t first_slot, const pqp_occupancy_stack *stack);
 int pqp_plan_set_occupancy_slots_device(pqp_plan_handle *h, int32_t first_slot, const pqp_occupancy_stack *stack,
                                         void *stream);
+/* pqp_bounds_set_occupancy_boxes(_device) on the plan's slots: a static image plus each slot's obstacle boxes. */
+int pqp_plan_set_occupancy_boxes(pqp_plan_handle *h, int32_t first_slot, const pqp_occupancy_stack *base,
+                                 int32_t shared_base, const pqp_obstacle_boxes *boxes);
+int pqp_plan_set_occupancy_boxes_device(pqp_plan_handle *h, int32_t first_slot, const pqp_occupancy_stack *base,
+                                        int32_t shared_base, const pqp_obstacle_boxes *boxes, void *stream);
 int pqp_plan_get_map_slot(pqp_plan_handle *h, int32_t slot, pqp_bounds_map *meta, float *distance);
 int32_t pqp_plan_map_count(const pqp_plan_handle *h);
 /* The footprint collision check of pqp_bounds.h on the plan's map slots, e.g. on a plan's final paths (out.path,

@@ -10,7 +10,9 @@
  * Memory: every device holds every slot, as pqp_plan_create_maps allocates it (a float32 distance layer and the uint8
  * staging of the host-form occupancy update: 5 B per cell per slot, 2.55 GB for 1024 demo-sized slots), and each
  * device other than the home one 1 B per cell per slot more: the staging that the device-form occupancy update
- * peer-copies the images into. A device's plan handle holds ceil(batch_max / n_devices) paths.
+ * peer-copies the images into, plus PQP_MAX_BOXES * PQP_BOX_FIELDS doubles (2.5 MiB) and 4 B per slot: the staging
+ * the device-form box update peer-copies the boxes into. A device's plan handle holds ceil(batch_max / n_devices)
+ * paths.
  *
  * The footprint collision check is not sharded (about 0.3 ms per 1024 paths against about 13 ms for the plan on an
  * H100): the home device holds every slot, so run pqp_plan_collision_check*_device on pqp_plan_multi_handle(m, 0) over
@@ -73,6 +75,14 @@ int pqp_plan_multi_set_map_slot(pqp_plan_multi_t *m, int32_t slot, const pqp_bou
 int pqp_plan_multi_set_occupancy_slots(pqp_plan_multi_t *m, int32_t first_slot, const pqp_occupancy_stack *stack);
 int pqp_plan_multi_set_occupancy_slots_device(pqp_plan_multi_t *m, int32_t first_slot, const pqp_occupancy_stack *stack,
                                               void *stream);
+/* pqp_plan_set_occupancy_boxes(_device) on every device, as the occupancy_slots forms above: the home handle first
+ * (its refusal refuses the call on every device); the device form peer-copies the base image(s), k and the boxes to
+ * every other device, and `stream` waits for every device. PQP_MAX_BOXES caps every form alike, so a call a single
+ * plan handle accepts is accepted here. */
+int pqp_plan_multi_set_occupancy_boxes(pqp_plan_multi_t *m, int32_t first_slot, const pqp_occupancy_stack *base,
+                                       int32_t shared_base, const pqp_obstacle_boxes *boxes);
+int pqp_plan_multi_set_occupancy_boxes_device(pqp_plan_multi_t *m, int32_t first_slot, const pqp_occupancy_stack *base,
+                                              int32_t shared_base, const pqp_obstacle_boxes *boxes, void *stream);
 /* as pqp_plan_get_map_slot on device index i's handle */
 int pqp_plan_multi_get_map_slot(pqp_plan_multi_t *m, int32_t device_index, int32_t slot, pqp_bounds_map *meta,
                                 float *distance);

@@ -24,10 +24,12 @@ EXPORTED_SYMBOLS = [
     "pqp_bounds_set_occupancy_slots", "pqp_bounds_set_occupancy_slots_device", "pqp_bounds_get_map_slot",
     "pqp_bounds_map_count", "pqp_bounds_compute_mapped", "pqp_bounds_compute_mapped_device",
     "pqp_bounds_collision_check", "pqp_bounds_collision_check_device", "pqp_bounds_collision_check_mapped",
-    "pqp_bounds_collision_check_mapped_device",
+    "pqp_bounds_collision_check_mapped_device", "pqp_bounds_set_occupancy_boxes", "pqp_bounds_set_occupancy_boxes_device",
 ]
 MAX_MAP_SLOTS = 65535
 MAP_TABLE_CHUNK = 1024  # table entries per table-write launch of a slot update
+BOX_FIELDS = 5  # x, y, heading, length, width of an obstacle box
+MAX_BOXES = 65536  # count * k_max of one set_occupancy_boxes call
 
 
 class BoundsMap(C.Structure):
@@ -46,6 +48,39 @@ class OccupancyStack(C.Structure):
     """pqp_occupancy_stack: `count` uint8 images [count, rows, cols] with one centre each (host arrays)."""
     _fields_ = [("count", C.c_int32), ("rows", C.c_int32), ("cols", C.c_int32), ("resolution", C.c_double),
                 ("center_x", C.c_void_p), ("center_y", C.c_void_p), ("cells", C.c_void_p), ("obstacle_max", C.c_int32)]
+
+
+class ObstacleBoxes(C.Structure):
+    """pqp_obstacle_boxes: k [count] boxes per slot out of boxes [count, k_max, BOX_FIELDS]."""
+    _fields_ = [("k_max", C.c_int32), ("k", C.c_void_p), ("boxes", C.c_void_p)]
+
+
+def pack_boxes(boxes, k, count):
+    """(float64 [count, k_max, BOX_FIELDS], int32 [count]) from `boxes` [count, k_max, BOX_FIELDS] with `k` (None: all
+    k_max), or from a list of `count` arrays [k_s, BOX_FIELDS]."""
+    if isinstance(boxes, (list, tuple)):
+        assert k is None and len(boxes) == count, "a list of boxes takes no k and has one entry per slot"
+        per = [np.asarray(b, dtype=np.float64).reshape(-1, BOX_FIELDS) for b in boxes]
+        k = np.array([len(b) for b in per], dtype=np.int32)
+        packed = np.zeros((count, int(k.max(initial=0)), BOX_FIELDS))
+        for s, b in enumerate(per):
+            packed[s, :len(b)] = b
+        return packed, k
+    packed = np.ascontiguousarray(boxes, dtype=np.float64)
+    assert packed.ndim == 3 and packed.shape[0] == count and packed.shape[2] == BOX_FIELDS
+    k = np.full(count, packed.shape[1], np.int32) if k is None else np.ascontiguousarray(k, dtype=np.int32)
+    assert k.shape == (count,)
+    return packed, k
+
+
+def box_base(shape, count=None):
+    """(count, shared_base, (rows, cols)) of a base image shape: [rows, cols] shared by `count` slots, or [count, rows,
+    cols]."""
+    if len(shape) == 2:
+        assert count is not None, "a shared base image needs the slot count (from the boxes)"
+        return int(count), 1, tuple(int(v) for v in shape)
+    assert len(shape) == 3
+    return int(shape[0]), 0, tuple(int(v) for v in shape[1:])
 
 
 def occupancy_stack(cells_ptr, shape, resolution, centers, obstacle_max):
@@ -166,6 +201,7 @@ def _declare(L):
     L.pqp_bounds_compute_mapped.argtypes = [vp, C.POINTER(BoundsIn), vp, C.POINTER(BoundsOut)]
     L.pqp_bounds_compute_mapped_device.argtypes = [vp, C.POINTER(BoundsIn), vp, C.POINTER(BoundsOut), vp]
     declare_collision(L, "pqp_bounds_")
+    declare_boxes(L, "pqp_bounds_")
     L._pqp_bounds_declared = True
     return L
 
@@ -177,6 +213,39 @@ def declare_collision(L, prefix):
     getattr(L, prefix + "collision_check_device").argtypes = [vp, cin, cout, vp]
     getattr(L, prefix + "collision_check_mapped").argtypes = [vp, cin, vp, cout]
     getattr(L, prefix + "collision_check_mapped_device").argtypes = [vp, cin, vp, cout, vp]
+
+
+def declare_boxes(L, prefix):
+    """The two set_occupancy_boxes entry points of the ABI `prefix` (pqp_bounds_, pqp_plan_, pqp_plan_multi_)."""
+    vp, st, bx = C.c_void_p, C.POINTER(OccupancyStack), C.POINTER(ObstacleBoxes)
+    getattr(L, prefix + "set_occupancy_boxes").argtypes = [vp, C.c_int32, st, C.c_int32, bx]
+    getattr(L, prefix + "set_occupancy_boxes_device").argtypes = [vp, C.c_int32, st, C.c_int32, bx, vp]
+
+
+def boxes_call(fn, h, base, resolution, boxes, k, centers, obstacle_max, first_slot):
+    """`fn` (a host-form set_occupancy_boxes) on host arrays, as MapSlots.set_occupancy_boxes documents them."""
+    base = np.ascontiguousarray(base, dtype=np.uint8)
+    n = len(boxes) if base.ndim == 2 else None
+    count, shared, (rows, cols) = box_base(base.shape, n)
+    packed, k = pack_boxes(boxes, k, count)
+    st, _keep = occupancy_stack(base.ctypes.data, (count, rows, cols), resolution, centers, obstacle_max)
+    ob = ObstacleBoxes(packed.shape[1], k.ctypes.data, packed.ctypes.data)
+    return fn(h, int(first_slot), C.byref(st), shared, C.byref(ob))
+
+
+def boxes_call_device(fn, h, base, resolution, boxes, k, centers, obstacle_max, first_slot, stream):
+    """`fn` (a device-form set_occupancy_boxes) on torch CUDA tensors, as MapSlots.set_occupancy_boxes_device documents
+    them; `stream` a raw cudaStream_t."""
+    import torch
+    assert base.is_cuda and base.is_contiguous() and base.dtype == torch.uint8 and base.dim() in (2, 3)
+    assert boxes.is_cuda and boxes.is_contiguous() and boxes.dtype == torch.float64 and boxes.dim() == 3
+    assert boxes.shape[2] == BOX_FIELDS
+    count, shared, (rows, cols) = box_base(tuple(base.shape), int(boxes.shape[0]))
+    assert int(boxes.shape[0]) == count
+    assert k.is_cuda and k.is_contiguous() and k.dtype == torch.int32 and tuple(k.shape) == (count,)
+    st, _keep = occupancy_stack(base.data_ptr(), (count, rows, cols), resolution, centers, obstacle_max)
+    ob = ObstacleBoxes(int(boxes.shape[1]), k.data_ptr(), boxes.data_ptr())
+    return fn(h, int(first_slot), C.byref(st), shared, C.byref(ob), C.c_void_p(stream))
 
 
 class MapSlots:
@@ -251,6 +320,24 @@ class MapSlots:
         assert imgs.is_cuda and imgs.is_contiguous() and imgs.dtype == torch.uint8 and imgs.dim() == 3
         st, _keep = occupancy_stack(imgs.data_ptr(), imgs.shape, resolution, centers, obstacle_max)
         self._check(self._fn("set_occupancy_slots_device")(self.h, int(first_slot), C.byref(st), C.c_void_p(stream)))
+
+    def set_occupancy_boxes(self, base, resolution, boxes, k=None, centers=None, obstacle_max=0, *, first_slot=0):
+        """Slots first_slot .. + count - 1 := the exact distance transforms of a static occupancy image plus each slot's
+        obstacle boxes, stamped on the GPU (host, synchronous). `base` uint8 [rows, cols] (every slot starts from it) or
+        [count, rows, cols]; `boxes` float64 [count, k_max, 5] (x, y, heading, length, width in the map's frame) with
+        `k` [count] boxes per slot (None: all k_max), or a list of `count` arrays [k_s, 5]. A cell is an obstacle when
+        its base value <= obstacle_max or its centre lies in or on one of its slot's boxes (include/pqp_bounds.h)."""
+        self._check(boxes_call(self._fn("set_occupancy_boxes"), self.h, base, resolution, boxes, k, centers,
+                               obstacle_max, first_slot))
+
+    def set_occupancy_boxes_device(self, base, resolution, boxes, k, centers=None, obstacle_max=0, *, first_slot=0,
+                                   stream=0):
+        """As `set_occupancy_boxes` from torch CUDA tensors: `base` uint8 [rows, cols] or [count, rows, cols], `boxes`
+        float64 [count, k_max, 5], `k` int32 [count] (clamped to [0, k_max] on the device). Asynchronous on `stream` (a
+        raw cudaStream_t), ordered as `set_occupancy_slots_device`; the tensors must stay alive until the stream has
+        run the update."""
+        self._check(boxes_call_device(self._fn("set_occupancy_boxes_device"), self.h, base, resolution, boxes, k,
+                                      centers, obstacle_max, first_slot, stream))
 
     def get_map(self, slot=0):
         """-> (float32 distance layer [rows, cols], resolution, (center_x, center_y)) of the current map (of `slot`);

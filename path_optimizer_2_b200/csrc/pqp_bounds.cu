@@ -14,6 +14,7 @@
 #include <new>
 #include <optional>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/pqp_bounds.h"
@@ -215,17 +216,73 @@ __global__ void map_table_kernel(const TableWrite w) {
     w.table[w.first + i] = m;
 }
 
+// The column pass's stamping argument: NoBoxes for the plain images, SlotBoxes for pqp_bounds_set_occupancy_boxes*.
+struct NoBoxes {};
+struct SlotBoxes {
+    const pqb::MapView *table;  // the slots' table entries from the first slot on (their centres), written before
+    const double *boxes;        // [count][k_max][kBoxFields]
+    const int32_t *k;           // [count], clamped to [0, k_max]; not read when k_max = 0
+    int k_max;
+    size_t img_stride;          // bytes from one slot's base image to the next: 0 when every slot shares one
+};
+
+// The box instantiation's work for column j of slot blockIdx.y: base image into g, the slot's boxes stamped in chunks
+// of one box per thread, then the two sweeps. Each chunk is loaded once per block (one sincos per box) and only the
+// boxes that can reach the block's columns are kept.
+__device__ __forceinline__ void stamped_column(const uint8_t *__restrict__ img, int rows, int cols, int obstacle_max,
+                                               int32_t *__restrict__ g, size_t slot_cells, const SlotBoxes &sb) {
+    __shared__ pqm::Box live[kEdtColumnThreads];
+    __shared__ int n_live;
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    const size_t y = blockIdx.y;
+    img += y * sb.img_stride;
+    g += y * slot_cells;
+    int kb = sb.k_max > 0 ? sb.k[y] : 0;
+    kb = kb < 0 ? 0 : (kb > sb.k_max ? sb.k_max : kb);
+    if (kb == 0) {  // uniform in the block: the plain column pass
+        if (j < cols) pqm::column_pass(img, rows, cols, j, obstacle_max, g);
+        return;
+    }
+    const pqb::MapView mv = sb.table[y];
+    const pqm::Cells m{rows, cols, mv.res, mv.half_lx, mv.half_ly, mv.cx, mv.cy};
+    const double ms = pqm::map_slack(m);
+    const int j0 = blockIdx.x * blockDim.x, j1 = (j0 + (int)blockDim.x < cols ? j0 + (int)blockDim.x : cols) - 1;
+    const double py_hi = pqm::cell_py(m, j0) + ms, py_lo = pqm::cell_py(m, j1) - ms;
+    const double py = pqm::cell_py(m, j < cols ? j : j1);
+    if (j < cols) pqm::column_init(img, rows, cols, j, obstacle_max, g);
+    const double *bs = sb.boxes + y * (size_t)sb.k_max * pqm::kBoxFields;
+    for (int first = 0; first < kb; first += kEdtColumnThreads) {
+        if (threadIdx.x == 0) n_live = 0;
+        __syncthreads();
+        const int b = first + threadIdx.x;
+        pqm::Box box;
+        if (b < kb && pqm::make_box(bs + (size_t)b * pqm::kBoxFields, box) && pqm::box_reaches(box, py_lo, py_hi))
+            live[atomicAdd(&n_live, 1)] = box;  // the order does not matter: stamps only ever set g = 0
+        __syncthreads();
+        if (j < cols)
+            for (int q = 0; q < n_live; ++q) pqm::stamp_column(g, m, j, py, ms, live[q]);
+        __syncthreads();
+    }
+    if (j < cols) pqm::column_sweeps(rows, cols, j, g);
+}
+
 // one thread per column of image blockIdx.y: consecutive threads read consecutive bytes of a row. Images are
 // rows * cols bytes apart, their g slot_cells int32 apart (in the layers of consecutive slots). A one-image update
-// also writes its slot's table entry (`entry_dst`, NULL for none) here, so it costs no launch of its own.
+// also writes its slot's table entry (`entry_dst`, NULL for none) here, so it costs no launch of its own. The SlotBoxes
+// instantiation stamps each slot's boxes into its image first (stamped_column; entry_dst is NULL there).
+template <class Stamp>
 __global__ void __launch_bounds__(kEdtColumnThreads) edt_column_kernel(const uint8_t *__restrict__ img, int rows, int cols,
                                                                         int obstacle_max, int32_t *__restrict__ g,
                                                                         size_t slot_cells, pqb::MapView *entry_dst,
-                                                                        const pqb::MapView entry) {
-    const int j = blockIdx.x * blockDim.x + threadIdx.x;
-    const size_t y = blockIdx.y;
-    if (entry_dst && j == 0 && y == 0) *entry_dst = entry;
-    if (j < cols) pqm::column_pass(img + y * rows * cols, rows, cols, j, obstacle_max, g + y * slot_cells);
+                                                                        const pqb::MapView entry, const Stamp stamp) {
+    if constexpr (std::is_same<Stamp, SlotBoxes>::value) {
+        stamped_column(img, rows, cols, obstacle_max, g, slot_cells, stamp);
+    } else {
+        const int j = blockIdx.x * blockDim.x + threadIdx.x;
+        const size_t y = blockIdx.y;
+        if (entry_dst && j == 0 && y == 0) *entry_dst = entry;
+        if (j < cols) pqm::column_pass(img + y * rows * cols, rows, cols, j, obstacle_max, g + y * slot_cells);
+    }
 }
 
 // one block per row of image blockIdx.y: the block loads the row's g, thread 0 builds the lower envelope, the block
@@ -263,6 +320,8 @@ struct pqp_bounds_handle {
     float *d_dist = nullptr;          // [n_maps][cap_cells] distance layers
     size_t cap_cells = 0;             // cells per slot: the largest map the handle was created with
     uint8_t *d_occ = nullptr;         // [n_maps][cap_cells] staging of the host set_occupancy calls' images
+    double *d_boxes = nullptr;        // [PQP_MAX_BOXES][PQP_BOX_FIELDS] staging of the host set_occupancy_boxes call
+    int32_t *d_box_k = nullptr;       // [n_maps] its box counts
     pqb::MapView *d_table = nullptr;  // [n_maps] the slots' metadata as the mapped kernels read it, in stream order
     std::unique_ptr<pqm::TableWrite> tw{new (std::nothrow) pqm::TableWrite};  // parameters of map_table_kernel
     cudaStream_t stream = nullptr;
@@ -395,17 +454,23 @@ int validate_slots(pqp_bounds_handle *h, long long first, long long count, const
 }
 
 // the two passes over `count` images of rows x cols (consecutive in `cells`) into slots first .. first + count - 1;
-// entry_dst (one image only): the table entry the column pass writes
+// entry_dst (one image only): the table entry the column pass writes; boxes: the slots' obstacle boxes (NULL for none),
+// whose column pass reads the slots' table entries, so those must be enqueued first
 int launch_edt(pqp_bounds_handle *h, int rows, int cols, double resolution, int obstacle_max, const uint8_t *cells,
-               int count, int first, pqb::MapView *entry_dst, const pqb::MapView &entry, cudaStream_t s) {
+               int count, int first, pqb::MapView *entry_dst, const pqb::MapView &entry, cudaStream_t s,
+               const pqm::SlotBoxes *boxes = nullptr) {
     const size_t smem = (size_t)pqm::kRowSmemPerCol * cols;
     // the dynamic share plus the kernel's static n_env may pass the 48 KB default at any width: always opt in
     PQP_CUDA(h->err, cudaFuncSetAttribute(pqm::edt_row_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     float *layer = slot_layer(h, first);
-    pqm::edt_column_kernel<<<dim3((cols + pqm::kEdtColumnThreads - 1) / pqm::kEdtColumnThreads, count),
-                             pqm::kEdtColumnThreads, 0, s>>>(cells, rows, cols, obstacle_max,
-                                                             reinterpret_cast<int32_t *>(layer), h->cap_cells, entry_dst,
-                                                             entry);
+    const dim3 grid((cols + pqm::kEdtColumnThreads - 1) / pqm::kEdtColumnThreads, count);
+    int32_t *g = reinterpret_cast<int32_t *>(layer);
+    if (boxes)
+        pqm::edt_column_kernel<<<grid, pqm::kEdtColumnThreads, 0, s>>>(cells, rows, cols, obstacle_max, g, h->cap_cells,
+                                                                       nullptr, entry, *boxes);
+    else
+        pqm::edt_column_kernel<<<grid, pqm::kEdtColumnThreads, 0, s>>>(cells, rows, cols, obstacle_max, g, h->cap_cells,
+                                                                       entry_dst, entry, pqm::NoBoxes{});
     PQP_CUDA(h->err, cudaGetLastError());
     pqm::edt_row_kernel<<<dim3(rows, count), pqm::kEdtRowThreads, smem, s>>>(layer, h->cap_cells, rows, cols,
                                                                              (float)resolution);
@@ -447,17 +512,56 @@ int validate_stack(pqp_bounds_handle *h, int first, const pqp_occupancy_stack *s
     return PQP_OK;
 }
 
+// `boxes` (NULL for none): the set_occupancy_boxes call's, with table and img_stride still to be filled in here. The
+// table entries go first: the box instantiation of the column pass reads the slots' centres from them.
 int set_occupancy_slots(pqp_bounds_handle *h, int first, const pqp_occupancy_stack *st, const uint8_t *cells,
-                        cudaStream_t s) {
+                        cudaStream_t s, const pqm::SlotBoxes *boxes = nullptr) {
     const pqb::MapView meta = make_view(slot_layer(h, first), st->rows, st->cols, st->resolution, 0.0, 0.0);
-    int rc = launch_edt(h, st->rows, st->cols, st->resolution, st->obstacle_max, cells, st->count, first, nullptr, meta, s);
+    int rc = write_table(h, first, st->count, meta, st->center_x, st->center_y, s);
     if (rc != PQP_OK) return rc;
-    rc = write_table(h, first, st->count, meta, st->center_x, st->center_y, s);
+    pqm::SlotBoxes sb{};
+    if (boxes) {
+        sb = *boxes;
+        sb.table = h->d_table + first;
+    }
+    rc = launch_edt(h, st->rows, st->cols, st->resolution, st->obstacle_max, cells, st->count, first, nullptr, meta, s,
+                    boxes ? &sb : nullptr);
     if (rc != PQP_OK) return rc;
     for (int i = 0; i < st->count; ++i)
         h->maps[first + i] = make_view(slot_layer(h, first + i), st->rows, st->cols, st->resolution, st->center_x[i],
                                        st->center_y[i]);
     return PQP_OK;
+}
+
+// what pqp_bounds_set_occupancy_boxes(_device) accept beyond validate_stack; `host`: the host form, which can read k
+int validate_boxes(pqp_bounds_handle *h, int first, const pqp_occupancy_stack *base, int shared_base,
+                   const pqp_obstacle_boxes *boxes, bool host, const char *what) {
+    int rc = validate_stack(h, first, base, what);
+    if (rc != PQP_OK) return rc;
+    std::string why;
+    if (shared_base != 0 && shared_base != 1) why = "shared_base must be 0 or 1";
+    else if (!boxes) why = "null boxes";
+    else if (boxes->k_max < 0) why = "k_max must be >= 0";
+    else if ((long long)base->count * boxes->k_max > PQP_MAX_BOXES)
+        why = "count * k_max = " + std::to_string((long long)base->count * boxes->k_max) + " exceeds PQP_MAX_BOXES (" +
+              std::to_string(PQP_MAX_BOXES) + ")";
+    else if (boxes->k_max > 0 && (!boxes->k || !boxes->boxes)) why = "null k or boxes with k_max > 0";
+    else if (host && boxes->k_max > 0)
+        for (int i = 0; i < base->count && why.empty(); ++i)
+            if (boxes->k[i] < 0 || boxes->k[i] > boxes->k_max)
+                why = "k[" + std::to_string(i) + "] = " + std::to_string(boxes->k[i]) + " outside [0, k_max]";
+    return why.empty() ? PQP_OK : fail(h->err, PQP_E_INVALID, std::string(what) + ": " + why);
+}
+
+// the box call once validated: `cells`, `k` and `xs` (the boxes) in device memory
+int set_occupancy_boxes(pqp_bounds_handle *h, int first, const pqp_occupancy_stack *base, const uint8_t *cells,
+                        int shared_base, const int32_t *k, const double *xs, int k_max, cudaStream_t s) {
+    pqm::SlotBoxes sb{};
+    sb.boxes = xs;
+    sb.k = k;
+    sb.k_max = k_max;
+    sb.img_stride = shared_base ? 0 : (size_t)base->rows * base->cols;
+    return set_occupancy_slots(h, first, base, cells, s, &sb);
 }
 
 int create(const pqp_bounds_map *maps, int n_maps, const pqp_bounds_params *params, int32_t device,
@@ -505,6 +609,8 @@ int create(const pqp_bounds_map *maps, int n_maps, const pqp_bounds_params *para
                                              std::to_string(cap) + " cells (" + std::to_string(total * sizeof(float)) +
                                              " bytes of layers): " + cudaGetErrorString(e));
         PQP_CUDA(err, h->res.alloc(h->d_occ, total));
+        PQP_CUDA(err, h->res.alloc(h->d_boxes, (size_t)PQP_MAX_BOXES * PQP_BOX_FIELDS));
+        PQP_CUDA(err, h->res.alloc(h->d_box_k, (size_t)n_maps));
         PQP_CUDA(err, h->res.alloc(h->d_table, (size_t)n_maps));
         h->maps.resize(n_maps);
         for (int i = 0; i < n_maps; ++i) {
@@ -905,6 +1011,37 @@ int pqp_bounds_set_occupancy_slots(pqp_bounds_handle *h, int32_t first_slot, con
     rc = set_occupancy_slots(h, first_slot, stack, staging, h->stream);
     if (rc != PQP_OK) return rc;
     PQP_CUDA(h->err, cudaStreamSynchronize(h->stream));
+    return PQP_OK;
+}
+
+int pqp_bounds_set_occupancy_boxes_device(pqp_bounds_handle *h, int32_t first_slot, const pqp_occupancy_stack *base,
+                                          int32_t shared_base, const pqp_obstacle_boxes *boxes, void *stream) {
+    const int rc = validate_boxes(h, first_slot, base, shared_base, boxes, false, "pqp_bounds_set_occupancy_boxes_device");
+    if (rc != PQP_OK) return rc;
+    pqp::DeviceGuard guard_(h->device);
+    return set_occupancy_boxes(h, first_slot, base, base->cells, shared_base, boxes->k, boxes->boxes, boxes->k_max,
+                               static_cast<cudaStream_t>(stream));
+}
+
+int pqp_bounds_set_occupancy_boxes(pqp_bounds_handle *h, int32_t first_slot, const pqp_occupancy_stack *base,
+                                   int32_t shared_base, const pqp_obstacle_boxes *boxes) {
+    int rc = validate_boxes(h, first_slot, base, shared_base, boxes, true, "pqp_bounds_set_occupancy_boxes");
+    if (rc != PQP_OK) return rc;
+    pqp::DeviceGuard guard_(h->device);
+    // the base image(s) into the slots' staging, as set_occupancy_slots stages its stack; the boxes into theirs
+    uint8_t *staging = h->d_occ + (size_t)first_slot * h->cap_cells;
+    const size_t bytes = (size_t)(shared_base ? 1 : base->count) * base->rows * base->cols;
+    const size_t n_box = (size_t)base->count * boxes->k_max;
+    cudaStream_t s = h->stream;
+    PQP_CUDA(h->err, cudaMemcpyAsync(staging, base->cells, bytes, cudaMemcpyHostToDevice, s));
+    if (n_box) {
+        PQP_CUDA(h->err, cudaMemcpyAsync(h->d_box_k, boxes->k, base->count * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+        PQP_CUDA(h->err, cudaMemcpyAsync(h->d_boxes, boxes->boxes, n_box * PQP_BOX_FIELDS * sizeof(double),
+                                         cudaMemcpyHostToDevice, s));
+    }
+    rc = set_occupancy_boxes(h, first_slot, base, staging, shared_base, h->d_box_k, h->d_boxes, boxes->k_max, s);
+    if (rc != PQP_OK) return rc;
+    PQP_CUDA(h->err, cudaStreamSynchronize(s));
     return PQP_OK;
 }
 

@@ -993,6 +993,18 @@ int pqp_plan_set_occupancy_slots(pqp_plan_handle *h, int32_t first_slot, const p
     PQL_MAP(h, pqp_bounds_set_occupancy_slots(h->bounds, first_slot, stack), occupancy_slots_launches(stack), false);
 }
 
+int pqp_plan_set_occupancy_boxes_device(pqp_plan_handle *h, int32_t first_slot, const pqp_occupancy_stack *base,
+                                        int32_t shared_base, const pqp_obstacle_boxes *boxes, void *stream) {
+    PQL_MAP(h, pqp_bounds_set_occupancy_boxes_device(h->bounds, first_slot, base, shared_base, boxes, stream),
+            occupancy_slots_launches(base), false);
+}
+
+int pqp_plan_set_occupancy_boxes(pqp_plan_handle *h, int32_t first_slot, const pqp_occupancy_stack *base,
+                                 int32_t shared_base, const pqp_obstacle_boxes *boxes) {
+    PQL_MAP(h, pqp_bounds_set_occupancy_boxes(h->bounds, first_slot, base, shared_base, boxes),
+            occupancy_slots_launches(base), false);
+}
+
 int pqp_plan_get_map(pqp_plan_handle *h, pqp_bounds_map *meta, float *distance) {
     PQL_MAP(h, pqp_bounds_get_map(h->bounds, meta, distance), 0, false);
 }

@@ -24,6 +24,8 @@ struct Staging {
     double *x = nullptr, *y = nullptr, *start = nullptr, *target = nullptr, *path = nullptr, *cost = nullptr;
     int32_t *cnt = nullptr, *map_index = nullptr, *status = nullptr, *n = nullptr, *iters = nullptr;
     uint8_t *occ = nullptr;  // n_maps * cap_cells: the images of a device-form occupancy update
+    double *boxes = nullptr;  // PQP_MAX_BOXES * PQP_BOX_FIELDS: the boxes of a device-form box update
+    int32_t *box_k = nullptr;  // n_maps: their counts
 };
 
 }  // namespace
@@ -281,6 +283,8 @@ int pqp_plan_multi_create_maps(const pqp_bounds_map *maps, int32_t n_maps, const
             PQP_CUDA(err, r.alloc(s.cost, B));
             PQP_CUDA(err, r.alloc(s.iters, B * 2));
             PQP_CUDA(err, r.alloc(s.occ, (size_t)n_maps * m->cap_cells));
+            PQP_CUDA(err, r.alloc(s.boxes, (size_t)PQP_MAX_BOXES * PQP_BOX_FIELDS));
+            PQP_CUDA(err, r.alloc(s.box_k, (size_t)n_maps));
             // direct copies over NVLink / PCIe between this device and the home one where the pair allows it
             int there = 0, back = 0;
             if (m->dev[d] != home && cudaDeviceCanAccessPeer(&there, m->dev[d], home) == cudaSuccess && there &&
@@ -367,6 +371,53 @@ int pqp_plan_multi_set_occupancy_slots_device(pqp_plan_multi_t *m, int32_t first
         // after the transform: once the caller's stream has passed the update, every device's slots are final, as the
         // single-device call's are, whichever stream (a host form's included) reads them next
         PQP_CUDA(m->err, cudaEventRecord(m->done[d], sd));
+    }
+    pqp::DeviceGuard g(home);
+    for (int d = 1; d < m->n_dev; ++d) PQP_CUDA(m->err, cudaStreamWaitEvent(s, m->done[d], 0));
+    return PQP_OK;
+}
+
+int pqp_plan_multi_set_occupancy_boxes(pqp_plan_multi_t *m, int32_t first_slot, const pqp_occupancy_stack *base,
+                                       int32_t shared_base, const pqp_obstacle_boxes *boxes) {
+    if (!m) return PQP_E_INVALID;
+    return update_all(m, [&](pqp_plan_handle *h) {
+        return pqp_plan_set_occupancy_boxes(h, first_slot, base, shared_base, boxes);
+    });
+}
+
+int pqp_plan_multi_set_occupancy_boxes_device(pqp_plan_multi_t *m, int32_t first_slot, const pqp_occupancy_stack *base,
+                                              int32_t shared_base, const pqp_obstacle_boxes *boxes, void *stream) {
+    if (!m) return PQP_E_INVALID;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const int home = m->dev[0];
+    {
+        pqp::DeviceGuard g(home);
+        PQP_CUDA(m->err, cudaEventRecord(m->fork, s));
+    }
+    // the home handle first: its refusal is every device's
+    int rc = pqp_plan_set_occupancy_boxes_device(m->h[0], first_slot, base, shared_base, boxes, stream);
+    if (rc != PQP_OK) return device_fail(m, 0, rc);
+    const size_t bytes = (size_t)(shared_base ? 1 : base->count) * base->rows * base->cols;
+    const size_t n_box = (size_t)base->count * boxes->k_max;
+    for (int d = 1; d < m->n_dev; ++d) {
+        const int dv = m->dev[d];
+        const Staging &st = m->st[d];
+        cudaStream_t sd = m->stream[d];
+        pqp::DeviceGuard g(dv);
+        PQP_CUDA(m->err, cudaStreamWaitEvent(sd, m->fork, 0));
+        PQP_CUDA(m->err, peer_copy(st.occ, dv, base->cells, home, bytes, sd));
+        pqp_occupancy_stack local = *base;
+        local.cells = st.occ;
+        pqp_obstacle_boxes lb = *boxes;
+        if (n_box) {
+            PQP_CUDA(m->err, peer_copy(st.box_k, dv, boxes->k, home, (size_t)base->count, sd));
+            PQP_CUDA(m->err, peer_copy(st.boxes, dv, boxes->boxes, home, n_box * PQP_BOX_FIELDS, sd));
+            lb.k = st.box_k;
+            lb.boxes = st.boxes;
+        }
+        rc = pqp_plan_set_occupancy_boxes_device(m->h[d], first_slot, &local, shared_base, &lb, sd);
+        if (rc != PQP_OK) return device_fail(m, d, rc);
+        PQP_CUDA(m->err, cudaEventRecord(m->done[d], sd));  // as set_occupancy_slots_device: the slots are final
     }
     pqp::DeviceGuard g(home);
     for (int d = 1; d < m->n_dev; ++d) PQP_CUDA(m->err, cudaStreamWaitEvent(s, m->done[d], 0));

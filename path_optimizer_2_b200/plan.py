@@ -16,7 +16,8 @@ EXPORTED_SYMBOLS = ["pqp_plan_default_params", "pqp_plan_create", "pqp_plan_dest
                     "pqp_plan_set_map_slot", "pqp_plan_set_map_slot_device", "pqp_plan_set_occupancy_slots",
                     "pqp_plan_set_occupancy_slots_device", "pqp_plan_get_map_slot", "pqp_plan_map_count",
                     "pqp_plan_collision_check", "pqp_plan_collision_check_device", "pqp_plan_collision_check_mapped",
-                    "pqp_plan_collision_check_mapped_device"]
+                    "pqp_plan_collision_check_mapped_device", "pqp_plan_set_occupancy_boxes",
+                    "pqp_plan_set_occupancy_boxes_device"]
 # kernel launches of one collision_check call
 COLLISION_LAUNCHES = 1
 # kernel launches of one set_occupancy call (the distance transform's column and row pass)
@@ -137,6 +138,7 @@ def _lib():
         L.pqp_plan_map_count.argtypes = [vp]
         L.pqp_plan_map_count.restype = C.c_int32
         bounds.declare_collision(L, "pqp_plan_")
+        bounds.declare_boxes(L, "pqp_plan_")
         L._plan_declared = True
     return L
 
@@ -307,6 +309,14 @@ class Planner(bounds.MapSlots):
         tensor must stay alive until the stream has run the transform."""
         super().set_occupancy_slots_device(imgs, resolution, centers, obstacle_max, first_slot=first_slot,
                                            stream=_stream(stream, imgs.device))
+
+    def set_occupancy_boxes_device(self, base, resolution, boxes, k, centers=None, obstacle_max=0, *, first_slot=0,
+                                   stream=None):
+        """As `set_occupancy_boxes` from torch CUDA tensors (`bounds.MapSlots.set_occupancy_boxes_device`),
+        asynchronous on `stream` (default: the current stream): plans enqueued before see the old slots, plans enqueued
+        after the new ones."""
+        super().set_occupancy_boxes_device(base, resolution, boxes, k, centers, obstacle_max, first_slot=first_slot,
+                                           stream=_stream(stream, base.device))
 
     def set_map_device(self, dist, resolution, center=(0.0, 0.0), *, stream=None):
         """As `set_map` from a torch float32 CUDA tensor [rows, cols], asynchronous on `stream` (default: the

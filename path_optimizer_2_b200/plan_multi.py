@@ -15,7 +15,8 @@ EXPORTED_SYMBOLS = ["pqp_plan_multi_create_maps", "pqp_plan_multi_destroy", "pqp
                     "pqp_plan_multi_points_device", "pqp_plan_multi_device", "pqp_plan_multi_set_map_slot",
                     "pqp_plan_multi_set_occupancy_slots", "pqp_plan_multi_set_occupancy_slots_device",
                     "pqp_plan_multi_get_map_slot", "pqp_plan_multi_shard", "pqp_plan_multi_handle",
-                    "pqp_plan_multi_last_error"]
+                    "pqp_plan_multi_last_error", "pqp_plan_multi_set_occupancy_boxes",
+                    "pqp_plan_multi_set_occupancy_boxes_device"]
 
 
 def _lib():
@@ -33,6 +34,7 @@ def _lib():
         L.pqp_plan_multi_set_map_slot.argtypes = [vp, i32, C.POINTER(bounds.BoundsMap)]
         L.pqp_plan_multi_set_occupancy_slots.argtypes = [vp, i32, C.POINTER(bounds.OccupancyStack)]
         L.pqp_plan_multi_set_occupancy_slots_device.argtypes = [vp, i32, C.POINTER(bounds.OccupancyStack), vp]
+        bounds.declare_boxes(L, "pqp_plan_multi_")
         L.pqp_plan_multi_get_map_slot.argtypes = [vp, i32, i32, C.POINTER(bounds.BoundsMap), vp]
         L.pqp_plan_multi_shard.argtypes = [vp, i32, C.POINTER(i32), C.POINTER(i32)]
         L.pqp_plan_multi_handle.argtypes = [vp, i32, C.POINTER(vp)]
@@ -130,6 +132,20 @@ class MultiPlanner:
         st, _keep = bounds.occupancy_stack(imgs.data_ptr(), imgs.shape, resolution, centers, obstacle_max)
         s = C.c_void_p(_plan._stream(stream, imgs.device))
         self._check(self.L.pqp_plan_multi_set_occupancy_slots_device(self.h, int(first_slot), C.byref(st), s))
+
+    def set_occupancy_boxes(self, base, resolution, boxes, k=None, centers=None, obstacle_max=0, *, first_slot=0):
+        """As `plan.Planner.set_occupancy_boxes` on every device, the updates concurrently (host, synchronous)."""
+        self._check(bounds.boxes_call(self.L.pqp_plan_multi_set_occupancy_boxes, self.h, base, resolution, boxes, k,
+                                      centers, obstacle_max, first_slot))
+
+    def set_occupancy_boxes_device(self, base, resolution, boxes, k, centers=None, obstacle_max=0, *, first_slot=0,
+                                   stream=None):
+        """As `plan.Planner.set_occupancy_boxes_device` from tensors on the home device, ordered on `stream` (default:
+        the current stream of the home device): the base image(s), k and the boxes are peer-copied to every other
+        device and stamped there, as `set_occupancy_slots_device` does with its images."""
+        s = _plan._stream(stream, base.device)
+        self._check(bounds.boxes_call_device(self.L.pqp_plan_multi_set_occupancy_boxes_device, self.h, base,
+                                             resolution, boxes, k, centers, obstacle_max, first_slot, s))
 
     def get_map_slot(self, device_index, slot=0):
         """-> (float32 distance layer, resolution, (center_x, center_y)) of `slot` on device index `device_index`."""
