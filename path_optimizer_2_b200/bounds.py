@@ -184,68 +184,74 @@ def _declare(L):
     L.pqp_bounds_last_kernel_ms.argtypes = [vp, C.POINTER(C.c_float)]
     L.pqp_bounds_last_error.argtypes = [vp]
     L.pqp_bounds_last_error.restype = C.c_char_p
-    L.pqp_bounds_set_map.argtypes = [vp, C.POINTER(BoundsMap)]
-    L.pqp_bounds_set_map_device.argtypes = [vp, C.POINTER(BoundsMap), vp]
-    L.pqp_bounds_set_occupancy.argtypes = [vp, C.POINTER(OccupancyMap)]
-    L.pqp_bounds_set_occupancy_device.argtypes = [vp, C.POINTER(OccupancyMap), vp]
-    L.pqp_bounds_get_map.argtypes = [vp, C.POINTER(BoundsMap), vp]
     L.pqp_bounds_create_maps.argtypes = [C.POINTER(BoundsMap), C.c_int32, C.POINTER(BoundsParams), C.c_int32,
                                          C.POINTER(vp)]
-    L.pqp_bounds_set_map_slot.argtypes = [vp, C.c_int32, C.POINTER(BoundsMap)]
-    L.pqp_bounds_set_map_slot_device.argtypes = [vp, C.c_int32, C.POINTER(BoundsMap), vp]
-    L.pqp_bounds_set_occupancy_slots.argtypes = [vp, C.c_int32, C.POINTER(OccupancyStack)]
-    L.pqp_bounds_set_occupancy_slots_device.argtypes = [vp, C.c_int32, C.POINTER(OccupancyStack), vp]
-    L.pqp_bounds_get_map_slot.argtypes = [vp, C.c_int32, C.POINTER(BoundsMap), vp]
-    L.pqp_bounds_map_count.argtypes = [vp]
-    L.pqp_bounds_map_count.restype = C.c_int32
     L.pqp_bounds_compute_mapped.argtypes = [vp, C.POINTER(BoundsIn), vp, C.POINTER(BoundsOut)]
     L.pqp_bounds_compute_mapped_device.argtypes = [vp, C.POINTER(BoundsIn), vp, C.POINTER(BoundsOut), vp]
-    declare_collision(L, "pqp_bounds_")
-    declare_boxes(L, "pqp_bounds_")
+    declare_map_surface(L, "pqp_bounds_")
     L._pqp_bounds_declared = True
     return L
 
 
-def declare_collision(L, prefix):
-    """The four collision-check entry points of the ABI `prefix` (pqp_bounds_, pqp_plan_)."""
-    vp, cin, cout = C.c_void_p, C.POINTER(CollisionIn), C.POINTER(CollisionOut)
-    getattr(L, prefix + "collision_check").argtypes = [vp, cin, cout]
-    getattr(L, prefix + "collision_check_device").argtypes = [vp, cin, cout, vp]
-    getattr(L, prefix + "collision_check_mapped").argtypes = [vp, cin, vp, cout]
-    getattr(L, prefix + "collision_check_mapped_device").argtypes = [vp, cin, vp, cout, vp]
+def declare_map_surface(L, prefix):
+    """The map entry points of the ABI `prefix` (pqp_bounds_, pqp_plan_): map and slot updates and reads, the slot
+    count and the collision check."""
+    vp, i32, bm, om = C.c_void_p, C.c_int32, C.POINTER(BoundsMap), C.POINTER(OccupancyMap)
+    cin, cout = C.POINTER(CollisionIn), C.POINTER(CollisionOut)
+    for name, argtypes in (
+            ("set_map", [vp, bm]), ("set_map_device", [vp, bm, vp]), ("set_occupancy", [vp, om]),
+            ("set_occupancy_device", [vp, om, vp]), ("get_map", [vp, bm, vp]), ("set_map_slot", [vp, i32, bm]),
+            ("set_map_slot_device", [vp, i32, bm, vp]), ("get_map_slot", [vp, i32, bm, vp]), ("map_count", [vp]),
+            ("collision_check", [vp, cin, cout]), ("collision_check_device", [vp, cin, cout, vp]),
+            ("collision_check_mapped", [vp, cin, vp, cout]),
+            ("collision_check_mapped_device", [vp, cin, vp, cout, vp])):
+        getattr(L, prefix + name).argtypes = argtypes
+    getattr(L, prefix + "map_count").restype = C.c_int32
+    declare_stack_updates(L, prefix)
 
 
-def declare_boxes(L, prefix):
-    """The two set_occupancy_boxes entry points of the ABI `prefix` (pqp_bounds_, pqp_plan_, pqp_plan_multi_)."""
-    vp, st, bx = C.c_void_p, C.POINTER(OccupancyStack), C.POINTER(ObstacleBoxes)
-    getattr(L, prefix + "set_occupancy_boxes").argtypes = [vp, C.c_int32, st, C.c_int32, bx]
-    getattr(L, prefix + "set_occupancy_boxes_device").argtypes = [vp, C.c_int32, st, C.c_int32, bx, vp]
+def declare_stack_updates(L, prefix):
+    """The set_occupancy_slots and set_occupancy_boxes entry points of the ABI `prefix` (pqp_bounds_, pqp_plan_,
+    pqp_plan_multi_)."""
+    vp, i32, st, bx = C.c_void_p, C.c_int32, C.POINTER(OccupancyStack), C.POINTER(ObstacleBoxes)
+    getattr(L, prefix + "set_occupancy_slots").argtypes = [vp, i32, st]
+    getattr(L, prefix + "set_occupancy_slots_device").argtypes = [vp, i32, st, vp]
+    getattr(L, prefix + "set_occupancy_boxes").argtypes = [vp, i32, st, i32, bx]
+    getattr(L, prefix + "set_occupancy_boxes_device").argtypes = [vp, i32, st, i32, bx, vp]
 
 
-def boxes_call(fn, h, base, resolution, boxes, k, centers, obstacle_max, first_slot):
-    """`fn` (a host-form set_occupancy_boxes) on host arrays, as MapSlots.set_occupancy_boxes documents them."""
-    base = np.ascontiguousarray(base, dtype=np.uint8)
-    n = len(boxes) if base.ndim == 2 else None
-    count, shared, (rows, cols) = box_base(base.shape, n)
-    packed, k = pack_boxes(boxes, k, count)
-    st, _keep = occupancy_stack(base.ctypes.data, (count, rows, cols), resolution, centers, obstacle_max)
-    ob = ObstacleBoxes(packed.shape[1], k.ctypes.data, packed.ctypes.data)
-    return fn(h, int(first_slot), C.byref(st), shared, C.byref(ob))
+def occupancy_call(fn, h, imgs, resolution, centers, obstacle_max, first_slot, boxes=None, k=None):
+    """`fn`, a host-form set_occupancy_slots or (with `boxes`) set_occupancy_boxes, on host arrays as
+    MapSlots.set_occupancy_slots and MapSlots.set_occupancy_boxes document them."""
+    imgs = np.ascontiguousarray(imgs, dtype=np.uint8)
+    assert imgs.ndim == 3 or (boxes is not None and imgs.ndim == 2)
+    shape, box_args = imgs.shape, ()
+    if boxes is not None:
+        count, shared, (rows, cols) = box_base(imgs.shape, len(boxes) if imgs.ndim == 2 else None)
+        packed, k = pack_boxes(boxes, k, count)
+        shape, box_args = (count, rows, cols), (shared, C.byref(ObstacleBoxes(packed.shape[1], k.ctypes.data,
+                                                                               packed.ctypes.data)))
+    st, _keep = occupancy_stack(imgs.ctypes.data, shape, resolution, centers, obstacle_max)
+    return fn(h, int(first_slot), C.byref(st), *box_args)
 
 
-def boxes_call_device(fn, h, base, resolution, boxes, k, centers, obstacle_max, first_slot, stream):
-    """`fn` (a device-form set_occupancy_boxes) on torch CUDA tensors, as MapSlots.set_occupancy_boxes_device documents
-    them; `stream` a raw cudaStream_t."""
+def occupancy_call_device(fn, h, imgs, resolution, centers, obstacle_max, first_slot, boxes=None, k=None, *, stream):
+    """As `occupancy_call` for the device form `fn`, on torch CUDA tensors as MapSlots.set_occupancy_slots_device and
+    MapSlots.set_occupancy_boxes_device document them; `stream` a raw cudaStream_t."""
     import torch
-    assert base.is_cuda and base.is_contiguous() and base.dtype == torch.uint8 and base.dim() in (2, 3)
-    assert boxes.is_cuda and boxes.is_contiguous() and boxes.dtype == torch.float64 and boxes.dim() == 3
-    assert boxes.shape[2] == BOX_FIELDS
-    count, shared, (rows, cols) = box_base(tuple(base.shape), int(boxes.shape[0]))
-    assert int(boxes.shape[0]) == count
-    assert k.is_cuda and k.is_contiguous() and k.dtype == torch.int32 and tuple(k.shape) == (count,)
-    st, _keep = occupancy_stack(base.data_ptr(), (count, rows, cols), resolution, centers, obstacle_max)
-    ob = ObstacleBoxes(int(boxes.shape[1]), k.data_ptr(), boxes.data_ptr())
-    return fn(h, int(first_slot), C.byref(st), shared, C.byref(ob), C.c_void_p(stream))
+    assert imgs.is_cuda and imgs.is_contiguous() and imgs.dtype == torch.uint8
+    assert imgs.dim() == 3 or (boxes is not None and imgs.dim() == 2)
+    shape, box_args = tuple(imgs.shape), ()
+    if boxes is not None:
+        assert boxes.is_cuda and boxes.is_contiguous() and boxes.dtype == torch.float64 and boxes.dim() == 3
+        assert boxes.shape[2] == BOX_FIELDS
+        count, shared, (rows, cols) = box_base(shape, int(boxes.shape[0]))
+        assert int(boxes.shape[0]) == count
+        assert k.is_cuda and k.is_contiguous() and k.dtype == torch.int32 and tuple(k.shape) == (count,)
+        shape, box_args = (count, rows, cols), (shared, C.byref(ObstacleBoxes(int(boxes.shape[1]), k.data_ptr(),
+                                                                               boxes.data_ptr())))
+    st, _keep = occupancy_stack(imgs.data_ptr(), shape, resolution, centers, obstacle_max)
+    return fn(h, int(first_slot), C.byref(st), *box_args, C.c_void_p(stream))
 
 
 class MapSlots:
@@ -304,22 +310,23 @@ class MapSlots:
         m, _keep = occupancy_map(img, resolution, center, obstacle_max)
         self._check(self._fn("set_occupancy")(self.h, C.byref(m)))
 
+    def _raw_stream(self, stream, device):
+        """The cudaStream_t a device-form map update runs on: `stream` as given, a raw cudaStream_t (None: 0).
+        `plan.Planner` takes a torch stream instead (None: the current stream of `device`)."""
+        return 0 if stream is None else stream
+
     def set_occupancy_slots(self, imgs, resolution, centers=None, obstacle_max=0, *, first_slot=0):
         """The exact distance transforms of a uint8 stack [count, rows, cols] into slots first_slot .. + count - 1,
         in one pair of launches (host, synchronous); `centers` [count, 2] (default: the origin)."""
-        imgs = np.ascontiguousarray(imgs, dtype=np.uint8)
-        assert imgs.ndim == 3
-        st, _keep = occupancy_stack(imgs.ctypes.data, imgs.shape, resolution, centers, obstacle_max)
-        self._check(self._fn("set_occupancy_slots")(self.h, int(first_slot), C.byref(st)))
+        self._check(occupancy_call(self._fn("set_occupancy_slots"), self.h, imgs, resolution, centers, obstacle_max,
+                                   first_slot))
 
-    def set_occupancy_slots_device(self, imgs, resolution, centers=None, obstacle_max=0, *, first_slot=0, stream=0):
-        """As `set_occupancy_slots` from a torch uint8 CUDA tensor [count, rows, cols], asynchronous on `stream` (a raw
-        cudaStream_t): calls enqueued before see the old slots, calls enqueued after the new ones. The tensor must
-        stay alive until the stream has run the transform."""
-        import torch
-        assert imgs.is_cuda and imgs.is_contiguous() and imgs.dtype == torch.uint8 and imgs.dim() == 3
-        st, _keep = occupancy_stack(imgs.data_ptr(), imgs.shape, resolution, centers, obstacle_max)
-        self._check(self._fn("set_occupancy_slots_device")(self.h, int(first_slot), C.byref(st), C.c_void_p(stream)))
+    def set_occupancy_slots_device(self, imgs, resolution, centers=None, obstacle_max=0, *, first_slot=0, stream=None):
+        """As `set_occupancy_slots` from a torch uint8 CUDA tensor [count, rows, cols], asynchronous on `stream` (as
+        `_raw_stream` takes it): calls enqueued before see the old slots, calls enqueued after the new ones. The tensor
+        must stay alive until the stream has run the transform."""
+        self._check(occupancy_call_device(self._fn("set_occupancy_slots_device"), self.h, imgs, resolution, centers,
+                                          obstacle_max, first_slot, stream=self._raw_stream(stream, imgs.device)))
 
     def set_occupancy_boxes(self, base, resolution, boxes, k=None, centers=None, obstacle_max=0, *, first_slot=0):
         """Slots first_slot .. + count - 1 := the exact distance transforms of a static occupancy image plus each slot's
@@ -327,17 +334,18 @@ class MapSlots:
         [count, rows, cols]; `boxes` float64 [count, k_max, 5] (x, y, heading, length, width in the map's frame) with
         `k` [count] boxes per slot (None: all k_max), or a list of `count` arrays [k_s, 5]. A cell is an obstacle when
         its base value <= obstacle_max or its centre lies in or on one of its slot's boxes (include/pqp_bounds.h)."""
-        self._check(boxes_call(self._fn("set_occupancy_boxes"), self.h, base, resolution, boxes, k, centers,
-                               obstacle_max, first_slot))
+        self._check(occupancy_call(self._fn("set_occupancy_boxes"), self.h, base, resolution, centers, obstacle_max,
+                                   first_slot, boxes, k))
 
     def set_occupancy_boxes_device(self, base, resolution, boxes, k, centers=None, obstacle_max=0, *, first_slot=0,
-                                   stream=0):
+                                   stream=None):
         """As `set_occupancy_boxes` from torch CUDA tensors: `base` uint8 [rows, cols] or [count, rows, cols], `boxes`
-        float64 [count, k_max, 5], `k` int32 [count] (clamped to [0, k_max] on the device). Asynchronous on `stream` (a
-        raw cudaStream_t), ordered as `set_occupancy_slots_device`; the tensors must stay alive until the stream has
-        run the update."""
-        self._check(boxes_call_device(self._fn("set_occupancy_boxes_device"), self.h, base, resolution, boxes, k,
-                                      centers, obstacle_max, first_slot, stream))
+        float64 [count, k_max, 5], `k` int32 [count] (clamped to [0, k_max] on the device). Asynchronous on `stream` (as
+        `_raw_stream` takes it), ordered as `set_occupancy_slots_device`; the tensors must stay alive until the stream
+        has run the update."""
+        self._check(occupancy_call_device(self._fn("set_occupancy_boxes_device"), self.h, base, resolution, centers,
+                                          obstacle_max, first_slot, boxes, k,
+                                          stream=self._raw_stream(stream, base.device)))
 
     def get_map(self, slot=0):
         """-> (float32 distance layer [rows, cols], resolution, (center_x, center_y)) of the current map (of `slot`);

@@ -453,115 +453,113 @@ int validate_slots(pqp_bounds_handle *h, long long first, long long count, const
     return PQP_OK;
 }
 
-// the two passes over `count` images of rows x cols (consecutive in `cells`) into slots first .. first + count - 1;
-// entry_dst (one image only): the table entry the column pass writes; boxes: the slots' obstacle boxes (NULL for none),
-// whose column pass reads the slots' table entries, so those must be enqueued first
-int launch_edt(pqp_bounds_handle *h, int rows, int cols, double resolution, int obstacle_max, const uint8_t *cells,
-               int count, int first, pqb::MapView *entry_dst, const pqb::MapView &entry, cudaStream_t s,
-               const pqm::SlotBoxes *boxes = nullptr) {
-    const size_t smem = (size_t)pqm::kRowSmemPerCol * cols;
-    // the dynamic share plus the kernel's static n_env may pass the 48 KB default at any width: always opt in
-    PQP_CUDA(h->err, cudaFuncSetAttribute(pqm::edt_row_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    float *layer = slot_layer(h, first);
-    const dim3 grid((cols + pqm::kEdtColumnThreads - 1) / pqm::kEdtColumnThreads, count);
-    int32_t *g = reinterpret_cast<int32_t *>(layer);
-    if (boxes)
-        pqm::edt_column_kernel<<<grid, pqm::kEdtColumnThreads, 0, s>>>(cells, rows, cols, obstacle_max, g, h->cap_cells,
-                                                                       nullptr, entry, *boxes);
-    else
-        pqm::edt_column_kernel<<<grid, pqm::kEdtColumnThreads, 0, s>>>(cells, rows, cols, obstacle_max, g, h->cap_cells,
-                                                                       entry_dst, entry, pqm::NoBoxes{});
-    PQP_CUDA(h->err, cudaGetLastError());
-    pqm::edt_row_kernel<<<dim3(rows, count), pqm::kEdtRowThreads, smem, s>>>(layer, h->cap_cells, rows, cols,
-                                                                             (float)resolution);
-    PQP_CUDA(h->err, cudaGetLastError());
-    return PQP_OK;
-}
+// One pqp_bounds_set_occupancy* call: the images of `stack` into slots first .. first + count - 1. `boxed`: the box
+// call, which stamps each slot's `boxes` into the base image(s) (one shared when shared_base is 1) and refuses a NULL
+// `boxes`. `single`: the one-image call, a count-1 stack at slot 0, whose column pass writes the slot's table entry.
+struct Occupancy {
+    int first;
+    const pqp_occupancy_stack *stack;
+    bool boxed;
+    int shared_base;
+    const pqp_obstacle_boxes *boxes;
+    bool single;
+};
 
-int validate_occupancy(pqp_bounds_handle *h, const pqp_occupancy_map *occ, const char *what) {
-    const int rc = occ ? validate_map(h, occ, occ->rows, occ->cols, occ->resolution, occ->center_x, occ->center_y,
-                                      occ->cells, what)
-                       : validate_map(h, nullptr, 0, 0, 0.0, 0.0, 0.0, nullptr, what);
-    if (rc != PQP_OK) return rc;
-    if (occ->rows > pqm::kMaxSide || occ->cols > pqm::kMaxSide)
-        return fail(h->err, PQP_E_INVALID, std::string(what) + ": rows and cols must be <= 16384 for the distance transform");
-    return PQP_OK;
-}
-
-// one image into slot 0, the table entry written by the column pass (no launch of its own)
-int set_occupancy0(pqp_bounds_handle *h, const pqp_occupancy_map *occ, const uint8_t *cells, cudaStream_t s) {
-    const pqb::MapView m = make_view(slot_layer(h, 0), occ->rows, occ->cols, occ->resolution, occ->center_x, occ->center_y);
-    const int rc = launch_edt(h, occ->rows, occ->cols, occ->resolution, occ->obstacle_max, cells, 1, 0, h->d_table, m, s);
-    if (rc != PQP_OK) return rc;
-    h->maps[0] = m;
-    return PQP_OK;
-}
-
-int validate_stack(pqp_bounds_handle *h, int first, const pqp_occupancy_stack *st, const char *what) {
+// what every pqp_bounds_set_occupancy* call refuses, in this order; `host`: the host form, which can read k
+int validate(pqp_bounds_handle *h, const Occupancy &r, bool host, const char *what) {
     if (!h) return PQP_E_INVALID;
+    const pqp_occupancy_stack *st = r.stack;
     if (!st || !st->cells || !st->center_x || !st->center_y)
-        return fail(h->err, PQP_E_INVALID, std::string(what) + ": null stack, image or centres");
-    int rc = validate_slots(h, first, st->count, what);
-    if (rc != PQP_OK) return rc;
-    for (int i = 0; i < st->count; ++i) {
+        return fail(h->err, PQP_E_INVALID,
+                    std::string(what) + (r.single ? ": null map or layer" : ": null stack, image or centres"));
+    int rc = validate_slots(h, r.first, st->count, what);
+    for (int i = 0; rc == PQP_OK && i < st->count; ++i)
         rc = validate_map(h, st, st->rows, st->cols, st->resolution, st->center_x[i], st->center_y[i], st->cells, what);
-        if (rc != PQP_OK) return rc;
-    }
+    if (rc != PQP_OK) return rc;
     if (st->rows > pqm::kMaxSide || st->cols > pqm::kMaxSide)
         return fail(h->err, PQP_E_INVALID, std::string(what) + ": rows and cols must be <= 16384 for the distance transform");
-    return PQP_OK;
-}
-
-// `boxes` (NULL for none): the set_occupancy_boxes call's, with table and img_stride still to be filled in here. The
-// table entries go first: the box instantiation of the column pass reads the slots' centres from them.
-int set_occupancy_slots(pqp_bounds_handle *h, int first, const pqp_occupancy_stack *st, const uint8_t *cells,
-                        cudaStream_t s, const pqm::SlotBoxes *boxes = nullptr) {
-    const pqb::MapView meta = make_view(slot_layer(h, first), st->rows, st->cols, st->resolution, 0.0, 0.0);
-    int rc = write_table(h, first, st->count, meta, st->center_x, st->center_y, s);
-    if (rc != PQP_OK) return rc;
-    pqm::SlotBoxes sb{};
-    if (boxes) {
-        sb = *boxes;
-        sb.table = h->d_table + first;
-    }
-    rc = launch_edt(h, st->rows, st->cols, st->resolution, st->obstacle_max, cells, st->count, first, nullptr, meta, s,
-                    boxes ? &sb : nullptr);
-    if (rc != PQP_OK) return rc;
-    for (int i = 0; i < st->count; ++i)
-        h->maps[first + i] = make_view(slot_layer(h, first + i), st->rows, st->cols, st->resolution, st->center_x[i],
-                                       st->center_y[i]);
-    return PQP_OK;
-}
-
-// what pqp_bounds_set_occupancy_boxes(_device) accept beyond validate_stack; `host`: the host form, which can read k
-int validate_boxes(pqp_bounds_handle *h, int first, const pqp_occupancy_stack *base, int shared_base,
-                   const pqp_obstacle_boxes *boxes, bool host, const char *what) {
-    int rc = validate_stack(h, first, base, what);
-    if (rc != PQP_OK) return rc;
+    if (!r.boxed) return PQP_OK;
     std::string why;
-    if (shared_base != 0 && shared_base != 1) why = "shared_base must be 0 or 1";
+    const pqp_obstacle_boxes *boxes = r.boxes;
+    if (r.shared_base != 0 && r.shared_base != 1) why = "shared_base must be 0 or 1";
     else if (!boxes) why = "null boxes";
     else if (boxes->k_max < 0) why = "k_max must be >= 0";
-    else if ((long long)base->count * boxes->k_max > PQP_MAX_BOXES)
-        why = "count * k_max = " + std::to_string((long long)base->count * boxes->k_max) + " exceeds PQP_MAX_BOXES (" +
+    else if ((long long)st->count * boxes->k_max > PQP_MAX_BOXES)
+        why = "count * k_max = " + std::to_string((long long)st->count * boxes->k_max) + " exceeds PQP_MAX_BOXES (" +
               std::to_string(PQP_MAX_BOXES) + ")";
     else if (boxes->k_max > 0 && (!boxes->k || !boxes->boxes)) why = "null k or boxes with k_max > 0";
     else if (host && boxes->k_max > 0)
-        for (int i = 0; i < base->count && why.empty(); ++i)
+        for (int i = 0; i < st->count && why.empty(); ++i)
             if (boxes->k[i] < 0 || boxes->k[i] > boxes->k_max)
                 why = "k[" + std::to_string(i) + "] = " + std::to_string(boxes->k[i]) + " outside [0, k_max]";
     return why.empty() ? PQP_OK : fail(h->err, PQP_E_INVALID, std::string(what) + ": " + why);
 }
 
-// the box call once validated: `cells`, `k` and `xs` (the boxes) in device memory
-int set_occupancy_boxes(pqp_bounds_handle *h, int first, const pqp_occupancy_stack *base, const uint8_t *cells,
-                        int shared_base, const int32_t *k, const double *xs, int k_max, cudaStream_t s) {
-    pqm::SlotBoxes sb{};
-    sb.boxes = xs;
-    sb.k = k;
-    sb.k_max = k_max;
-    sb.img_stride = shared_base ? 0 : (size_t)base->rows * base->cols;
-    return set_occupancy_slots(h, first, base, cells, s, &sb);
+// every pqp_bounds_set_occupancy* entry point; `stream` empty for the host forms, which stage the image(s), k and the
+// boxes into the handle's buffers, run on the handle's stream and wait
+int occupancy(pqp_bounds_handle *h, const Occupancy &r, std::optional<cudaStream_t> stream, const char *what) {
+    int rc = validate(h, r, !stream, what);
+    if (rc != PQP_OK) return rc;
+    pqp::DeviceGuard guard_(h->device);
+    const pqp_occupancy_stack &st = *r.stack;
+    const cudaStream_t s = stream ? *stream : h->stream;
+    const int k_max = r.boxed ? r.boxes->k_max : 0;
+    const uint8_t *cells = st.cells;
+    const int32_t *k = r.boxed ? r.boxes->k : nullptr;
+    const double *xs = r.boxed ? r.boxes->boxes : nullptr;
+    if (!stream) {
+        // the images are consecutive in the slots' staging: count * rows * cols <= count * cap_cells bytes
+        uint8_t *staging = h->d_occ + (size_t)r.first * h->cap_cells;
+        const size_t bytes = (size_t)(r.shared_base ? 1 : st.count) * st.rows * st.cols;
+        const size_t n_box = (size_t)st.count * k_max;
+        PQP_CUDA(h->err, cudaMemcpyAsync(staging, st.cells, bytes, cudaMemcpyHostToDevice, s));
+        if (n_box) {
+            PQP_CUDA(h->err, cudaMemcpyAsync(h->d_box_k, k, st.count * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+            PQP_CUDA(h->err, cudaMemcpyAsync(h->d_boxes, xs, n_box * PQP_BOX_FIELDS * sizeof(double),
+                                             cudaMemcpyHostToDevice, s));
+        }
+        cells = staging;
+        k = h->d_box_k;
+        xs = h->d_boxes;
+    }
+    float *layer = slot_layer(h, r.first);
+    const pqb::MapView meta = make_view(layer, st.rows, st.cols, st.resolution, r.single ? st.center_x[0] : 0.0,
+                                        r.single ? st.center_y[0] : 0.0);
+    // the box instantiation of the column pass reads the slots' centres from their table entries: those go first
+    if (!r.single) {
+        rc = write_table(h, r.first, st.count, meta, st.center_x, st.center_y, s);
+        if (rc != PQP_OK) return rc;
+    }
+    const size_t smem = (size_t)pqm::kRowSmemPerCol * st.cols;
+    // the dynamic share plus the kernel's static n_env may pass the 48 KB default at any width: always opt in
+    PQP_CUDA(h->err, cudaFuncSetAttribute(pqm::edt_row_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const dim3 grid((st.cols + pqm::kEdtColumnThreads - 1) / pqm::kEdtColumnThreads, st.count);
+    int32_t *g = reinterpret_cast<int32_t *>(layer);
+    if (r.boxed)
+        pqm::edt_column_kernel<<<grid, pqm::kEdtColumnThreads, 0, s>>>(
+            cells, st.rows, st.cols, st.obstacle_max, g, h->cap_cells, nullptr, meta,
+            pqm::SlotBoxes{h->d_table + r.first, xs, k, k_max, r.shared_base ? 0 : (size_t)st.rows * st.cols});
+    else
+        pqm::edt_column_kernel<<<grid, pqm::kEdtColumnThreads, 0, s>>>(cells, st.rows, st.cols, st.obstacle_max, g,
+                                                                       h->cap_cells, r.single ? h->d_table : nullptr,
+                                                                       meta, pqm::NoBoxes{});
+    PQP_CUDA(h->err, cudaGetLastError());
+    pqm::edt_row_kernel<<<dim3(st.rows, st.count), pqm::kEdtRowThreads, smem, s>>>(layer, h->cap_cells, st.rows, st.cols,
+                                                                                   (float)st.resolution);
+    PQP_CUDA(h->err, cudaGetLastError());
+    for (int i = 0; i < st.count; ++i)
+        h->maps[r.first + i] = make_view(slot_layer(h, r.first + i), st.rows, st.cols, st.resolution, st.center_x[i],
+                                         st.center_y[i]);
+    if (!stream) PQP_CUDA(h->err, cudaStreamSynchronize(s));
+    return PQP_OK;
+}
+
+// pqp_bounds_set_occupancy(_device): `occ` as a count-1 stack at slot 0 with its centre
+int occupancy_image(pqp_bounds_handle *h, const pqp_occupancy_map *occ, std::optional<cudaStream_t> stream,
+                    const char *what) {
+    pqp_occupancy_stack st{};
+    if (occ) st = {1, occ->rows, occ->cols, occ->resolution, &occ->center_x, &occ->center_y, occ->cells, occ->obstacle_max};
+    return occupancy(h, {0, occ ? &st : nullptr, false, 0, nullptr, true}, stream, what);
 }
 
 int create(const pqp_bounds_map *maps, int n_maps, const pqp_bounds_params *params, int32_t device,
@@ -974,75 +972,33 @@ int pqp_bounds_set_map_slot(pqp_bounds_handle *h, int32_t slot, const pqp_bounds
 }
 
 int pqp_bounds_set_occupancy_device(pqp_bounds_handle *h, const pqp_occupancy_map *occ, void *stream) {
-    const int rc = validate_occupancy(h, occ, "pqp_bounds_set_occupancy_device");
-    if (rc != PQP_OK) return rc;
-    pqp::DeviceGuard guard_(h->device);
-    return set_occupancy0(h, occ, occ->cells, static_cast<cudaStream_t>(stream));
+    return occupancy_image(h, occ, static_cast<cudaStream_t>(stream), "pqp_bounds_set_occupancy_device");
 }
 
 int pqp_bounds_set_occupancy(pqp_bounds_handle *h, const pqp_occupancy_map *occ) {
-    int rc = validate_occupancy(h, occ, "pqp_bounds_set_occupancy");
-    if (rc != PQP_OK) return rc;
-    pqp::DeviceGuard guard_(h->device);
-    const size_t cells = (size_t)occ->rows * occ->cols;
-    PQP_CUDA(h->err, cudaMemcpyAsync(h->d_occ, occ->cells, cells, cudaMemcpyHostToDevice, h->stream));
-    rc = set_occupancy0(h, occ, h->d_occ, h->stream);
-    if (rc != PQP_OK) return rc;
-    PQP_CUDA(h->err, cudaStreamSynchronize(h->stream));
-    return PQP_OK;
+    return occupancy_image(h, occ, std::nullopt, "pqp_bounds_set_occupancy");
 }
 
 int pqp_bounds_set_occupancy_slots_device(pqp_bounds_handle *h, int32_t first_slot, const pqp_occupancy_stack *stack,
                                           void *stream) {
-    const int rc = validate_stack(h, first_slot, stack, "pqp_bounds_set_occupancy_slots_device");
-    if (rc != PQP_OK) return rc;
-    pqp::DeviceGuard guard_(h->device);
-    return set_occupancy_slots(h, first_slot, stack, stack->cells, static_cast<cudaStream_t>(stream));
+    return occupancy(h, {first_slot, stack, false, 0, nullptr, false}, static_cast<cudaStream_t>(stream),
+                     "pqp_bounds_set_occupancy_slots_device");
 }
 
 int pqp_bounds_set_occupancy_slots(pqp_bounds_handle *h, int32_t first_slot, const pqp_occupancy_stack *stack) {
-    int rc = validate_stack(h, first_slot, stack, "pqp_bounds_set_occupancy_slots");
-    if (rc != PQP_OK) return rc;
-    pqp::DeviceGuard guard_(h->device);
-    // the images are consecutive in the slots' staging: count * rows * cols <= count * cap_cells bytes
-    uint8_t *staging = h->d_occ + (size_t)first_slot * h->cap_cells;
-    const size_t bytes = (size_t)stack->count * stack->rows * stack->cols;
-    PQP_CUDA(h->err, cudaMemcpyAsync(staging, stack->cells, bytes, cudaMemcpyHostToDevice, h->stream));
-    rc = set_occupancy_slots(h, first_slot, stack, staging, h->stream);
-    if (rc != PQP_OK) return rc;
-    PQP_CUDA(h->err, cudaStreamSynchronize(h->stream));
-    return PQP_OK;
+    return occupancy(h, {first_slot, stack, false, 0, nullptr, false}, std::nullopt, "pqp_bounds_set_occupancy_slots");
 }
 
 int pqp_bounds_set_occupancy_boxes_device(pqp_bounds_handle *h, int32_t first_slot, const pqp_occupancy_stack *base,
                                           int32_t shared_base, const pqp_obstacle_boxes *boxes, void *stream) {
-    const int rc = validate_boxes(h, first_slot, base, shared_base, boxes, false, "pqp_bounds_set_occupancy_boxes_device");
-    if (rc != PQP_OK) return rc;
-    pqp::DeviceGuard guard_(h->device);
-    return set_occupancy_boxes(h, first_slot, base, base->cells, shared_base, boxes->k, boxes->boxes, boxes->k_max,
-                               static_cast<cudaStream_t>(stream));
+    return occupancy(h, {first_slot, base, true, shared_base, boxes, false}, static_cast<cudaStream_t>(stream),
+                     "pqp_bounds_set_occupancy_boxes_device");
 }
 
 int pqp_bounds_set_occupancy_boxes(pqp_bounds_handle *h, int32_t first_slot, const pqp_occupancy_stack *base,
                                    int32_t shared_base, const pqp_obstacle_boxes *boxes) {
-    int rc = validate_boxes(h, first_slot, base, shared_base, boxes, true, "pqp_bounds_set_occupancy_boxes");
-    if (rc != PQP_OK) return rc;
-    pqp::DeviceGuard guard_(h->device);
-    // the base image(s) into the slots' staging, as set_occupancy_slots stages its stack; the boxes into theirs
-    uint8_t *staging = h->d_occ + (size_t)first_slot * h->cap_cells;
-    const size_t bytes = (size_t)(shared_base ? 1 : base->count) * base->rows * base->cols;
-    const size_t n_box = (size_t)base->count * boxes->k_max;
-    cudaStream_t s = h->stream;
-    PQP_CUDA(h->err, cudaMemcpyAsync(staging, base->cells, bytes, cudaMemcpyHostToDevice, s));
-    if (n_box) {
-        PQP_CUDA(h->err, cudaMemcpyAsync(h->d_box_k, boxes->k, base->count * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-        PQP_CUDA(h->err, cudaMemcpyAsync(h->d_boxes, boxes->boxes, n_box * PQP_BOX_FIELDS * sizeof(double),
-                                         cudaMemcpyHostToDevice, s));
-    }
-    rc = set_occupancy_boxes(h, first_slot, base, staging, shared_base, h->d_box_k, h->d_boxes, boxes->k_max, s);
-    if (rc != PQP_OK) return rc;
-    PQP_CUDA(h->err, cudaStreamSynchronize(s));
-    return PQP_OK;
+    return occupancy(h, {first_slot, base, true, shared_base, boxes, false}, std::nullopt,
+                     "pqp_bounds_set_occupancy_boxes");
 }
 
 int pqp_bounds_get_map(pqp_bounds_handle *h, pqp_bounds_map *meta, float *distance) {

@@ -142,6 +142,32 @@ cudaError_t peer_copy(T *dst, int dst_dev, const T *src, int src_dev, size_t cou
     return cudaMemcpyPeerAsync(dst, dst_dev, src, src_dev, count * sizeof(T), s);
 }
 
+// A device-form call on every device: `run(d, s)` enqueues device index d's part on stream s (a handle's refusal
+// through device_fail). The home part runs first, on the caller's stream, so its refusal enqueues nothing anywhere;
+// every other device with active(d) runs on its own stream between the fork and the caller's stream's join.
+template <typename Run, typename Active>
+int fork_join(pqp_plan_multi_t *m, cudaStream_t stream, Run &&run, Active &&active) {
+    const int home = m->dev[0];
+    {
+        pqp::DeviceGuard g(home);
+        PQP_CUDA(m->err, cudaEventRecord(m->fork, stream));
+    }
+    int rc = run(0, stream);
+    if (rc != PQP_OK) return rc;
+    for (int d = 1; d < m->n_dev; ++d) {
+        if (!active(d)) continue;
+        pqp::DeviceGuard g(m->dev[d]);
+        PQP_CUDA(m->err, cudaStreamWaitEvent(m->stream[d], m->fork, 0));
+        rc = run(d, m->stream[d]);
+        if (rc != PQP_OK) return rc;
+        PQP_CUDA(m->err, cudaEventRecord(m->done[d], m->stream[d]));
+    }
+    pqp::DeviceGuard g(home);
+    for (int d = 1; d < m->n_dev; ++d)
+        if (active(d)) PQP_CUDA(m->err, cudaStreamWaitEvent(stream, m->done[d], 0));
+    return PQP_OK;
+}
+
 int plan_device(pqp_plan_multi_t *m, const Call &c, const int32_t *map_index, const pqp_plan_out *out,
                 cudaStream_t stream) {
     int rc = validate(m, c, out);
@@ -152,23 +178,15 @@ int plan_device(pqp_plan_multi_t *m, const Call &c, const int32_t *map_index, co
                     "host form");
     const int G = m->n_dev, B = c.batch(), per = pqp::shard_per(B, G), home = m->dev[0];
     const size_t S = c.stride(), N = m->N;
-    {
-        pqp::DeviceGuard g(home);
-        PQP_CUDA(m->err, cudaEventRecord(m->fork, stream));
-    }
-    // the home shard [0, per) on the caller's buffers and stream; its refusal is every device's
-    rc = c.run(m->h[0], pqp::shard_of(B, per, 0).count, c.x(), c.y(), c.cnt(), c.start(), c.target(), map_index, out,
-               &stream);
-    if (rc != PQP_OK) return device_fail(m, 0, rc);
-    for (int d = 1; d < G; ++d) {
+    rc = fork_join(m, stream, [&](int d, cudaStream_t sd) -> int {
         const pqp::Shard sh = pqp::shard_of(B, per, d);
-        if (sh.count == 0) continue;
+        if (d == 0) {  // the home shard [0, per) on the caller's buffers
+            const int hrc = c.run(m->h[0], sh.count, c.x(), c.y(), c.cnt(), c.start(), c.target(), map_index, out, &sd);
+            return hrc == PQP_OK ? PQP_OK : device_fail(m, 0, hrc);
+        }
         const size_t lo = sh.first, n = sh.count;
         const int dv = m->dev[d];
         const Staging &s = m->st[d];
-        cudaStream_t sd = m->stream[d];
-        pqp::DeviceGuard g(dv);
-        PQP_CUDA(m->err, cudaStreamWaitEvent(sd, m->fork, 0));
         PQP_CUDA(m->err, peer_copy(s.x, dv, c.x() + lo * S, home, n * S, sd));
         PQP_CUDA(m->err, peer_copy(s.y, dv, c.y() + lo * S, home, n * S, sd));
         PQP_CUDA(m->err, peer_copy(s.cnt, dv, c.cnt() + lo, home, n, sd));
@@ -176,21 +194,71 @@ int plan_device(pqp_plan_multi_t *m, const Call &c, const int32_t *map_index, co
         PQP_CUDA(m->err, peer_copy(s.target, dv, c.target() + 3 * lo, home, 3 * n, sd));
         if (map_index) PQP_CUDA(m->err, peer_copy(s.map_index, dv, map_index + lo, home, n, sd));
         const pqp_plan_out o = {s.status, s.n, s.path, s.cost, s.iters, nullptr};
-        rc = c.run(m->h[d], sh.count, s.x, s.y, s.cnt, s.start, s.target, map_index ? s.map_index : nullptr, &o, &sd);
-        if (rc != PQP_OK) return device_fail(m, d, rc);
+        const int drc = c.run(m->h[d], sh.count, s.x, s.y, s.cnt, s.start, s.target, map_index ? s.map_index : nullptr,
+                              &o, &sd);
+        if (drc != PQP_OK) return device_fail(m, d, drc);
         PQP_CUDA(m->err, peer_copy(out->status + lo, home, s.status, dv, n, sd));
         PQP_CUDA(m->err, peer_copy(out->n + lo, home, s.n, dv, n, sd));
         PQP_CUDA(m->err, peer_copy(out->path + lo * PQP_PLAN_PATH_ROWS * N, home, s.path, dv, n * PQP_PLAN_PATH_ROWS * N, sd));
         PQP_CUDA(m->err, peer_copy(out->cost + lo, home, s.cost, dv, n, sd));
         PQP_CUDA(m->err, peer_copy(out->iters + 2 * lo, home, s.iters, dv, 2 * n, sd));
-        PQP_CUDA(m->err, cudaEventRecord(m->done[d], sd));
-    }
-    pqp::DeviceGuard g(home);
-    for (int d = 1; d < G; ++d)
-        if (pqp::shard_of(B, per, d).count > 0) PQP_CUDA(m->err, cudaStreamWaitEvent(stream, m->done[d], 0));
+        return PQP_OK;
+    }, [&](int d) { return pqp::shard_of(B, per, d).count > 0; });
+    if (rc != PQP_OK) return rc;
     m->last_batch = B;
     m->last_per = per;
     return PQP_OK;
+}
+
+// A device-form occupancy update of slots first .. first + count - 1: pqp_plan_set_occupancy_boxes_device when
+// `boxed`, else pqp_plan_set_occupancy_slots_device.
+struct Occupancy {
+    int first;
+    const pqp_occupancy_stack *stack;
+    bool boxed;
+    int shared_base;
+    const pqp_obstacle_boxes *boxes;
+};
+
+// An update the home handle accepted, peer-copied on sd into device index d's staging: the image(s), and k and the
+// boxes when there are any. `r` becomes the update that reads them there, through `stack` and `boxes`.
+int stage(pqp_plan_multi_t *m, int d, cudaStream_t sd, Occupancy &r, pqp_occupancy_stack &stack,
+          pqp_obstacle_boxes &boxes) {
+    const int dv = m->dev[d], home = m->dev[0];
+    const Staging &st = m->st[d];
+    stack = *r.stack;
+    boxes = r.boxed ? *r.boxes : pqp_obstacle_boxes{};
+    const size_t bytes = (size_t)(r.shared_base ? 1 : stack.count) * stack.rows * stack.cols;
+    const size_t n_box = (size_t)stack.count * boxes.k_max;
+    PQP_CUDA(m->err, peer_copy(st.occ, dv, stack.cells, home, bytes, sd));
+    if (n_box) {
+        PQP_CUDA(m->err, peer_copy(st.box_k, dv, boxes.k, home, (size_t)stack.count, sd));
+        PQP_CUDA(m->err, peer_copy(st.boxes, dv, boxes.boxes, home, n_box * PQP_BOX_FIELDS, sd));
+        boxes.k = st.box_k;
+        boxes.boxes = st.boxes;
+    }
+    stack.cells = st.occ;
+    r.stack = &stack;
+    if (r.boxed) r.boxes = &boxes;
+    return PQP_OK;
+}
+
+// the occupancy update on every device: once the caller's stream has passed it, every device's slots are final, as the
+// single-device call's are, whichever stream (a host form's included) reads them next
+int occupancy_device(pqp_plan_multi_t *m, const Occupancy &r, cudaStream_t stream) {
+    if (!m) return PQP_E_INVALID;
+    return fork_join(m, stream, [&](int d, cudaStream_t sd) -> int {
+        Occupancy u = r;
+        pqp_occupancy_stack stack;
+        pqp_obstacle_boxes boxes;
+        if (d > 0) {
+            const int rc = stage(m, d, sd, u, stack, boxes);
+            if (rc != PQP_OK) return rc;
+        }
+        const int rc = u.boxed ? pqp_plan_set_occupancy_boxes_device(m->h[d], u.first, u.stack, u.shared_base, u.boxes, sd)
+                               : pqp_plan_set_occupancy_slots_device(m->h[d], u.first, u.stack, sd);
+        return rc == PQP_OK ? PQP_OK : device_fail(m, d, rc);
+    }, [](int) { return true; });
 }
 
 // a host-form update of every device's handle, concurrently
@@ -347,34 +415,7 @@ int pqp_plan_multi_set_occupancy_slots(pqp_plan_multi_t *m, int32_t first_slot, 
 
 int pqp_plan_multi_set_occupancy_slots_device(pqp_plan_multi_t *m, int32_t first_slot, const pqp_occupancy_stack *stack,
                                               void *stream) {
-    if (!m) return PQP_E_INVALID;
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    const int home = m->dev[0];
-    {
-        pqp::DeviceGuard g(home);
-        PQP_CUDA(m->err, cudaEventRecord(m->fork, s));
-    }
-    // the home handle first: its refusal is every device's
-    int rc = pqp_plan_set_occupancy_slots_device(m->h[0], first_slot, stack, stream);
-    if (rc != PQP_OK) return device_fail(m, 0, rc);
-    const size_t bytes = (size_t)stack->count * stack->rows * stack->cols;
-    for (int d = 1; d < m->n_dev; ++d) {
-        const int dv = m->dev[d];
-        cudaStream_t sd = m->stream[d];
-        pqp::DeviceGuard g(dv);
-        PQP_CUDA(m->err, cudaStreamWaitEvent(sd, m->fork, 0));
-        PQP_CUDA(m->err, peer_copy(m->st[d].occ, dv, stack->cells, home, bytes, sd));
-        pqp_occupancy_stack local = *stack;
-        local.cells = m->st[d].occ;
-        rc = pqp_plan_set_occupancy_slots_device(m->h[d], first_slot, &local, sd);
-        if (rc != PQP_OK) return device_fail(m, d, rc);
-        // after the transform: once the caller's stream has passed the update, every device's slots are final, as the
-        // single-device call's are, whichever stream (a host form's included) reads them next
-        PQP_CUDA(m->err, cudaEventRecord(m->done[d], sd));
-    }
-    pqp::DeviceGuard g(home);
-    for (int d = 1; d < m->n_dev; ++d) PQP_CUDA(m->err, cudaStreamWaitEvent(s, m->done[d], 0));
-    return PQP_OK;
+    return occupancy_device(m, {first_slot, stack, false, 0, nullptr}, static_cast<cudaStream_t>(stream));
 }
 
 int pqp_plan_multi_set_occupancy_boxes(pqp_plan_multi_t *m, int32_t first_slot, const pqp_occupancy_stack *base,
@@ -387,41 +428,7 @@ int pqp_plan_multi_set_occupancy_boxes(pqp_plan_multi_t *m, int32_t first_slot, 
 
 int pqp_plan_multi_set_occupancy_boxes_device(pqp_plan_multi_t *m, int32_t first_slot, const pqp_occupancy_stack *base,
                                               int32_t shared_base, const pqp_obstacle_boxes *boxes, void *stream) {
-    if (!m) return PQP_E_INVALID;
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    const int home = m->dev[0];
-    {
-        pqp::DeviceGuard g(home);
-        PQP_CUDA(m->err, cudaEventRecord(m->fork, s));
-    }
-    // the home handle first: its refusal is every device's
-    int rc = pqp_plan_set_occupancy_boxes_device(m->h[0], first_slot, base, shared_base, boxes, stream);
-    if (rc != PQP_OK) return device_fail(m, 0, rc);
-    const size_t bytes = (size_t)(shared_base ? 1 : base->count) * base->rows * base->cols;
-    const size_t n_box = (size_t)base->count * boxes->k_max;
-    for (int d = 1; d < m->n_dev; ++d) {
-        const int dv = m->dev[d];
-        const Staging &st = m->st[d];
-        cudaStream_t sd = m->stream[d];
-        pqp::DeviceGuard g(dv);
-        PQP_CUDA(m->err, cudaStreamWaitEvent(sd, m->fork, 0));
-        PQP_CUDA(m->err, peer_copy(st.occ, dv, base->cells, home, bytes, sd));
-        pqp_occupancy_stack local = *base;
-        local.cells = st.occ;
-        pqp_obstacle_boxes lb = *boxes;
-        if (n_box) {
-            PQP_CUDA(m->err, peer_copy(st.box_k, dv, boxes->k, home, (size_t)base->count, sd));
-            PQP_CUDA(m->err, peer_copy(st.boxes, dv, boxes->boxes, home, n_box * PQP_BOX_FIELDS, sd));
-            lb.k = st.box_k;
-            lb.boxes = st.boxes;
-        }
-        rc = pqp_plan_set_occupancy_boxes_device(m->h[d], first_slot, &local, shared_base, &lb, sd);
-        if (rc != PQP_OK) return device_fail(m, d, rc);
-        PQP_CUDA(m->err, cudaEventRecord(m->done[d], sd));  // as set_occupancy_slots_device: the slots are final
-    }
-    pqp::DeviceGuard g(home);
-    for (int d = 1; d < m->n_dev; ++d) PQP_CUDA(m->err, cudaStreamWaitEvent(s, m->done[d], 0));
-    return PQP_OK;
+    return occupancy_device(m, {first_slot, base, true, shared_base, boxes}, static_cast<cudaStream_t>(stream));
 }
 
 int pqp_plan_multi_get_map_slot(pqp_plan_multi_t *m, int32_t device_index, int32_t slot, pqp_bounds_map *meta,

@@ -119,26 +119,13 @@ def _lib():
         L.pqp_plan_launch_count.argtypes = [vp, C.POINTER(C.c_int64)]
         L.pqp_plan_last_error.argtypes = [vp]
         L.pqp_plan_last_error.restype = C.c_char_p
-        L.pqp_plan_set_map.argtypes = [vp, C.POINTER(bounds.BoundsMap)]
-        L.pqp_plan_set_map_device.argtypes = [vp, C.POINTER(bounds.BoundsMap), vp]
-        L.pqp_plan_set_occupancy.argtypes = [vp, C.POINTER(bounds.OccupancyMap)]
-        L.pqp_plan_set_occupancy_device.argtypes = [vp, C.POINTER(bounds.OccupancyMap), vp]
-        L.pqp_plan_get_map.argtypes = [vp, C.POINTER(bounds.BoundsMap), vp]
         L.pqp_plan_create_maps.argtypes = [C.POINTER(bounds.BoundsMap), C.c_int32, C.POINTER(PlanParams)] + \
             [C.c_int32] * 6 + [C.POINTER(vp)]
         L.pqp_plan_mapped.argtypes = [vp, C.POINTER(PlanIn), vp, C.POINTER(PlanOut)]
         L.pqp_plan_mapped_device.argtypes = [vp, C.POINTER(PlanIn), vp, C.POINTER(PlanOut), vp]
         L.pqp_plan_points_mapped.argtypes = [vp, C.POINTER(PlanPointsIn), vp, C.POINTER(PlanOut)]
         L.pqp_plan_points_mapped_device.argtypes = [vp, C.POINTER(PlanPointsIn), vp, C.POINTER(PlanOut), vp]
-        L.pqp_plan_set_map_slot.argtypes = [vp, C.c_int32, C.POINTER(bounds.BoundsMap)]
-        L.pqp_plan_set_map_slot_device.argtypes = [vp, C.c_int32, C.POINTER(bounds.BoundsMap), vp]
-        L.pqp_plan_set_occupancy_slots.argtypes = [vp, C.c_int32, C.POINTER(bounds.OccupancyStack)]
-        L.pqp_plan_set_occupancy_slots_device.argtypes = [vp, C.c_int32, C.POINTER(bounds.OccupancyStack), vp]
-        L.pqp_plan_get_map_slot.argtypes = [vp, C.c_int32, C.POINTER(bounds.BoundsMap), vp]
-        L.pqp_plan_map_count.argtypes = [vp]
-        L.pqp_plan_map_count.restype = C.c_int32
-        bounds.declare_collision(L, "pqp_plan_")
-        bounds.declare_boxes(L, "pqp_plan_")
+        bounds.declare_map_surface(L, "pqp_plan_")
         L._plan_declared = True
     return L
 
@@ -302,21 +289,10 @@ class Planner(bounds.MapSlots):
             self._check(mapped_fn(self.h, C.byref(pin), map_index.data_ptr(), C.byref(pout), s))
         return out
 
-    def set_occupancy_slots_device(self, imgs, resolution, centers=None, obstacle_max=0, *, first_slot=0,
-                                   stream=None):
-        """As `set_occupancy_slots` from a torch uint8 CUDA tensor [count, rows, cols], asynchronous on `stream`
-        (default: the current stream): plans enqueued before see the old slots, plans enqueued after the new ones. The
-        tensor must stay alive until the stream has run the transform."""
-        super().set_occupancy_slots_device(imgs, resolution, centers, obstacle_max, first_slot=first_slot,
-                                           stream=_stream(stream, imgs.device))
-
-    def set_occupancy_boxes_device(self, base, resolution, boxes, k, centers=None, obstacle_max=0, *, first_slot=0,
-                                   stream=None):
-        """As `set_occupancy_boxes` from torch CUDA tensors (`bounds.MapSlots.set_occupancy_boxes_device`),
-        asynchronous on `stream` (default: the current stream): plans enqueued before see the old slots, plans enqueued
-        after the new ones."""
-        super().set_occupancy_boxes_device(base, resolution, boxes, k, centers, obstacle_max, first_slot=first_slot,
-                                           stream=_stream(stream, base.device))
+    def _raw_stream(self, stream, device):
+        """A torch stream's cudaStream_t (None: the current stream of `device`): plans enqueued on it before a
+        device-form map update see the old slots, plans enqueued after the new ones."""
+        return _stream(stream, device)
 
     def set_map_device(self, dist, resolution, center=(0.0, 0.0), *, stream=None):
         """As `set_map` from a torch float32 CUDA tensor [rows, cols], asynchronous on `stream` (default: the

@@ -32,9 +32,7 @@ def _lib():
         L.pqp_plan_multi_points_device.argtypes = [vp, ppts, vp, pout, vp]
         L.pqp_plan_multi_device.argtypes = [vp, pin, vp, pout, vp]
         L.pqp_plan_multi_set_map_slot.argtypes = [vp, i32, C.POINTER(bounds.BoundsMap)]
-        L.pqp_plan_multi_set_occupancy_slots.argtypes = [vp, i32, C.POINTER(bounds.OccupancyStack)]
-        L.pqp_plan_multi_set_occupancy_slots_device.argtypes = [vp, i32, C.POINTER(bounds.OccupancyStack), vp]
-        bounds.declare_boxes(L, "pqp_plan_multi_")
+        bounds.declare_stack_updates(L, "pqp_plan_multi_")
         L.pqp_plan_multi_get_map_slot.argtypes = [vp, i32, i32, C.POINTER(bounds.BoundsMap), vp]
         L.pqp_plan_multi_shard.argtypes = [vp, i32, C.POINTER(i32), C.POINTER(i32)]
         L.pqp_plan_multi_handle.argtypes = [vp, i32, C.POINTER(vp)]
@@ -117,35 +115,31 @@ class MultiPlanner:
 
     def set_occupancy_slots(self, imgs, resolution, centers=None, obstacle_max=0, *, first_slot=0):
         """As `plan.Planner.set_occupancy_slots` on every device, the transforms concurrently (host, synchronous)."""
-        imgs = np.ascontiguousarray(imgs, dtype=np.uint8)
-        assert imgs.ndim == 3
-        st, _keep = bounds.occupancy_stack(imgs.ctypes.data, imgs.shape, resolution, centers, obstacle_max)
-        self._check(self.L.pqp_plan_multi_set_occupancy_slots(self.h, int(first_slot), C.byref(st)))
+        self._check(bounds.occupancy_call(self.L.pqp_plan_multi_set_occupancy_slots, self.h, imgs, resolution, centers,
+                                          obstacle_max, first_slot))
 
     def set_occupancy_slots_device(self, imgs, resolution, centers=None, obstacle_max=0, *, first_slot=0, stream=None):
         """As `set_occupancy_slots` from a torch uint8 tensor [count, rows, cols] on the home device, ordered on `stream`
         (default: the current stream of the home device): the images are peer-copied to every other device and
         transformed there. Plans enqueued before see the old slots on every device, plans enqueued after the new ones;
         the tensor may be released once `stream` has passed the call."""
-        import torch
-        assert imgs.is_cuda and imgs.is_contiguous() and imgs.dtype == torch.uint8 and imgs.dim() == 3
-        st, _keep = bounds.occupancy_stack(imgs.data_ptr(), imgs.shape, resolution, centers, obstacle_max)
-        s = C.c_void_p(_plan._stream(stream, imgs.device))
-        self._check(self.L.pqp_plan_multi_set_occupancy_slots_device(self.h, int(first_slot), C.byref(st), s))
+        self._check(bounds.occupancy_call_device(self.L.pqp_plan_multi_set_occupancy_slots_device, self.h, imgs,
+                                                 resolution, centers, obstacle_max, first_slot,
+                                                 stream=_plan._stream(stream, imgs.device)))
 
     def set_occupancy_boxes(self, base, resolution, boxes, k=None, centers=None, obstacle_max=0, *, first_slot=0):
         """As `plan.Planner.set_occupancy_boxes` on every device, the updates concurrently (host, synchronous)."""
-        self._check(bounds.boxes_call(self.L.pqp_plan_multi_set_occupancy_boxes, self.h, base, resolution, boxes, k,
-                                      centers, obstacle_max, first_slot))
+        self._check(bounds.occupancy_call(self.L.pqp_plan_multi_set_occupancy_boxes, self.h, base, resolution, centers,
+                                          obstacle_max, first_slot, boxes, k))
 
     def set_occupancy_boxes_device(self, base, resolution, boxes, k, centers=None, obstacle_max=0, *, first_slot=0,
                                    stream=None):
         """As `plan.Planner.set_occupancy_boxes_device` from tensors on the home device, ordered on `stream` (default:
         the current stream of the home device): the base image(s), k and the boxes are peer-copied to every other
         device and stamped there, as `set_occupancy_slots_device` does with its images."""
-        s = _plan._stream(stream, base.device)
-        self._check(bounds.boxes_call_device(self.L.pqp_plan_multi_set_occupancy_boxes_device, self.h, base,
-                                             resolution, boxes, k, centers, obstacle_max, first_slot, s))
+        self._check(bounds.occupancy_call_device(self.L.pqp_plan_multi_set_occupancy_boxes_device, self.h, base,
+                                                 resolution, centers, obstacle_max, first_slot, boxes, k,
+                                                 stream=_plan._stream(stream, base.device)))
 
     def get_map_slot(self, device_index, slot=0):
         """-> (float32 distance layer, resolution, (center_x, center_y)) of `slot` on device index `device_index`."""
